@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py — the headline measurement of the PGCN hot path on B200 (see DESIGN.md §Measurement).
+"""bench.py — the headline measurement of the PGCN hot path on the H100 (see DESIGN.md §Measurement).
 
     python bench.py --gpus N --steps K --warmup W            (N > 1: launched by torch.distributed.run)
     python bench.py --impl reference --gpus N --steps K --warmup W
+    python bench.py ... --dump-outputs DIR       (also writes what the last timed step computed, see dump_outputs)
 
 metric  : aggregated edges/s of ONE layer's forward aggregation (PSpMM.forward = halo exchange +
           Z = A_local * H), whole job, = nnz(A^) / max-over-ranks time per step   (BASELINE.json metric)
@@ -16,7 +17,7 @@ value   : device-resident inputs, CUDA-event timed, K steps after W warm-ups, ma
 e2e     : the same step through the C-ABI host entry point pgcn_forward_host — H in pinned HOST
           memory, copied in, aggregated, Z copied back, every step.
 roofline: the SpMM kernel — algorithmic bytes (SURVEY.md §8d) / CUDA-event time per launch vs the
-          measured HBM copy bandwidth in MEASURED_PEAKS.json.
+          measured HBM copy bandwidth in MEASURED_PEAKS.json, else the H100 SXM data-sheet 3.35 TB/s.
 cpu_baseline / --impl reference: the C/OpenMP restatement of the reference's GraphBLAS aggregation
           (oracle/spmm_oracle.c, Parallel-GCN/main.c:271,295) on the host cores — the real GraphBLAS
           trainer cannot be built offline (no GraphBLAS.h / mpicc), see DESIGN.md.
@@ -27,6 +28,7 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -48,12 +50,14 @@ def parse():
     ap.add_argument("--config", default=None, help="C2 | C3 | C4 | C5 (default: C2 on one GPU, C5 on several)")
     ap.add_argument("--partition", default="auto", help="auto | block | rp | path to a part vector")
     ap.add_argument("--transport", default="auto", choices=["auto", "nccl", "p2p"])
-    ap.add_argument("--cache", default=os.environ.get("PGCN_CACHE", "/tmp/pgcn_b200_cache"))
+    ap.add_argument("--cache", default=os.environ.get("PGCN_CACHE", os.path.join(tempfile.gettempdir(), "pgcn_b200_cache")))
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-lib-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true", help="skip the host-buffer (e2e) measurement (side runs only)")
     ap.add_argument("--no-single", action="store_true", help="N > 1: skip the single-GPU run of the same config")
     ap.add_argument("--opt", action="append", default=[], help="plan option name=value (tuning)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write a fixed sample of the last timed step's output Z to DIR/*.npy (run-to-run comparable)")
     args = ap.parse_args()
     if args.config is None:
         args.config = "C2" if args.gpus <= 1 else "C5"
@@ -86,11 +90,11 @@ def peaks():
             return float(json.load(open(path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3; not measured)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -135,6 +139,25 @@ class ClockSampler:
                     reasons.add(name)
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
                 "reasons": sorted(reasons), "samples": len(sm)}
+
+
+# bytes of Z written by --dump-outputs, over all ranks (the row sample is what stays below it)
+DUMP_BYTES = 32 << 20
+
+
+def dump_outputs(out_dir, Z, rank, world):
+    """Z (this rank's owned rows) of the last timed step: the same seeded sample of rows every run, in float32, plus
+    the sampled row ids (local to the rank) in float64. The inputs (graph, part vector, H) are seeded too, so two
+    builds run with the same arguments can be compared output for output."""
+    m, f = Z.shape
+    nrows = min(m, max(1, DUMP_BYTES // world // (4 * max(f, 1))))
+    rows = np.sort(np.random.RandomState(12345 + rank).choice(m, size=nrows, replace=False)) if m else np.zeros(0, np.int64)
+    import torch
+    sample = Z[torch.from_numpy(rows).to(Z.device)].cpu().numpy().astype(np.float32)
+    os.makedirs(out_dir, exist_ok=True)
+    tag = "" if world == 1 else "_rank%d" % rank
+    np.save(os.path.join(out_dir, "Z%s.npy" % tag), sample)
+    np.save(os.path.join(out_dir, "Z_rows%s.npy" % tag), rows.astype(np.float64))
 
 
 def load_graph(args):
@@ -295,7 +318,7 @@ def main():
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a CUDA device: the PGCN B200 path has no CPU fallback")
+        raise SystemExit("bench.py needs a CUDA device: the PGCN GPU path has no CPU fallback")
     torch.cuda.set_device(local_rank)
     device = torch.device("cuda", local_rank)
     if world > 1:
@@ -356,6 +379,8 @@ def main():
     launches = plan.launch_count() - l0
     ms = e0.elapsed_time(e1) / args.steps
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, Z, rank, world)
 
     # ---- the dominant kernel alone (local SpMM over [own | halo]) -----------------------------
     halo = torch.zeros((max(lp.h, 1), f), device=device)
@@ -482,7 +507,7 @@ def main():
             },
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                          "traffic": None,
-                         "kernel": ("spmm_ring_g4_kernel (TMA tile::gather4 into per-warp shared-memory row rings)"
+                         "kernel": ("spmm_ring_tm_kernel (2-D tensor-map TMA into per-warp shared-memory row rings)"
                                     if f % 128 == 0 else "spmm_rowblock_kernel (register pipeline)"),
                          "ms_per_launch": ms_kernel,
                          "algorithmic_bytes_per_launch": bytes_per_rank, "peak_source": peak_src},

@@ -1,5 +1,5 @@
 /*
- * pgcn_b200.h — C-ABI of the B200-native PGCN aggregation path.
+ * pgcn_b200.h — C-ABI of the H100-native PGCN aggregation path.
  *
  * This is the drop-in boundary for ONE hot path of the reference
  * (gunduzvd/Scalable-Graph-Convolutional-Network-Training-on-Distributed-Memory-Systems):
@@ -61,7 +61,7 @@ typedef struct pgcn_bytes {
 
 /* ---- library-level ---------------------------------------------------------------------- */
 
-/* Version / build string, e.g. "pgcn_b200 0.1 sm_100a". Never NULL. */
+/* Version / build string, e.g. "pgcn_b200 0.1 sm_90a". Never NULL. */
 const char* pgcn_version(void);
 
 /* Number of visible CUDA devices, or a negative pgcn_status. */
@@ -97,9 +97,9 @@ int pgcn_plan_destroy(pgcn_plan* plan);
 /*
  * Plan options (take effect at the next compute call). Names:
  *   "kernel"               0 = automatic (default): widths that are multiples of 128 floats with 16-byte aligned
- *                          operands take the shared-memory ring kernel fed by TMA tile::gather4, everything else the
+ *                          operands take the shared-memory ring kernel fed by 2-D tensor-map TMA, everything else the
  *                          register-pipeline kernel; 4 = always the register kernel; 5 / 6 / 7 = ring kernel fed by
- *                          1-D cp.async.bulk / cp.async / tile::gather4
+ *                          1-D cp.async.bulk / cp.async / 2-D tensor-map TMA (one row per copy)
  *   "ring_slots"           row slots per warp of the ring kernel: 16 (default), 32, 64; "ring_groups" 2 | 4 (64 slots)
  *   "ring_edges_per_block" target nnz of one row block = one warp's unit of work          (default 512)
  *   "ring_long_row"        rows with more nnz than this are split into segments           (default 2 * block)

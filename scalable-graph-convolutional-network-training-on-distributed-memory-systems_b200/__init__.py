@@ -1,4 +1,4 @@
-"""pgcn_b200 — B200-native drop-in for the PGCN aggregation hot path
+"""pgcn_b200 — H100-native drop-in for the PGCN aggregation hot path
 (Z = A_local * H + halo exchange; reference GPU/PGCN.py:85-134).
 
 Importable as `pgcn_b200` through the shim at the repo root (the directory name contains

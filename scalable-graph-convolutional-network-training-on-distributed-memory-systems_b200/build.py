@@ -1,6 +1,6 @@
 """Build the native pieces in-tree (so the .so files travel to the GPU box with the snapshot).
 
-  lib/libpgcn_b200.so   csrc/pgcn_b200.cu (+ spmm_kernels.cuh, spmm_ring.cuh)   nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo
+  lib/libpgcn_b200.so   csrc/pgcn_b200.cu (+ spmm_kernels.cuh, spmm_ring.cuh)   nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo
   (the CPU oracle under oracle/ is built by oracle/build_oracle.py — test infrastructure only)
 
 nvcc cross-compiles without a GPU; `python -m <pkg>.build` or `__graft_entry__.build()` runs this.
@@ -19,11 +19,12 @@ LIBDIR = os.path.join(HERE, "lib")
 _VARIANT = os.environ.get("PGCN_B200_VARIANT", "")
 LIB = os.path.join(LIBDIR, "libpgcn_b200%s.so" % ("_" + _VARIANT if _VARIANT else ""))
 SOURCES = [os.path.join(CSRC, "pgcn_b200.cu")]
+# this file too: a library built with other compiler flags (another GPU architecture) is stale
 DEPS = SOURCES + [os.path.join(CSRC, "spmm_kernels.cuh"), os.path.join(CSRC, "spmm_ring.cuh"),
-                  os.path.join(ROOT, "include", "pgcn_b200.h")]
+                  os.path.join(ROOT, "include", "pgcn_b200.h"), os.path.abspath(__file__)]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",
 ]
@@ -44,7 +45,7 @@ def is_stale():
 
 
 def build(force=False, verbose=False):
-    """Compile libpgcn_b200.so for sm_100a if missing or older than its sources. Returns its path."""
+    """Compile libpgcn_b200.so for sm_90a if missing or older than its sources. Returns its path."""
     if not force and not is_stale():
         return LIB
     nvcc = _nvcc()

@@ -139,17 +139,17 @@ struct pgcn_plan {
     float* d_hsend_slab = nullptr;   // h x f_max   (reverse send: halo partials of A^T g)
 
     // options
-    int64_t opt_epb = 128, opt_long = 0, opt_tile = 0, opt_overlap = 1, opt_hot_mb = 64;
+    int64_t opt_epb = 128, opt_long = 0, opt_tile = 0, opt_overlap = 1, opt_hot_mb = 24;
     int64_t opt_relu = 0;            // fused layer epilogue of pgcn_forward: Z = max(0, A_local * H)
     // kernel: 0 auto (ring with TMA bulk copies where it applies), 4 register pipeline, 5 ring/1-D TMA,
-    //         6 ring/cp.async, 7 ring/TMA tile::gather4 (= auto)
+    //         6 ring/cp.async, 7 ring/2-D tensor-map TMA (= auto)
     int64_t opt_ring_groups = 2;
     int64_t opt_persistent_multi = 0;
     int64_t opt_kernel = 0, opt_ring_slots = 16, opt_ring_epb = 512, opt_ring_long = 0, opt_persistent = 1;
     bool ring_attr_set[48] = {false};
     int ring_ctas_per_sm[48] = {0};
     unsigned int* d_counter = nullptr;     // block counters of the persistent ring kernel (one per feature tile)
-    int num_sms = 148;
+    int num_sms = 132;
 
     // NCCL
     ncclComm_t comm = nullptr;
@@ -407,7 +407,7 @@ spmm_fn pick_lpe(int lpe, int vpl, bool halo)
 }
 
 typedef void (*ring_fn)(const SpmmArgs, const RingArgs);
-typedef void (*ring_g4_fn)(const SpmmArgs, const RingArgs, const CUtensorMap, const CUtensorMap);
+typedef void (*ring_tm_fn)(const SpmmArgs, const RingArgs, const CUtensorMap, const CUtensorMap);
 
 // cuTensorMapEncodeTiled, resolved through the runtime (no link-time dependency on libcuda)
 typedef CUresult (*encode_tiled_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -431,7 +431,7 @@ encode_tiled_fn encode_tiled()
     return g_encode_tiled;
 }
 
-// Tensor map of a row-major fp32 matrix [rows, f] for tile::gather4 loads of `tile` floats per row.
+// Tensor map of a row-major fp32 matrix [rows, f] for tile loads of `tile` floats of `box_rows` rows.
 bool make_row_map(CUtensorMap* tm, const float* base, int64_t rows, int f, int tile, int box_rows)
 {
     encode_tiled_fn enc = encode_tiled();
@@ -461,19 +461,19 @@ ring_fn pick_ring(int vpl, int shape, int mode, bool halo)
     return halo ? pick_ring_t<1, true>(shape, mode) : pick_ring_t<1, false>(shape, mode);
 }
 template <int VPL, bool HALO>
-ring_g4_fn pick_ring_g4_t(int shape)
+ring_tm_fn pick_ring_tm_t(int shape)
 {
     switch (shape) {
-        case 1: return spmm_ring_g4_kernel<VPL, 16, 2, HALO>;
-        case 2: return spmm_ring_g4_kernel<VPL, 32, 2, HALO>;
-        case 3: return spmm_ring_g4_kernel<VPL, 16, 4, HALO>;
-        default: return spmm_ring_g4_kernel<VPL, 8, 2, HALO>;
+        case 1: return spmm_ring_tm_kernel<VPL, 16, 2, HALO>;
+        case 2: return spmm_ring_tm_kernel<VPL, 32, 2, HALO>;
+        case 3: return spmm_ring_tm_kernel<VPL, 16, 4, HALO>;
+        default: return spmm_ring_tm_kernel<VPL, 8, 2, HALO>;
     }
 }
-ring_g4_fn pick_ring_g4(int vpl, int shape, bool halo)
+ring_tm_fn pick_ring_tm(int vpl, int shape, bool halo)
 {
-    if (vpl == 2) return halo ? pick_ring_g4_t<2, true>(shape) : pick_ring_g4_t<2, false>(shape);
-    return halo ? pick_ring_g4_t<1, true>(shape) : pick_ring_g4_t<1, false>(shape);
+    if (vpl == 2) return halo ? pick_ring_tm_t<2, true>(shape) : pick_ring_tm_t<2, false>(shape);
+    return halo ? pick_ring_tm_t<1, true>(shape) : pick_ring_tm_t<1, false>(shape);
 }
 
 // CUDA loads kernels lazily, at their first launch, and that load synchronises with the device. A rank whose
@@ -493,7 +493,7 @@ void preload_kernels()
             for (int vpl = 1; vpl <= 4; vpl *= 2) { touch_kernel(pick_lpe<4>(lpe, vpl, halo != 0)); touch_kernel(pick_lpe<1>(lpe, vpl, halo != 0)); }
     for (int vpl = 1; vpl <= 2; ++vpl)
         for (int halo = 0; halo < 2; ++halo) {
-            for (int shape = 0; shape < 4; ++shape) touch_kernel(pick_ring_g4(vpl, shape, halo != 0));
+            for (int shape = 0; shape < 4; ++shape) touch_kernel(pick_ring_tm(vpl, shape, halo != 0));
             for (int shape = 0; shape < 2; ++shape) touch_kernel(pick_ring(vpl, shape, 0, halo != 0));
             touch_kernel(pick_ring(vpl, 0, 1, halo != 0));
         }
@@ -552,7 +552,7 @@ int launch_spmm(pgcn_plan* p, DevCsr& c, const float* H0, const float* H1, int s
         const int vpl = (f % 256 == 0) ? 2 : 1;
         const int tiles = f / (128 * vpl);
         const bool halo = (H1 != nullptr);
-        int mode = p->opt_kernel == 6 ? 1 : (p->opt_kernel == 5 ? 0 : 2);   // default: tile::gather4
+        int mode = p->opt_kernel == 6 ? 1 : (p->opt_kernel == 5 ? 0 : 2);   // default: 2-D tensor-map TMA
         // ring shape from the options: ring_slots = 16 | 32 | 64, ring_groups = 2 | 4 (only with 64 slots)
         const int64_t want_slots = c.tuned_slots > 0 ? c.tuned_slots : p->opt_ring_slots;
         int shape = want_slots <= 16 ? 0 : (want_slots <= 32 ? 1 : (p->opt_ring_groups == 4 ? 3 : 2));
@@ -569,8 +569,8 @@ int launch_spmm(pgcn_plan* p, DevCsr& c, const float* H0, const float* H1, int s
         if (mode == 0 && shape > 1) shape = 1;
         const int g = kRingShapes[shape].g, ng = kRingShapes[shape].ng;
         ring_fn fn = mode == 2 ? nullptr : pick_ring(vpl, shape, mode, halo);
-        ring_g4_fn fn4 = mode == 2 ? pick_ring_g4(vpl, shape, halo) : nullptr;
-        const void* fptr = mode == 2 ? (const void*)fn4 : (const void*)fn;
+        ring_tm_fn fn_tm = mode == 2 ? pick_ring_tm(vpl, shape, halo) : nullptr;
+        const void* fptr = mode == 2 ? (const void*)fn_tm : (const void*)fn;
         const size_t smem = ring_smem_bytes(vpl, g * ng, ng);
         // opt-in to > 48 KB of dynamic shared memory, once per kernel instance
         const int slot = (((vpl - 1) * 4 + shape) * 3 + mode) * 2 + (halo ? 1 : 0);
@@ -595,7 +595,7 @@ int launch_spmm(pgcn_plan* p, DevCsr& c, const float* H0, const float* H1, int s
             ra.counter = p->d_counter;
             grid.x = std::min<unsigned>(grid.x, (unsigned)(p->num_sms * p->ring_ctas_per_sm[slot]));
         }
-        if (mode == 2) fn4<<<grid, kRingWarps * 32, smem, st>>>(a, ra, tm0, tm1);
+        if (mode == 2) fn_tm<<<grid, kRingWarps * 32, smem, st>>>(a, ra, tm0, tm1);
         else fn<<<grid, kRingWarps * 32, smem, st>>>(a, ra);
         ++p->launches;
     } else if (sc.nblocks > 0) {
@@ -628,10 +628,10 @@ int check_f(pgcn_plan* p, int f)
     return 0;
 }
 
-unsigned grid_for(long long total)
+unsigned grid_for(long long total, int num_sms)
 {
     long long g = (total + 255) / 256;
-    return (unsigned)std::max<long long>(1, std::min<long long>(g, 148LL * 32));
+    return (unsigned)std::max<long long>(1, std::min<long long>(g, 32LL * num_sms));
 }
 
 int launch_pack(pgcn_plan* p, const float* H, float* slab, int f, cudaStream_t st)
@@ -640,7 +640,7 @@ int launch_pack(pgcn_plan* p, const float* H, float* slab, int f, cudaStream_t s
     PackArgs a;
     a.send_idx = p->d_send_idx; a.S = p->S; a.H = H; a.slab = slab; a.f = f;
     const int vw = (f % 4 == 0) ? 4 : 1;
-    const unsigned grid = grid_for(p->S * (f / vw));
+    const unsigned grid = grid_for(p->S * (f / vw), p->num_sms);
     if (vw == 4) pack_rows_kernel<4><<<grid, 256, 0, st>>>(a);
     else pack_rows_kernel<1><<<grid, 256, 0, st>>>(a);
     ++p->launches;
@@ -731,7 +731,7 @@ int p2p_wait(pgcn_plan* p, int src, cudaStream_t st)
 // ==========================================================================================
 extern "C" {
 
-const char* pgcn_version(void) { return "pgcn_b200 0.1 (sm_100a, CSR row-block SpMM + halo exchange)"; }
+const char* pgcn_version(void) { return "pgcn_b200 0.1 (sm_90a, CSR row-block SpMM + halo exchange)"; }
 
 int pgcn_device_count(void)
 {
@@ -759,7 +759,7 @@ int pgcn_plan_create(const int32_t* rowptr, const int32_t* colidx, const float* 
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
         cudaGetLastError();
-        return fail(nullptr, PGCN_ERR_NOGPU, "no CUDA device: the PGCN B200 path has no CPU fallback");
+        return fail(nullptr, PGCN_ERR_NOGPU, "no CUDA device: the PGCN GPU path has no CPU fallback");
     }
     const int64_t nnz = rowptr[m];
     if (nnz > 0 && (!colidx || !vals || !t_colidx || !t_vals)) return fail(nullptr, PGCN_ERR_INVALID, "null colidx/vals");
@@ -783,7 +783,7 @@ int pgcn_plan_create(const int32_t* rowptr, const int32_t* colidx, const float* 
     std::vector<int> refs_fwd((size_t)m + h), refs_tr((size_t)m);
     for (int r = 0; r < m + h; ++r) refs_fwd[r] = t_rowptr[r + 1] - t_rowptr[r];
     for (int r = 0; r < m; ++r) refs_tr[r] = rowptr[r + 1] - rowptr[r];
-    // rows of H kept hot in L2: about half of the 126 MB L2, the rest is left to the streams
+    // rows of H kept hot in L2: about half of the H100's 50 MB L2, the rest is left to the streams
     if (const char* e = getenv("PGCN_HOT_MB")) p->opt_hot_mb = std::max<long long>(0, atoll(e));   // tuning knob
     const int64_t hot_rows = std::max<int64_t>(1, (p->opt_hot_mb << 20) / ((int64_t)f_max * 4));
     auto cold_threshold = [&](const std::vector<int>& refs) -> int {

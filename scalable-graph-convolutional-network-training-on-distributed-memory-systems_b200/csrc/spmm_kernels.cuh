@@ -1,6 +1,6 @@
-// spmm_kernels.cuh — sm_100a kernels of the PGCN aggregation path.
+// spmm_kernels.cuh — sm_90a kernels of the PGCN aggregation path.
 //
-// Replaces, on a B200:
+// Replaces, on an H100:
 //   torch.sparse.mm(A, H)        GPU/PGCN.py:127      -> spmm_rowblock_kernel (forward CSR)
 //   torch.sparse.mm(A.t(), g)    GPU/PGCN.py:132      -> spmm_rowblock_kernel (pre-transposed CSR)
 //   H[send_map[p]] per peer      GPU/PGCN.py:104      -> pack_rows_kernel (all peers, one launch)
@@ -33,9 +33,9 @@ namespace pgcn {
 // pointers at all — it walks a block's edge range and flushes when it meets the mark.
 // Bit 30 marks a COLD column (few references): its H row is loaded with an L2 evict_first policy
 // while the hot rows (hubs, the part of H that fits in L2) are loaded evict_last, so streaming
-// traffic does not push the re-used rows out of the 126 MB L2.
+// traffic does not push the re-used rows out of the 50 MB L2.
 // Device layout of a CSR's entries: consecutive PIECES of 32 entries, one 272-byte record each (one TMA bulk copy):
-//   int   col[32]    plain column indices (no flag bits: they go straight into TMA gather4 coordinates)
+//   int   col[32]    plain column indices (no flag bits: they go straight into TMA row coordinates)
 //   float val[32]
 //   uint  emask      bit i: entry i is the LAST of its row        uint cmask   bit i: entry i's column is COLD
 //   uint  pad[2]

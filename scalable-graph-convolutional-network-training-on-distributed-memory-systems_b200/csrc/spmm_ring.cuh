@@ -1,6 +1,6 @@
-// spmm_ring.cuh — the Blackwell-native SpMM of the PGCN aggregation path: gathered H rows are staged
-// ASYNCHRONOUSLY in shared memory (1-D TMA bulk copies, cp.async.bulk + mbarrier complete_tx), the
-// segmented FMA runs out of shared memory.
+// spmm_ring.cuh — the Hopper (sm_90a) SpMM of the PGCN aggregation path: gathered H rows are staged
+// ASYNCHRONOUSLY in shared memory (TMA: 1-D cp.async.bulk or 2-D tensor-map copies, mbarrier complete_tx),
+// the segmented FMA runs out of shared memory.
 //
 // Replaces torch.sparse.mm(A, H) / torch.sparse.mm(A.t(), g) of GPU/PGCN.py:127,132 for feature widths
 // that are multiples of 128 floats (the benchmark widths 128 and 256); other widths take the register
@@ -56,15 +56,15 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
         "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
         ::"r"(dst), "l"(src), "r"(bytes), "r"(bar), "l"(pol) : "memory");
 }
-// 2-D tensor-map TMA in tile::gather4 mode: FOUR arbitrary rows of H (row indices r0..r3, column offset x) land as
-// four consecutive row slots in shared memory with ONE instruction (UTMALDG.2D.GATHER4).
-__device__ __forceinline__ void tma_gather4(uint32_t dst, const CUtensorMap* tm, int x, int r0, int r1, int r2, int r3,
-                                            uint32_t bar, unsigned long long pol)
+// 2-D tensor-map TMA in tile mode: one row tile of H (row r, column offset x; the map's box is {tile, 1 row}) lands
+// in one row slot (UTMALDG.2D). The map carries the row pitch, so the issuing lane computes no address.
+__device__ __forceinline__ void tma_row(uint32_t dst, const CUtensorMap* tm, int x, int r, uint32_t bar,
+                                       unsigned long long pol)
 {
     asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cta.global.tile::gather4.mbarrier::complete_tx::bytes.L2::cache_hint"
-        " [%0], [%1, {%2, %3, %4, %5, %6}], [%7], %8;"
-        ::"r"(dst), "l"(tm), "r"(x), "r"(r0), "r"(r1), "r"(r2), "r"(r3), "r"(bar), "l"(pol) : "memory");
+        "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.L2::cache_hint"
+        " [%0], [%1, {%2, %3}], [%4], %5;"
+        ::"r"(dst), "l"(tm), "r"(x), "r"(r), "r"(bar), "l"(pol) : "memory");
 }
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, unsigned long long pol)
 {
@@ -135,16 +135,16 @@ __device__ __forceinline__ void reg_set(uint32_t (&a)[N], int i, uint32_t v)
 // VPL : 128-float vector groups per row (tile of f).
 // G   : edges per completion group (8, 16 or 32); NG: groups in the ring (2 or 4); the warp owns NS = G * NG row slots.
 // MODE: 0 = 1-D TMA bulk copies (UBLKCP, one per row), 1 = per-lane 16-byte cp.async (LDGSTS + wait_group),
-//       2 = 2-D tensor-map TMA in tile::gather4 mode (UTMALDG.2D.GATHER4, FOUR rows per instruction; quads that mix
-//           own and halo columns, or groups cut by a block boundary, fall back to the 1-D copies of MODE 0).
+//       2 = 2-D tensor-map TMA in tile mode (UTMALDG.2D, one row per instruction; own and halo rows through
+//           their own tensor map).
 // HALO: columns >= split live in a second matrix (the halo slab).
 //
 // The entries are walked in GLOBALLY ALIGNED units: a piece = entries [32 P, 32 P + 32) (one 272-byte record =
 // one bulk copy: 32 plain column indices, 32 values, a row-end bit mask and a cold-column bit mask), a group =
 // entries [G g, G g + G) (one completion unit of the row ring, slot group g % NG). A row block [e0, e1) starts and
 // ends anywhere; entries of its first / last group outside the block are masked. The steady state per group is:
-//   issue   : one broadcast LDS.64 (masks), lanes 0..G/4-1 read their four column indices with one LDS.128 and
-//             fire one gather4 each; lane 0 arms the group's mbarrier with G x row bytes;
+//   issue   : one broadcast LDS.64 (masks), lanes 0..G-1 read their column index and fire one TMA copy each;
+//             lane 0 arms the group's mbarrier with G x row bytes;
 //   consume : mbarrier wait, 8 x LDS.128 rows + 2 x LDS.128 values (straight from the resident piece), 32 FFMA per
 //             8 edges; a row-end test per edge only in groups whose row-end mask is non-zero.
 // Pieces stay resident until their last group has been CONSUMED (the values are read at consumption time), so
@@ -269,35 +269,15 @@ __device__ __forceinline__ void ring_body(const SpmmArgs& a, const RingArgs& ra,
                 return;
             }
             if (lane == 0) mbar_expect_tx(s_gbar + sg * 8, (uint32_t)__popc(vm) * RB);
-            uint32_t single = vm;                                        // entries copied one row at a time (1-D bulk)
-            if (MODE == 2 && vm == FULL) {
-                bool fire = lane < G / 4;
-                int4 q4 = make_int4(0, 0, 0, 0);
-                if (fire) q4 = *reinterpret_cast<const int4*>(cols + lane * 4);
-                bool allhalo = false;
-                if (HALO) {
-                    const unsigned r0 = (unsigned)q4.x, r1 = (unsigned)q4.y, r2 = (unsigned)q4.z, r3 = (unsigned)q4.w;
-                    const bool allown = r0 < usplit && r1 < usplit && r2 < usplit && r3 < usplit;
-                    allhalo = r0 >= usplit && r1 >= usplit && r2 >= usplit && r3 >= usplit;
-                    fire = fire && (allown || allhalo);
-                    const uint32_t okq = __ballot_sync(0xffffffffu, fire);      // bit q: quad q goes out as one gather4
-                    single = 0;
-#pragma unroll
-                    for (int q = 0; q < G / 4; ++q) single |= (okq >> q & 1) ? 0u : (0xfu << (4 * q));
-                } else {
-                    single = 0;
-                }
-                if (fire) {
-                    const int sub = allhalo ? (int)usplit : 0;
-                    const bool cold = ((cm >> (lane * 4)) & 0xfu) == 0xfu;
-                    tma_gather4(s_data + (sg * G + lane * 4) * RB, allhalo ? tm1 : tm0, (int)(blockIdx.y * (RB / 4)),
-                                q4.x - sub, q4.y - sub, q4.z - sub, q4.w - sub, s_gbar + sg * 8, cold ? pol_cold : pol_hot);
-                }
-            }
-            if (lane < G && (single >> lane & 1)) {
+            if (lane < G && (vm >> lane & 1)) {
                 const unsigned cj = (unsigned)cols[lane];
-                bulk_g2s(s_data + (sg * G + lane) * RB, (cj >= usplit ? hb1 : hb0) + (size_t)cj * pitch, RB,
-                         s_gbar + sg * 8, (cm >> lane & 1) ? pol_cold : pol_hot);
+                const bool halo = cj >= usplit;
+                const unsigned long long pol = (cm >> lane & 1) ? pol_cold : pol_hot;
+                if (MODE == 2)
+                    tma_row(s_data + (sg * G + lane) * RB, halo ? tm1 : tm0, (int)(blockIdx.y * (RB / 4)),
+                            (int)(halo ? cj - usplit : cj), s_gbar + sg * 8, pol);
+                else
+                    bulk_g2s(s_data + (sg * G + lane) * RB, (halo ? hb1 : hb0) + (size_t)cj * pitch, RB, s_gbar + sg * 8, pol);
             }
         };
         // consume slot group sg = the group at sub-position qs of piece `pc`
@@ -425,10 +405,10 @@ spmm_ring_kernel(const SpmmArgs a, const RingArgs ra)
     ring_body<VPL, G, NG, MODE, HALO>(a, ra, nullptr, nullptr);
 }
 
-// gather4 variant: the tensor maps of H_own (tm0) and of the halo slab (tm1) travel as __grid_constant__ parameters
+// tensor-map variant: the tensor maps of H_own (tm0) and of the halo slab (tm1) travel as __grid_constant__ parameters
 template <int VPL, int G, int NG, bool HALO>
 __global__ void __launch_bounds__(kRingWarps * 32)
-spmm_ring_g4_kernel(const SpmmArgs a, const RingArgs ra, const __grid_constant__ CUtensorMap tm0,
+spmm_ring_tm_kernel(const SpmmArgs a, const RingArgs ra, const __grid_constant__ CUtensorMap tm0,
                     const __grid_constant__ CUtensorMap tm1)
 {
     ring_body<VPL, G, NG, 2, HALO>(a, ra, &tm0, &tm1);

@@ -112,7 +112,7 @@ def read_cpu_buff(path):
 
 
 def read_cpu_partition(dirpath, k):
-    """Everything `gcnhgp -o dir -k k` wrote, as the inputs of the B200 path: the global adjacency (union of the
+    """Everything `gcnhgp -o dir -k k` wrote, as the inputs of the H100 path: the global adjacency (union of the
     A.k blocks, scipy COO) and the part vector (from the H.k row lists), plus the parsed conn/buff files so a
     caller can compare the reference's connectivity with the one the plan builder derives from A.
     Note: the reference derives `conn` from the OUT-entries of a vertex (owner(i) sends i to owner(j) for A[i][j] != 0,

@@ -59,7 +59,7 @@ def batch_local_plans(A, partvec, rank, size, batch_size, seed=1, index_sets=Non
 # ---- training driver ---------------------------------------------------------------------------------------------
 
 def run(rank, size, nlayers, nfeatures, path_A, path_partvec, backend, batch_size, out=None, seed=None):
-    """GPU/PGCN-Mini-batch.py:199-310 on the B200 path. Returns {"losses", "elapsed", "total_vol", "total_nmsg"}."""
+    """GPU/PGCN-Mini-batch.py:199-310 on the H100 path. Returns {"losses", "elapsed", "total_vol", "total_nmsg"}."""
     import sys
     import time
     import torch
@@ -71,7 +71,7 @@ def run(rank, size, nlayers, nfeatures, path_A, path_partvec, backend, batch_siz
     import torch.nn.functional as F
     out = sys.stdout if out is None else out
     if backend != "nccl":
-        raise RuntimeError("backend '%s': the B200 PGCN path runs on CUDA devices over NCCL/NVLink only "
+        raise RuntimeError("backend '%s': the H100 PGCN path runs on CUDA devices over NCCL/NVLink only "
                            "(no CPU fallback); use -b nccl" % backend)
     device = torch.device("cuda", rank % torch.cuda.device_count())
     torch.cuda.set_device(device)

@@ -1,4 +1,4 @@
-"""PSpMM — the operator boundary of the hot path (GPU/PGCN.py:121-134), B200-native.
+"""PSpMM — the operator boundary of the hot path (GPU/PGCN.py:121-134), H100-native.
 
     PSpMM.apply(A, H)     A = PgcnPlan (the opaque plan handle standing in for the sparse tensor)
                           H = fp32 CUDA tensor
@@ -26,7 +26,7 @@ def _stream_ptr():
 
 def _check_feat(plan, H, rows, what):
     if not H.is_cuda:
-        raise RuntimeError("%s must be a CUDA tensor: the PGCN B200 path has no CPU fallback" % what)
+        raise RuntimeError("%s must be a CUDA tensor: the PGCN H100 path has no CPU fallback" % what)
     if H.dtype != torch.float32:
         raise TypeError("%s must be float32, got %s" % (what, H.dtype))
     if H.dim() != 2 or H.shape[0] != rows:

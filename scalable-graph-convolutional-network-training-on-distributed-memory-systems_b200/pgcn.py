@@ -1,4 +1,4 @@
-"""PGCN trainer CLI — the reference's surface (GPU/PGCN.py:136-286) over the B200 operator.
+"""PGCN trainer CLI — the reference's surface (GPU/PGCN.py:136-286) over the H100 operator.
 
     python PGCN.py -a A.mtx -p A.mtx.8.hp -b nccl -s 8 -l 2 -f 128
 
@@ -13,7 +13,7 @@ dict, `Elapsed time {:.4f}`, `total_vol: .. total_nmsg: ..` (:224-238).
 Different by design (SURVEY.md §8a/§8b): every tensor is [m_local, f] instead of [n, f]; the loss is
 the reference's value computed from owned rows only, loss = (sum_owned nll + (n - m) * log f) / n,
 which has exactly the reference's gradients (its non-owned rows are all-zero logits); the elapsed
-time is bracketed by torch.cuda.synchronize(); `-b gloo` is refused — the B200 path has no CPU
+time is bracketed by torch.cuda.synchronize(); `-b gloo` is refused — the H100 path has no CPU
 fallback (the CPU oracle lives under oracle/ and is test infrastructure).
 `--ref-quirks` reproduces quirk Q1 (halo rows counted twice in layer 1 because `run` feeds a fully
 populated H into `H + X`, GPU/PGCN.py:117,186) so loss curves can be compared with seeded weights.
@@ -90,7 +90,7 @@ def reference_loss(logits_own, labels_own, n):
 def run(rank, size, nlayers, nfeatures, path_A, path_partvec, backend, ref_quirks=False, transport="auto",
         out=sys.stdout, seed=None, fused=False):
     if backend != "nccl":
-        raise RuntimeError("backend '%s': the B200 PGCN path runs on CUDA devices over NCCL/NVLink only "
+        raise RuntimeError("backend '%s': the H100 PGCN path runs on CUDA devices over NCCL/NVLink only "
                            "(no CPU fallback); use -b nccl" % backend)
     device = torch.device("cuda", rank % torch.cuda.device_count())      # GPU/PGCN.py:169
     torch.cuda.set_device(device)

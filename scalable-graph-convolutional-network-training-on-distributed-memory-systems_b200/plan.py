@@ -6,7 +6,7 @@ n x n COO with global indices (:53-64). Here the same information is produced wi
   * `compute_communication_maps` / `get_partition_of_adjacency_matrix`: same names, arguments and
     return meaning as the reference functions (dicts of sorted global ids per peer; the owned rows
     of A) — drop-in for callers that want the reference's data structures;
-  * `build_local_plan`: the compact per-rank layout the B200 kernels consume — local CSR (int32)
+  * `build_local_plan`: the compact per-rank layout the H100 kernels consume — local CSR (int32)
     over the column space [own | halo grouped by source peer, sorted by global id], its transpose,
     send_idx / send_off / recv_off. Sender order == receiver order because both sides sort by
     global id (the invariant GPU/PGCN.py:47-48 relies on);

@@ -26,16 +26,16 @@ def test_library_exports_every_declared_symbol():
     lib = cabi.load()
     for name in header_symbols():
         assert hasattr(lib, name), "libpgcn_b200.so does not export " + name
-    assert b"sm_100a" in lib.pgcn_version()
+    assert b"sm_90a" in lib.pgcn_version()
 
 
-def test_built_for_sm_100a():
+def test_built_for_sm_90a():
     import shutil
     import subprocess
     if shutil.which("cuobjdump") is None:
         pytest.skip("cuobjdump not available")
     out = subprocess.run(["cuobjdump", "-lelf", cabi.lib_path()], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out
 
 
 def test_invalid_arguments_are_reported_not_crashing():

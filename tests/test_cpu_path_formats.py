@@ -1,6 +1,6 @@
 """Reader of the CPU path's on-disk formats (SURVEY.md §8f rank 4) against files written by the reference's
 own partitioner binary (tests/golden/cpu_path, make_cpu_path_fixtures.py): A.k / H.k / conn.k / buff.k /
-config of GCN-HP/main.cpp -> the (A, partvec) inputs of the B200 plan builder."""
+config of GCN-HP/main.cpp -> the (A, partvec) inputs of the plan builder."""
 import os
 
 import numpy as np

@@ -1,11 +1,11 @@
-"""Parity of the sm_100a path (called through the C-ABI, libpgcn_b200.so) against
+"""Parity of the sm_90a path (called through the C-ABI, libpgcn_b200.so) against
   * the golden outputs of the unmodified reference (tests/golden, k = 1, 2, 3 ranks),
   * the fp64 truth within the fp32 bound of SURVEY.md §8a:  |Z - Z64| <= 2 d 2^-24 (|A||H|),
   * the CPU oracle on seeded R-MAT inputs with hubs, empty rows, duplicates, odd feature widths,
 and, at the benchmark's full size, through size-independent properties (column-sum checksum,
 adjointness <A H, G> == <H, A^T G>, linearity).
 
-Every rank's plan lives on the one GPU of the box here: the kernels, the compact layout and the
+Every rank's plan lives on one GPU here: the kernels, the compact layout and the
 pack / unpack kernels are exercised per rank, with the wire step replaced by a device copy in
 wire order. The real transports (NCCL, peer memory) are covered by tests/test_multigpu.py.
 """
@@ -24,7 +24,7 @@ pytestmark = pytest.mark.gpu
 
 def dev():
     if not torch.cuda.is_available():
-        pytest.fail("no CUDA device: -m gpu tests must run on the B200 box")
+        pytest.fail("no CUDA device: -m gpu tests must run on a GPU machine")
     return torch.device("cuda", 0)
 
 

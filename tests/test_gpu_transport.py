@@ -1,4 +1,4 @@
-"""The peer-memory transport of the halo exchange on ONE GPU (so the driver's single-GPU box sees it run):
+"""The peer-memory transport of the halo exchange on ONE GPU (so a single-GPU machine runs it):
 
   * every rank's plan in this process on cuda:0, wired with plan.link_local_plans (same-process peers are reached
     through plain device pointers): fused put + epoch-signal kernels, per-peer wait kernels, the per-peer pipelined
@@ -27,7 +27,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 def dev():
     if not torch.cuda.is_available():
-        pytest.fail("no CUDA device: -m gpu tests must run on the B200 box")
+        pytest.fail("no CUDA device: -m gpu tests must run on a GPU machine")
     return torch.device("cuda", 0)
 
 

@@ -3,7 +3,7 @@
 exchange and how the SpMM work is balanced, per method (hp / gp shipped under bench_data/, rp = uniform random seed 1,
 block = contiguous ranges). One markdown row per (method, k): halo rows in (max / mean per rank), stored entries (max /
 mean per rank), total halo rows, and the two bounds they imply per layer at f floats per row:
-   t_xchg >= 4 f max_in / 770 GB/s (measured peer copy rate, B200_PROFILING.md)     t_spmm ~ max entries / single-GPU rate.
+   t_xchg >= 4 f max_in / 450 GB/s (H100 NVLink 4 per direction, data sheet)     t_spmm ~ max entries / single-GPU rate.
 
     python tools/partition_table.py --config C5 --k 8 [--methods hp gp rp block]
 """

@@ -138,7 +138,7 @@ def main():
             point({"edges_per_block": epb, "tile_floats": 0, "long_row": lr})
     elif args.sweep == "ring":
         # register pipeline (kernel 4) vs the shared-memory ring filled by 1-D TMA bulk copies (5) / cp.async (6) /
-        # TMA tile::gather4 (7); ring shapes: 16 slots (2 groups of 8), 32 (2 x 16), 64 (2 x 32 or 4 x 16)
+        # 2-D tensor-map TMA (7); ring shapes: 16 slots (2 groups of 8), 32 (2 x 16), 64 (2 x 32 or 4 x 16)
         point({"kernel": 4})
         for kern, (slots, groups), epb in itertools.product((7, 5), ((16, 2), (32, 2), (64, 2), (64, 4)), (256, 512, 1024)):
             if kern == 5 and slots == 64:
