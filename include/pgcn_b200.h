@@ -101,6 +101,10 @@ int pgcn_plan_destroy(pgcn_plan* plan);
  *                          register-pipeline kernel; 4 = always the register kernel; 5 / 6 / 7 = ring kernel fed by
  *                          1-D cp.async.bulk / cp.async / 2-D tensor-map TMA (one row per copy)
  *   "ring_slots"           row slots per warp of the ring kernel: 16 (default), 32, 64; "ring_groups" 2 | 4 (64 slots)
+ *   "ring_tile_floats"     floats of H one ring slot holds: 0 = tuned by pgcn_plan_autotune, else the full width
+ *                          (256 when f % 256 == 0, else 128) (default); 64 = 256-byte slices, gathered one slice of
+ *                          every row after the other so that less of H competes for L2; 128, 256. A width that does
+ *                          not divide f, and 64 with "kernel" 6, take the full width. Results do not depend on it.
  *   "ring_edges_per_block" target nnz of one row block = one warp's unit of work          (default 512)
  *   "ring_long_row"        rows with more nnz than this are split into segments           (default 2 * block)
  *   "persistent"           1 = persistent CTAs fetch row blocks dynamically (default; single-rank plans and plans
@@ -111,8 +115,8 @@ int pgcn_plan_destroy(pgcn_plan* plan);
  *                          (Parallel-GCN/main.c:271 then :275-299)                         (default 1)
  *   "relu"                 1 = pgcn_forward writes max(0, A_local * H)                      (default 0)
  *   "p2p"                  0 = never use the peer-memory transport (all ranks must agree)  (default 1)
- * pgcn_plan_autotune overrides block sizes / ring depth per matrix; setting one of them explicitly clears the tuned
- * values. "hot_mb" (L2-resident hot set of H rows) is fixed at plan creation: environment variable PGCN_HOT_MB.
+ * pgcn_plan_autotune overrides block sizes / ring depth / ring tile width per matrix; setting a block size or the
+ * ring depth explicitly clears the tuned values, a non-zero "ring_tile_floats" overrides the tuned width. "hot_mb" (L2-resident hot set of H rows) is fixed at plan creation: environment variable PGCN_HOT_MB.
  * Split rows are always reduced in a fixed order: results are run-to-run deterministic.
  * Read-only names for pgcn_plan_get_option: "nccl", "blocks_fwd", "long_rows_fwd", "ring_blocks_fwd",
  * "ring_long_rows_fwd".

@@ -77,7 +77,8 @@ struct DevCsr {
     int nrows_c = 0;                // non-empty rows = rows the schedule walks
     int64_t nnz = 0;
     std::vector<int> h_rowptr;      // COMPACT row pointers (empty rows squeezed out), for scheduling
-    int* d_cw = nullptr;            // entries in 272-byte pieces of 32: col[32] | val[32] | row-end mask | cold mask | pad
+    int* d_cw = nullptr;            // entries in 272-byte pieces of 32: col[32] | val[32] | row-end mask | cold mask |
+                                    // cold mask of 64-float slices | pad
     int* d_rowids = nullptr;        // compact row -> output row, null when the identity
     int* d_empty = nullptr;         // output rows without entries (zero-filled when beta == 0)
     int nempty = 0;
@@ -87,6 +88,7 @@ struct DevCsr {
     unsigned char* d_final = nullptr;     // per walked row: this matrix is the LAST launch of the forward that writes it
     int64_t tuned_epb[2] = {0, 0};  // per-matrix autotune results (0: use the plan option): [0] register, [1] ring
     int tuned_slots = 0;
+    int tuned_tile = 0;             // ring row tile in floats (0: the full width 128 or 256)
     // schedules: [0] register-pipeline kernel (small row blocks, one per lane group),
     //            [1] shared-memory ring kernel (large row blocks, one per warp)
     struct Sched {
@@ -146,9 +148,10 @@ struct pgcn_plan {
     int64_t opt_ring_groups = 2;
     int64_t opt_persistent_multi = 0;
     int64_t opt_kernel = 0, opt_ring_slots = 16, opt_ring_epb = 512, opt_ring_long = 0, opt_persistent = 1;
-    bool ring_attr_set[48] = {false};
-    int ring_ctas_per_sm[48] = {0};
-    unsigned int* d_counter = nullptr;     // block counters of the persistent ring kernel (one per feature tile)
+    int64_t opt_ring_tile = 0;       // ring row tile in floats: 0 = tuned (else full width), 64 | 128 | 256
+    bool ring_attr_set[72] = {false};
+    int ring_ctas_per_sm[72] = {0};
+    unsigned int* d_counter = nullptr;     // work-item counter of the persistent ring kernel
     int num_sms = 132;
 
     // NCCL
@@ -220,11 +223,12 @@ int upload(pgcn_plan* p, T** dst, const T* src, size_t n)
 // Upload one CSR. Rows without entries are squeezed out of the walked row space (their outputs are
 // zero-filled by a separate launch); `ext_rowmap` maps the rows of an already-compact matrix (the
 // halo-column part, which only holds boundary rows) to output rows.
-// `col_refs[j]` = number of stored entries in column j and `cold_thresh` the reference count at or
-// below which a column is COLD (-1: no marking): cold columns get kColdFlag and are gathered with an
-// L2 evict_first policy, the most-referenced rows of H (as many as fit the hot budget) evict_last.
+// `col_refs[j]` = number of stored entries in column j and `cold[0]` the reference count at or
+// below which a column is COLD for full-width rows, `cold[1]` the same for 64-float slices (-1: no marking):
+// cold columns are gathered with an L2 evict_first policy, the most-referenced rows of H (as many as fit the hot
+// budget) evict_last.
 int csr_upload(pgcn_plan* p, DevCsr& c, int nrows, const int* rowptr, const int* colidx, const float* vals,
-               const std::vector<int>* ext_rowmap = nullptr, const int* col_refs = nullptr, int cold_thresh = -1,
+               const std::vector<int>* ext_rowmap = nullptr, const int* col_refs = nullptr, const int* cold = nullptr,
                bool keep_host = false)
 {
     c.nrows = nrows;
@@ -236,7 +240,8 @@ int csr_upload(pgcn_plan* p, DevCsr& c, int nrows, const int* rowptr, const int*
         const int i = (int)(e & 31);
         pc[i] = colidx[e];
         memcpy(&pc[32 + i], &vals[e], 4);
-        if (col_refs && cold_thresh >= 0 && col_refs[colidx[e]] <= cold_thresh) pc[65] |= (int)(1u << i);
+        for (int w = 0; w < 2; ++w)
+            if (col_refs && cold && cold[w] >= 0 && col_refs[colidx[e]] <= cold[w]) pc[65 + w] |= (int)(1u << i);
     }
     std::vector<int> rowids, empty;
     c.h_rowptr.clear();
@@ -449,31 +454,36 @@ bool make_row_map(CUtensorMap* tm, const float* base, int64_t rows, int f, int t
 struct RingShape { int g, ng; };
 const RingShape kRingShapes[4] = {{8, 2}, {16, 2}, {32, 2}, {16, 4}};
 
-template <int VPL, bool HALO>
+// Row tiles: tf = 64 (256-byte slices), 128 or 256 floats. The cp.async fill (mode 1) needs tf >= 128.
+template <int TF, bool HALO>
 ring_fn pick_ring_t(int shape, int mode)
 {
-    if (mode == 1) return spmm_ring_kernel<VPL, 8, 2, 1, HALO>;
-    return shape == 1 ? spmm_ring_kernel<VPL, 16, 2, 0, HALO> : spmm_ring_kernel<VPL, 8, 2, 0, HALO>;
+    if constexpr (TF >= 128) {
+        if (mode == 1) return spmm_ring_kernel<TF, 8, 2, 1, HALO>;
+    }
+    return shape == 1 ? spmm_ring_kernel<TF, 16, 2, 0, HALO> : spmm_ring_kernel<TF, 8, 2, 0, HALO>;
 }
-ring_fn pick_ring(int vpl, int shape, int mode, bool halo)
+ring_fn pick_ring(int tf, int shape, int mode, bool halo)
 {
-    if (vpl == 2) return halo ? pick_ring_t<2, true>(shape, mode) : pick_ring_t<2, false>(shape, mode);
-    return halo ? pick_ring_t<1, true>(shape, mode) : pick_ring_t<1, false>(shape, mode);
+    if (tf == 256) return halo ? pick_ring_t<256, true>(shape, mode) : pick_ring_t<256, false>(shape, mode);
+    if (tf == 64) return halo ? pick_ring_t<64, true>(shape, mode) : pick_ring_t<64, false>(shape, mode);
+    return halo ? pick_ring_t<128, true>(shape, mode) : pick_ring_t<128, false>(shape, mode);
 }
-template <int VPL, bool HALO>
+template <int TF, bool HALO>
 ring_tm_fn pick_ring_tm_t(int shape)
 {
     switch (shape) {
-        case 1: return spmm_ring_tm_kernel<VPL, 16, 2, HALO>;
-        case 2: return spmm_ring_tm_kernel<VPL, 32, 2, HALO>;
-        case 3: return spmm_ring_tm_kernel<VPL, 16, 4, HALO>;
-        default: return spmm_ring_tm_kernel<VPL, 8, 2, HALO>;
+        case 1: return spmm_ring_tm_kernel<TF, 16, 2, HALO>;
+        case 2: return spmm_ring_tm_kernel<TF, 32, 2, HALO>;
+        case 3: return spmm_ring_tm_kernel<TF, 16, 4, HALO>;
+        default: return spmm_ring_tm_kernel<TF, 8, 2, HALO>;
     }
 }
-ring_tm_fn pick_ring_tm(int vpl, int shape, bool halo)
+ring_tm_fn pick_ring_tm(int tf, int shape, bool halo)
 {
-    if (vpl == 2) return halo ? pick_ring_tm_t<2, true>(shape) : pick_ring_tm_t<2, false>(shape);
-    return halo ? pick_ring_tm_t<1, true>(shape) : pick_ring_tm_t<1, false>(shape);
+    if (tf == 256) return halo ? pick_ring_tm_t<256, true>(shape) : pick_ring_tm_t<256, false>(shape);
+    if (tf == 64) return halo ? pick_ring_tm_t<64, true>(shape) : pick_ring_tm_t<64, false>(shape);
+    return halo ? pick_ring_tm_t<128, true>(shape) : pick_ring_tm_t<128, false>(shape);
 }
 
 // CUDA loads kernels lazily, at their first launch, and that load synchronises with the device. A rank whose
@@ -491,11 +501,11 @@ void preload_kernels()
     for (int halo = 0; halo < 2; ++halo)
         for (int lpe = 4; lpe <= 32; lpe *= 2)
             for (int vpl = 1; vpl <= 4; vpl *= 2) { touch_kernel(pick_lpe<4>(lpe, vpl, halo != 0)); touch_kernel(pick_lpe<1>(lpe, vpl, halo != 0)); }
-    for (int vpl = 1; vpl <= 2; ++vpl)
+    for (int tf = 64; tf <= 256; tf *= 2)
         for (int halo = 0; halo < 2; ++halo) {
-            for (int shape = 0; shape < 4; ++shape) touch_kernel(pick_ring_tm(vpl, shape, halo != 0));
-            for (int shape = 0; shape < 2; ++shape) touch_kernel(pick_ring(vpl, shape, 0, halo != 0));
-            touch_kernel(pick_ring(vpl, 0, 1, halo != 0));
+            for (int shape = 0; shape < 4; ++shape) touch_kernel(pick_ring_tm(tf, shape, halo != 0));
+            for (int shape = 0; shape < 2; ++shape) touch_kernel(pick_ring(tf, shape, 0, halo != 0));
+            if (tf >= 128) touch_kernel(pick_ring(tf, 0, 1, halo != 0));
         }
     touch_kernel(zero_rows_kernel<4>); touch_kernel(zero_rows_kernel<1>);
     touch_kernel(spmm_fixup_kernel<4>); touch_kernel(spmm_fixup_kernel<1>);
@@ -549,31 +559,35 @@ int launch_spmm(pgcn_plan* p, DevCsr& c, const float* H0, const float* H1, int s
     a.partial = sc.d_partial; a.f = f; a.beta = beta;
     a.relu = relu; a.final = (relu && use_final) ? c.d_final : nullptr;
     if (sc.nblocks > 0 && ring) {
-        const int vpl = (f % 256 == 0) ? 2 : 1;
-        const int tiles = f / (128 * vpl);
-        const bool halo = (H1 != nullptr);
         int mode = p->opt_kernel == 6 ? 1 : (p->opt_kernel == 5 ? 0 : 2);   // default: 2-D tensor-map TMA
+        // row tile: the option, else the tuned width, else the full width (256 floats when f allows, else 128);
+        // a width that does not divide f, and 64-float slices with the cp.async fill, take the full width
+        const int full = (f % 256 == 0) ? 256 : 128;
+        int tf = (int)(p->opt_ring_tile > 0 ? p->opt_ring_tile : (c.tuned_tile > 0 ? c.tuned_tile : full));
+        if (f % tf != 0 || (mode == 1 && tf < 128)) tf = full;
+        const int tiles = f / tf;
+        const bool halo = (H1 != nullptr);
         // ring shape from the options: ring_slots = 16 | 32 | 64, ring_groups = 2 | 4 (only with 64 slots)
         const int64_t want_slots = c.tuned_slots > 0 ? c.tuned_slots : p->opt_ring_slots;
         int shape = want_slots <= 16 ? 0 : (want_slots <= 32 ? 1 : (p->opt_ring_groups == 4 ? 3 : 2));
         CUtensorMap tm0, tm1;
         if (mode == 2) {
             // H0 holds the columns below `split` (all of them when there is no halo slab), H1 the rest
-            const int tile = 128 * vpl;
-            bool ok = make_row_map(&tm0, H0, 1 << 30, f, tile, 1);
-            if (ok && H1) ok = make_row_map(&tm1, H1, 1 << 30, f, tile, 1);
+            bool ok = make_row_map(&tm0, H0, 1 << 30, f, tf, 1);
+            if (ok && H1) ok = make_row_map(&tm1, H1, 1 << 30, f, tf, 1);
             else if (ok) tm1 = tm0;
             if (!ok) mode = 0;                                   // no driver entry point: 1-D bulk copies
         }
         if (mode == 1) shape = 0;
         if (mode == 0 && shape > 1) shape = 1;
         const int g = kRingShapes[shape].g, ng = kRingShapes[shape].ng;
-        ring_fn fn = mode == 2 ? nullptr : pick_ring(vpl, shape, mode, halo);
-        ring_tm_fn fn_tm = mode == 2 ? pick_ring_tm(vpl, shape, halo) : nullptr;
+        ring_fn fn = mode == 2 ? nullptr : pick_ring(tf, shape, mode, halo);
+        ring_tm_fn fn_tm = mode == 2 ? pick_ring_tm(tf, shape, halo) : nullptr;
         const void* fptr = mode == 2 ? (const void*)fn_tm : (const void*)fn;
-        const size_t smem = ring_smem_bytes(vpl, g * ng, ng);
+        const size_t smem = ring_smem_bytes(tf, g * ng, ng);
         // opt-in to > 48 KB of dynamic shared memory, once per kernel instance
-        const int slot = (((vpl - 1) * 4 + shape) * 3 + mode) * 2 + (halo ? 1 : 0);
+        const int tslot = tf == 64 ? 0 : (tf == 128 ? 1 : 2);
+        const int slot = ((tslot * 4 + shape) * 3 + mode) * 2 + (halo ? 1 : 0);
         if (!p->ring_attr_set[slot]) {
             CU(p, cudaFuncSetAttribute(fptr, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
             int nb = 0;
@@ -591,9 +605,12 @@ int launch_spmm(pgcn_plan* p, DevCsr& c, const float* H0, const float* H1, int s
         // `persistent_multi` asks otherwise.
         const bool persistent = p->opt_persistent && (p->k == 1 || !p->opt_overlap || p->opt_persistent_multi);
         if (persistent) {
-            CU(p, cudaMemsetAsync(p->d_counter, 0, 64 * sizeof(unsigned int), st));
+            // one counter over all (tile, row block) items, tile-major: the tiles run one after the other
+            CU(p, cudaMemsetAsync(p->d_counter, 0, sizeof(unsigned int), st));
             ra.counter = p->d_counter;
-            grid.x = std::min<unsigned>(grid.x, (unsigned)(p->num_sms * p->ring_ctas_per_sm[slot]));
+            const unsigned items = (unsigned)(((int64_t)sc.nblocks * tiles + kRingWarps - 1) / kRingWarps);
+            grid.x = std::min<unsigned>(items, (unsigned)(p->num_sms * p->ring_ctas_per_sm[slot]));
+            grid.y = 1;
         }
         if (mode == 2) fn_tm<<<grid, kRingWarps * 32, smem, st>>>(a, ra, tm0, tm1);
         else fn<<<grid, kRingWarps * 32, smem, st>>>(a, ra);
@@ -785,15 +802,19 @@ int pgcn_plan_create(const int32_t* rowptr, const int32_t* colidx, const float* 
     for (int r = 0; r < m; ++r) refs_tr[r] = rowptr[r + 1] - rowptr[r];
     // rows of H kept hot in L2: about half of the H100's 50 MB L2, the rest is left to the streams
     if (const char* e = getenv("PGCN_HOT_MB")) p->opt_hot_mb = std::max<long long>(0, atoll(e));   // tuning knob
-    const int64_t hot_rows = std::max<int64_t>(1, (p->opt_hot_mb << 20) / ((int64_t)f_max * 4));
-    auto cold_threshold = [&](const std::vector<int>& refs) -> int {
+    // Two hot sets: one for full-width rows (f_max floats) and one for 64-float slices, which holds as many more rows
+    // as the slice is narrower (the ring kernel gathers one slice of every row before the next slice).
+    auto cold_threshold = [&](const std::vector<int>& refs, int64_t row_bytes) -> int {
+        const int64_t hot_rows = std::max<int64_t>(1, (p->opt_hot_mb << 20) / row_bytes);
         const int64_t ncols = (int64_t)refs.size();
         if (ncols <= hot_rows) return -1;                  // everything fits: nothing is cold
         std::vector<int> sorted(refs);
         std::nth_element(sorted.begin(), sorted.begin() + (ncols - hot_rows), sorted.end());
         return sorted[ncols - hot_rows];
     };
-    const int cold_fwd = cold_threshold(refs_fwd), cold_tr = cold_threshold(refs_tr);
+    const int64_t full_bytes = (int64_t)f_max * 4, slice_bytes = std::min<int64_t>(full_bytes, 64 * 4);
+    const int cold_fwd[2] = {cold_threshold(refs_fwd, full_bytes), cold_threshold(refs_fwd, slice_bytes)};
+    const int cold_tr[2] = {cold_threshold(refs_tr, full_bytes), cold_threshold(refs_tr, slice_bytes)};
     TRY(csr_upload(p, p->fwd, m, rowptr, colidx, vals, nullptr, refs_fwd.data(), cold_fwd));
     TRY(csr_upload(p, p->tr, m + h, t_rowptr, t_colidx, t_vals, nullptr, refs_tr.data(), cold_tr, true));
 
@@ -959,9 +980,9 @@ int pgcn_plan_set_option(pgcn_plan* p, const char* name, int64_t value)
     const std::string n(name);
     auto clear_tuned = [&]() {
         DevCsr* all[] = {&p->fwd, &p->tr, &p->own, &p->tr_own};
-        for (DevCsr* c : all) { c->tuned_epb[0] = c->tuned_epb[1] = 0; c->tuned_slots = 0; }
-        for (auto& c : p->halo_q) { c.tuned_epb[0] = c.tuned_epb[1] = 0; c.tuned_slots = 0; }
-        for (auto& c : p->tr_halo_q) { c.tuned_epb[0] = c.tuned_epb[1] = 0; c.tuned_slots = 0; }
+        for (DevCsr* c : all) { c->tuned_epb[0] = c->tuned_epb[1] = 0; c->tuned_slots = 0; c->tuned_tile = 0; }
+        for (auto& c : p->halo_q) { c.tuned_epb[0] = c.tuned_epb[1] = 0; c.tuned_slots = 0; c.tuned_tile = 0; }
+        for (auto& c : p->tr_halo_q) { c.tuned_epb[0] = c.tuned_epb[1] = 0; c.tuned_slots = 0; c.tuned_tile = 0; }
     };
     if (n == "edges_per_block" || n == "ring_edges_per_block" || n == "ring_slots") clear_tuned();   // explicit beats tuned
     if (n == "edges_per_block") p->opt_epb = value;
@@ -972,6 +993,11 @@ int pgcn_plan_set_option(pgcn_plan* p, const char* name, int64_t value)
     else if (n == "persistent") p->opt_persistent = value;
     else if (n == "persistent_multi") p->opt_persistent_multi = value;
     else if (n == "ring_groups") p->opt_ring_groups = value;
+    else if (n == "ring_tile_floats") {
+        if (value != 0 && value != 64 && value != 128 && value != 256)
+            return fail(p, PGCN_ERR_INVALID, "ring_tile_floats must be 0 (tuned), 64, 128 or 256, not %lld", (long long)value);
+        p->opt_ring_tile = value;
+    }
     else if (n == "long_row") p->opt_long = value;
     else if (n == "tile_floats") p->opt_tile = value;
     else if (n == "hot_mb")
@@ -1002,6 +1028,7 @@ int64_t pgcn_plan_get_option(const pgcn_plan* p, const char* name)
     if (n == "persistent") return p->opt_persistent;
     if (n == "persistent_multi") return p->opt_persistent_multi;
     if (n == "ring_groups") return p->opt_ring_groups;
+    if (n == "ring_tile_floats") return p->opt_ring_tile > 0 ? p->opt_ring_tile : p->fwd.tuned_tile;
     if (n == "long_row") return p->opt_long;
     if (n == "tile_floats") return p->opt_tile;
     if (n == "hot_mb") return p->opt_hot_mb;
@@ -1073,29 +1100,32 @@ int pgcn_plan_autotune(pgcn_plan* p, int32_t f)
         const int ncand = ring ? (int)(sizeof ring_cand / sizeof ring_cand[0]) : (int)(sizeof reg_cand / sizeof reg_cand[0]);
         const int which = ring ? 1 : 0;
         const int64_t keep_epb = c.tuned_epb[which];
-        const int keep_slots = c.tuned_slots;
-        int best = -1;
+        const int keep_slots = c.tuned_slots, keep_tile = c.tuned_tile;
+        // ring row tile: the full width (tuned_tile 0) and 64-float slices, unless the option fixes it
+        const int ntile = (ring && p->opt_ring_tile == 0) ? 2 : 1;
+        int best = -1, best_tile = 0;
         float best_ms = 1e30f;
+        for (int ti = 0; ti < ntile; ++ti)
         for (int i = 0; i < ncand; ++i) {
             c.tuned_epb[which] = cand[i].epb;
-            if (ring) c.tuned_slots = cand[i].slots;
+            if (ring) { c.tuned_slots = cand[i].slots; c.tuned_tile = ti ? 64 : 0; }
             float ms_min = 1e30f;
             for (int it = 0; it < 4; ++it) {                 // first pass also builds the schedule
                 cudaEventRecord(e0, st);
                 int r2 = launch_spmm(p, c, h0, h1, split, z0, z1, zsplit, f, beta, st);
                 cudaEventRecord(e1, st);
                 if (r2 || cudaEventSynchronize(e1) != cudaSuccess) {
-                    c.tuned_epb[which] = keep_epb; c.tuned_slots = keep_slots;
+                    c.tuned_epb[which] = keep_epb; c.tuned_slots = keep_slots; c.tuned_tile = keep_tile;
                     return r2 ? r2 : fail(p, PGCN_ERR_CUDA, "autotune: kernel failed");
                 }
                 float ms = 0.f;
                 cudaEventElapsedTime(&ms, e0, e1);
                 if (it > 0) ms_min = std::min(ms_min, ms);
             }
-            if (ms_min < best_ms) { best_ms = ms_min; best = i; }
+            if (ms_min < best_ms) { best_ms = ms_min; best = i; best_tile = ring ? c.tuned_tile : 0; }
         }
         c.tuned_epb[which] = cand[best].epb;
-        if (ring) c.tuned_slots = cand[best].slots;
+        if (ring) { c.tuned_slots = cand[best].slots; c.tuned_tile = best_tile; }
         return 0;
     };
 #define TUNE(...) do { if ((rc = tune(__VA_ARGS__))) { cleanup(); return rc; } } while (0)

@@ -38,7 +38,8 @@ namespace pgcn {
 //   int   col[32]    plain column indices (no flag bits: they go straight into TMA row coordinates)
 //   float val[32]
 //   uint  emask      bit i: entry i is the LAST of its row        uint cmask   bit i: entry i's column is COLD
-//   uint  pad[2]
+//   uint  smask      bit i: entry i's column is COLD for 64-float slices (the ring kernel's larger slice hot set)
+//   uint  pad
 // Entry e lives in piece e >> 5 at index e & 31. The register kernel rebuilds {col | flags, val} pairs as it loads.
 constexpr int kPieceInts = 68;
 constexpr int kPieceBytes = kPieceInts * 4;
@@ -85,6 +86,10 @@ __device__ __forceinline__ void vfma(float4& a, float w, const float4& r) {
     a.x = fmaf(w, r.x, a.x); a.y = fmaf(w, r.y, a.y); a.z = fmaf(w, r.z, a.z); a.w = fmaf(w, r.w, a.w);
 }
 __device__ __forceinline__ void vfma(float& a, float w, const float& r) { a = fmaf(w, r, a); }
+__device__ __forceinline__ void vfma(float2& a, float w, const float2& r) { a.x = fmaf(w, r.x, a.x); a.y = fmaf(w, r.y, a.y); }
+__device__ __forceinline__ void vadd(float2& a, const float2& r) { a.x += r.x; a.y += r.y; }
+__device__ __forceinline__ float2 vrelu(const float2& a) { return make_float2(fmaxf(a.x, 0.f), fmaxf(a.y, 0.f)); }
+__device__ __forceinline__ float2 vzero(float2*) { return make_float2(0.f, 0.f); }
 __device__ __forceinline__ void vadd(float4& a, const float4& r) { a.x += r.x; a.y += r.y; a.z += r.z; a.w += r.w; }
 __device__ __forceinline__ void vadd(float& a, const float& r) { a += r; }
 
@@ -142,6 +147,7 @@ __device__ __forceinline__ int2 ld_entry(const int* pieces, int e)
 // outputs: written once -> streaming stores.
 __device__ __forceinline__ void st_out(float4* p, const float4& v) { __stcs(p, v); }
 __device__ __forceinline__ void st_out(float* p, const float& v) { __stcs(p, v); }
+__device__ __forceinline__ void st_out(float2* p, const float2& v) { __stcs(p, v); }
 
 constexpr int kSpmmThreads = 256;
 

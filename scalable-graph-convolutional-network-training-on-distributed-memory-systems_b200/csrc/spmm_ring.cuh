@@ -18,6 +18,9 @@
 //     4 FFMA, a row-end test; bytes in flight per SM = warps x NS x row bytes (e.g. 12 x 32 x 512 B =
 //     192 KB) instead of 48 KB, at ~10 issue slots per edge.
 //   * MODE 1 is the same ring filled with per-lane 16-byte cp.async (LDGSTS) copies — kept for comparison.
+//   * a slot holds a row TILE of TF floats: the full width (128 or 256) or a 64-float slice (256 B; one LDS.64 and
+//     2 FFMA per edge and lane). Slices are walked one after the other, so only TF / f of H is live in L2 at a
+//     time: more of the gathered rows hit, for twice the issue work per edge.
 // Row blocks come from the same host schedule as the register kernel (rows cut into blocks of about
 // edges_per_block entries, long rows split into single-row segments that the fixup kernel sums in a fixed
 // order), one block per warp; with `counter` set, the CTAs are persistent and warps fetch blocks dynamically.
@@ -76,8 +79,8 @@ __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_gr
 
 // One call site per row end would replicate the store sequence 32+ times in the unrolled consumer; keeping it
 // out of line keeps the hot loop inside the instruction cache (the rows-end path runs once per ~17 edges).
-template <int VPL>
-__device__ __noinline__ void ring_store_row(float4 a0, float4 a1, const int* rowids, int row, float* Z0, float* Z1,
+template <class V, int NV>
+__device__ __noinline__ void ring_store_row(V a0, V a1, const int* rowids, int row, float* Z0, float* Z1,
                                             int zsplit, size_t pitch, size_t off, int beta, int relu, const unsigned char* final)
 {
     const bool relu_row = relu && (final == nullptr || __ldg(final + row) != 0);
@@ -85,12 +88,12 @@ __device__ __noinline__ void ring_store_row(float4 a0, float4 a1, const int* row
     char* zb = (orow < zsplit) ? reinterpret_cast<char*>(Z0) + (size_t)(unsigned)orow * pitch
                                : reinterpret_cast<char*>(Z1) + (size_t)(unsigned)(orow - zsplit) * pitch;
     zb += off;
-    float4* zp = reinterpret_cast<float4*>(zb);
+    V* zp = reinterpret_cast<V*>(zb);
     if (beta) vadd(a0, *zp);
     if (relu_row) a0 = vrelu(a0);
     st_out(zp, a0);
-    if (VPL == 2) {
-        float4* zq = reinterpret_cast<float4*>(zb + 512);
+    if (NV == 2) {
+        V* zq = reinterpret_cast<V*>(zb + 512);
         if (beta) vadd(a1, *zq);
         if (relu_row) a1 = vrelu(a1);
         st_out(zq, a1);
@@ -101,20 +104,26 @@ constexpr int kRingWarps = 2;        // warps per CTA (each fully independent: C
 constexpr int kRingPieces = 4;       // index pieces (32 entries, kPieceBytes each) resident per warp
 
 struct RingArgs {
-    unsigned int* counter;   // null: block = blockIdx.x * kRingWarps + warp; else dynamic (persistent CTAs)
+    unsigned int* counter;   // null: block blockIdx.x * kRingWarps + warp of tile blockIdx.y; else the next
+                             // (tile, block) work item, tile-major (persistent CTAs)
     const float* hub;        // reserved (hub rows resident in shared memory)
     int nhub;
 };
 
-// per warp: NS row slots | NP index pieces | NG + NP mbarriers
-__host__ __device__ constexpr size_t ring_warp_bytes(int vpl, int ns, int ng)
+// per warp: NS row slots of tf floats | NP index pieces | NG + NP mbarriers
+__host__ __device__ constexpr size_t ring_warp_bytes(int tf, int ns, int ng)
 {
-    return ((size_t)ns * vpl * 512 + (size_t)kRingPieces * kPieceBytes + (size_t)(ng + kRingPieces) * 8 + 127) / 128 * 128;
+    return ((size_t)ns * tf * 4 + (size_t)kRingPieces * kPieceBytes + (size_t)(ng + kRingPieces) * 8 + 127) / 128 * 128;
 }
-__host__ __device__ constexpr size_t ring_smem_bytes(int vpl, int ns, int ng)
+__host__ __device__ constexpr size_t ring_smem_bytes(int tf, int ns, int ng)
 {
-    return ring_warp_bytes(vpl, ns, ng) * kRingWarps + 128;
+    return ring_warp_bytes(tf, ns, ng) * kRingWarps + 128;
 }
+
+// What one lane holds of a row tile of TF floats: one float2 (64-float slices, 256 B), one float4 (128 floats) or
+// two float4 (256 floats; the second 512 B further on).
+template <int TF> struct RingLane { typedef float4 V; static constexpr int NV = TF / 128; };
+template <> struct RingLane<64> { typedef float2 V; static constexpr int NV = 1; };
 
 // runtime-indexed access to a tiny register array (compare chain instead of local memory)
 template <int N>
@@ -132,7 +141,7 @@ __device__ __forceinline__ void reg_set(uint32_t (&a)[N], int i, uint32_t v)
     for (int k = 0; k < N; ++k) a[k] = (i == k) ? v : a[k];
 }
 
-// VPL : 128-float vector groups per row (tile of f).
+// TF  : floats per row tile (64, 128 or 256; f is walked in f / TF tiles, each one row slot wide).
 // G   : edges per completion group (8, 16 or 32); NG: groups in the ring (2 or 4); the warp owns NS = G * NG row slots.
 // MODE: 0 = 1-D TMA bulk copies (UBLKCP, one per row), 1 = per-lane 16-byte cp.async (LDGSTS + wait_group),
 //       2 = 2-D tensor-map TMA in tile mode (UTMALDG.2D, one row per instruction; own and halo rows through
@@ -149,27 +158,36 @@ __device__ __forceinline__ void reg_set(uint32_t (&a)[N], int i, uint32_t v)
 //             8 edges; a row-end test per edge only in groups whose row-end mask is non-zero.
 // Pieces stay resident until their last group has been CONSUMED (the values are read at consumption time), so
 // nothing is copied between issue and consumption except the row-end mask, which travels in a register.
-template <int VPL, int G, int NG, int MODE, bool HALO>
+//
+// Work item w = (tile w / nblocks, row block w % nblocks). Persistent CTAs take items from ONE counter, so the tiles
+// run one after the other: while tile t is gathered only that tile of H (TF / f of it) competes for L2, which
+// is what makes 64-float slices pay (a 256-byte slice of a row is twice as likely to still be in L2 as a 512-byte
+// row). Each output element sums the same products in the same order whatever TF is: results are bit-identical.
+template <int TF, int G, int NG, int MODE, bool HALO>
 __device__ __forceinline__ void ring_body(const SpmmArgs& a, const RingArgs& ra, const CUtensorMap* tm0, const CUtensorMap* tm1)
 {
+    typedef typename RingLane<TF>::V V;
+    constexpr int NV = RingLane<TF>::NV;
     constexpr int NS = G * NG, NP = kRingPieces;
     constexpr int PG = 32 / G;                                           // groups per index piece
     constexpr int U = (NG > PG) ? NG / PG : 1;                           // pieces per loop body (body groups % NG == 0)
-    constexpr uint32_t RB = VPL * 512;                                   // bytes of one row tile
+    constexpr uint32_t RB = TF * 4;                                      // bytes of one row tile
+    constexpr int RV = RB / sizeof(V);                                   // lane vectors per row slot
     constexpr uint32_t FULL = (G == 32) ? 0xffffffffu : ((1u << G) - 1u);
     static_assert((G == 8 || G == 16 || G == 32) && (NG == 2 || NG == 4), "unsupported ring shape");
     static_assert((U * PG) % NG == 0, "slot groups must repeat with the loop body");
     static_assert(NP * 32 >= NS + 64, "pieces must stay resident from prefetch to consumption");
+    static_assert(MODE != 1 || TF >= 128, "the cp.async fill copies 16 bytes per lane");
     extern __shared__ __align__(128) unsigned char ring_smem[];
 
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    unsigned char* wbase = ring_smem + (size_t)warp * ring_warp_bytes(VPL, NS, NG);
+    unsigned char* wbase = ring_smem + (size_t)warp * ring_warp_bytes(TF, NS, NG);
     const uint32_t s_data = smem_u32(wbase);                             // NS slots of RB bytes
     const uint32_t s_idx = s_data + NS * RB;                             // NP pieces
     const uint32_t s_gbar = s_idx + NP * kPieceBytes;                    // NG group barriers
     const uint32_t s_pbar = s_gbar + NG * 8;                             // NP piece barriers
     const int* idx_gen = reinterpret_cast<const int*>(wbase + (size_t)NS * RB);
-    const float4* data_gen = reinterpret_cast<const float4*>(wbase) + lane;
+    const V* data_gen = reinterpret_cast<const V*>(wbase) + lane;
 
     if (lane == 0) {
 #pragma unroll
@@ -181,29 +199,33 @@ __device__ __forceinline__ void ring_body(const SpmmArgs& a, const RingArgs& ra,
 
     const unsigned long long pol_hot = l2_policy_evict_last();
     const unsigned long long pol_cold = l2_policy_evict_first();
-    // blockIdx.y walks feature tiles of 128 * VPL floats (f = 384, 512, ...): row pitch f * 4, tile offset y * RB
+    // row pitch f * 4; tile t covers floats [t TF, t TF + TF)
     const size_t pitch = (size_t)a.f * 4;
-    const size_t toff = (size_t)blockIdx.y * RB;
-    const char* hb0 = reinterpret_cast<const char*>(a.H0) + toff;
-    const char* hb1 = HALO ? reinterpret_cast<const char*>(a.H1) + toff - (size_t)a.split * pitch : hb0;
     const unsigned usplit = HALO ? (unsigned)a.split : 0xffffffffu;
-    unsigned int* counter = ra.counter ? ra.counter + blockIdx.y : nullptr;
+    unsigned int* counter = ra.counter;
+    const int nitems = a.nblocks * (a.f / TF);
 
     uint32_t gpar = 0;                   // phase parity of each group barrier (bit sg)
     // pieces move through the NP slots as a FIFO: fetched -> landed (issue side) -> consumed
     uint32_t pfetch = 0, pwait = 0, pcons = 0;
 
-    float4 acc[VPL];
+    V acc[NV];
 #pragma unroll
-    for (int v = 0; v < VPL; ++v) acc[v] = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int v = 0; v < NV; ++v) acc[v] = vzero((V*)nullptr);
 
-    int blk = counter ? 0 : (int)(blockIdx.x * kRingWarps + warp);
+    // without a counter: one item per warp, tile blockIdx.y
+    int w = (int)(blockIdx.x * kRingWarps + warp);
+    w = w < a.nblocks ? (int)blockIdx.y * a.nblocks + w : nitems;
     if (counter) {
-        if (lane == 0) blk = (int)atomicAdd(counter, 1u);
-        blk = __shfl_sync(0xffffffffu, blk, 0);
+        if (lane == 0) w = (int)atomicAdd(counter, 1u);
+        w = __shfl_sync(0xffffffffu, w, 0);
     }
 
-    while (blk < a.nblocks) {
+    while (w < nitems) {
+        const int tile = w / a.nblocks, blk = w - tile * a.nblocks;
+        const size_t toff = (size_t)tile * RB;
+        const char* hb0 = reinterpret_cast<const char*>(a.H0) + toff;
+        const char* hb1 = HALO ? reinterpret_cast<const char*>(a.H1) + toff - (size_t)a.split * pitch : hb0;
         const int4 b = __ldg(a.blocks + blk);
         const bool seg = b.y < 0;
         const int e0 = b.z, e1 = b.w;
@@ -240,14 +262,18 @@ __device__ __forceinline__ void ring_body(const SpmmArgs& a, const RingArgs& ra,
             fetch_piece();
         };
         auto flush_row = [&]() {
-            ring_store_row<VPL>(acc[0], acc[VPL - 1], a.rowids, row, a.Z0, a.Z1, a.zsplit, pitch, toff + lane * 16, a.beta, a.relu, a.final);
+            ring_store_row<V, NV>(acc[0], acc[NV - 1], a.rowids, row, a.Z0, a.Z1, a.zsplit, pitch, toff + lane * sizeof(V), a.beta,
+                                  a.relu, a.final);
 #pragma unroll
-            for (int v = 0; v < VPL; ++v) acc[v] = make_float4(0.f, 0.f, 0.f, 0.f);
+            for (int v = 0; v < NV; ++v) acc[v] = vzero((V*)nullptr);
             ++row;
         };
         // issue the group at sub-position qs of piece `pi` into slot group sg; vm = valid entries (FULL inside the block)
         auto issue = [&](int qs, int sg, uint32_t vm) {
-            const uint2 m = *reinterpret_cast<const uint2*>(pi + 64);    // {row-end mask, cold mask} of the piece
+            // {row-end mask, cold mask} of the piece; 64-float slices use the cold mask of their own (larger) hot set
+            uint2 m;
+            if (TF == 64) { const uint4 q = *reinterpret_cast<const uint4*>(pi + 64); m = make_uint2(q.x, q.z); }
+            else m = *reinterpret_cast<const uint2*>(pi + 64);
             const uint32_t em = seg ? 0u : ((m.x >> (qs * G)) & vm);
             const uint32_t cm = (m.y >> (qs * G)) & FULL;
             reg_set(emask, sg, em);
@@ -260,7 +286,7 @@ __device__ __forceinline__ void ring_body(const SpmmArgs& a, const RingArgs& ra,
                         const unsigned cj = (unsigned)cols[j];
                         const char* src = (cj >= usplit ? hb1 : hb0) + (size_t)cj * pitch + lane * 16;
 #pragma unroll
-                        for (int v = 0; v < VPL; ++v)
+                        for (int v = 0; v < NV; ++v)
                             cp_async16(s_data + (sg * G + j) * RB + v * 512 + lane * 16, src + v * 512,
                                        (cm >> j & 1) ? pol_cold : pol_hot);
                     }
@@ -274,7 +300,7 @@ __device__ __forceinline__ void ring_body(const SpmmArgs& a, const RingArgs& ra,
                 const bool halo = cj >= usplit;
                 const unsigned long long pol = (cm >> lane & 1) ? pol_cold : pol_hot;
                 if (MODE == 2)
-                    tma_row(s_data + (sg * G + lane) * RB, halo ? tm1 : tm0, (int)(blockIdx.y * (RB / 4)),
+                    tma_row(s_data + (sg * G + lane) * RB, halo ? tm1 : tm0, tile * TF,
                             (int)(halo ? cj - usplit : cj), s_gbar + sg * 8, pol);
                 else
                     bulk_g2s(s_data + (sg * G + lane) * RB, (halo ? hb1 : hb0) + (size_t)cj * pitch, RB, s_gbar + sg * 8, pol);
@@ -290,29 +316,29 @@ __device__ __forceinline__ void ring_body(const SpmmArgs& a, const RingArgs& ra,
             if (MODE != 1) { mbar_wait(s_gbar + sg * 8, (gpar >> sg) & 1); gpar ^= 1u << sg; }
             else cp_async_wait<NG - 1>();
             const uint32_t em = reg_get(emask, sg);
-            const float4* slot = data_gen + (size_t)(sg * G) * (RB / 16);
+            const V* slot = data_gen + (size_t)(sg * G) * RV;
             const float* wv = reinterpret_cast<const float*>(pc) + 32 + qs * G;
             if (vm == FULL) {
 #pragma unroll
-                for (int c = 0; c < G; c += 8) {                         // 8 rows at a time: 8 x LDS.128 in flight
+                for (int c = 0; c < G; c += 8) {                         // 8 rows at a time: 8 x LDS.64 / LDS.128 in flight
                     const float4 wa = *reinterpret_cast<const float4*>(wv + c);
                     const float4 wb = *reinterpret_cast<const float4*>(wv + c + 4);
                     const float w[8] = {wa.x, wa.y, wa.z, wa.w, wb.x, wb.y, wb.z, wb.w};
-                    float4 r[8][VPL];
+                    V r[8][NV];
 #pragma unroll
                     for (int j = 0; j < 8; ++j)
 #pragma unroll
-                        for (int v = 0; v < VPL; ++v) r[j][v] = slot[(c + j) * (RB / 16) + v * 32];
-                    if (((em >> c) & 0xffu) == 0) {                      // no row end inside: 8 x (LDS.128, 4 FFMA)
+                        for (int v = 0; v < NV; ++v) r[j][v] = slot[(c + j) * RV + v * 32];
+                    if (((em >> c) & 0xffu) == 0) {                      // no row end inside: 8 x (LDS, TF / 32 FFMA)
 #pragma unroll
                         for (int j = 0; j < 8; ++j)
 #pragma unroll
-                            for (int v = 0; v < VPL; ++v) vfma(acc[v], w[j], r[j][v]);
+                            for (int v = 0; v < NV; ++v) vfma(acc[v], w[j], r[j][v]);
                     } else {
 #pragma unroll
                         for (int j = 0; j < 8; ++j) {
 #pragma unroll
-                            for (int v = 0; v < VPL; ++v) vfma(acc[v], w[j], r[j][v]);
+                            for (int v = 0; v < NV; ++v) vfma(acc[v], w[j], r[j][v]);
                             if (em >> (c + j) & 1) flush_row();
                         }
                     }
@@ -323,7 +349,7 @@ __device__ __forceinline__ void ring_body(const SpmmArgs& a, const RingArgs& ra,
                     if (vm >> j & 1) {
                         const float wj = wv[j];
 #pragma unroll
-                        for (int v = 0; v < VPL; ++v) vfma(acc[v], wj, slot[j * (RB / 16) + v * 32]);
+                        for (int v = 0; v < NV; ++v) vfma(acc[v], wj, slot[j * RV + v * 32]);
                         if (em >> j & 1) flush_row();
                     }
                 }
@@ -385,33 +411,33 @@ __device__ __forceinline__ void ring_body(const SpmmArgs& a, const RingArgs& ra,
         if (seg) {
             char* pb = reinterpret_cast<char*>(a.partial) + (size_t)(unsigned)(-b.y - 1) * pitch + toff;
 #pragma unroll
-            for (int v = 0; v < VPL; ++v) {
-                reinterpret_cast<float4*>(pb + v * 512)[lane] = acc[v];
-                acc[v] = make_float4(0.f, 0.f, 0.f, 0.f);
+            for (int v = 0; v < NV; ++v) {
+                reinterpret_cast<V*>(pb + v * 512)[lane] = acc[v];
+                acc[v] = vzero((V*)nullptr);
             }
         }
 
         if (!counter) break;
-        if (lane == 0) blk = (int)atomicAdd(counter, 1u);
-        blk = __shfl_sync(0xffffffffu, blk, 0);
+        if (lane == 0) w = (int)atomicAdd(counter, 1u);
+        w = __shfl_sync(0xffffffffu, w, 0);
     }
     if (MODE == 1) cp_async_wait<0>();
 }
 
-template <int VPL, int G, int NG, int MODE, bool HALO>
+template <int TF, int G, int NG, int MODE, bool HALO>
 __global__ void __launch_bounds__(kRingWarps * 32)
 spmm_ring_kernel(const SpmmArgs a, const RingArgs ra)
 {
-    ring_body<VPL, G, NG, MODE, HALO>(a, ra, nullptr, nullptr);
+    ring_body<TF, G, NG, MODE, HALO>(a, ra, nullptr, nullptr);
 }
 
 // tensor-map variant: the tensor maps of H_own (tm0) and of the halo slab (tm1) travel as __grid_constant__ parameters
-template <int VPL, int G, int NG, bool HALO>
+template <int TF, int G, int NG, bool HALO>
 __global__ void __launch_bounds__(kRingWarps * 32)
 spmm_ring_tm_kernel(const SpmmArgs a, const RingArgs ra, const __grid_constant__ CUtensorMap tm0,
                     const __grid_constant__ CUtensorMap tm1)
 {
-    ring_body<VPL, G, NG, 2, HALO>(a, ra, &tm0, &tm1);
+    ring_body<TF, G, NG, 2, HALO>(a, ra, &tm0, &tm1);
 }
 
 }  // namespace pgcn

@@ -5,6 +5,7 @@
     python tools/tune_spmm.py --config C2 --sweep default
     python tools/tune_spmm.py --config C2 --single edges_per_block=256,tile_floats=0 --iters 5   (for ncu)
     python tools/tune_spmm.py --gather-sweep        (L2 capacity / bandwidth probe with windowed columns)
+    python tools/tune_spmm.py --config C2 --sweep slices   (ring row tile: full width vs 64-float slices)
 """
 import argparse
 import itertools
@@ -77,11 +78,11 @@ def main():
             A = sp.coo_matrix((np.ones(n * d, dtype=np.float32), (row, col)), shape=(n, n))
             p = planmod.build_plan(A, np.zeros(n, dtype=np.int64), 0, 1, f, device=dev)
             H = torch.rand((n, f), device=dev); Z = torch.empty((n, f), device=dev)
-            for tile, unroll in ((0, 0), (32, 0)):
-                p.set_option("tile_floats", tile)
+            for tile in (0, 64):                 # ring row tile: full width, 64-float slices
+                p.set_option("ring_tile_floats", tile)
                 med, mn = timed(lambda: cabi.check(lib.pgcn_spmm(p.handle, 0, H.data_ptr(), None, Z.data_ptr(), None, f, stream), p.handle), args.iters)
                 nnz = p.lp.nnz()
-                emit({"probe": "gather", "window_rows": W, "window_MB": W * f * 4 / 1e6, "tile_floats": tile, "unroll": unroll, "ms": med,
+                emit({"probe": "gather", "window_rows": W, "window_MB": W * f * 4 / 1e6, "ring_tile_floats": tile, "ms": med,
                       "gather_GBs": nnz * f * 4 / med / 1e6, "edges_per_s": nnz / med * 1e3})
             p.close()
         return
@@ -146,6 +147,9 @@ def main():
             point({"kernel": kern, "ring_slots": slots, "ring_groups": groups, "ring_edges_per_block": epb, "persistent": 1})
         point({"kernel": 7, "ring_slots": 32, "ring_groups": 2, "ring_edges_per_block": 512, "persistent": 0})
         point({"kernel": 6, "ring_slots": 16, "ring_groups": 2, "ring_edges_per_block": 512, "persistent": 1})
+    elif args.sweep == "slices":
+        for tile, slots, epb in itertools.product((0, 64), (16, 32, 64), (256, 512, 1024)):
+            point({"ring_tile_floats": tile, "ring_slots": slots, "ring_edges_per_block": epb})
     elif args.sweep == "ring-small":
         point({"kernel": 4})
         for kern, slots, epb, pers in ((5, 32, 1024, 0), (5, 16, 1024, 0), (5, 32, 2048, 1), (6, 32, 1024, 0), (6, 16, 1024, 0)):
