@@ -119,7 +119,8 @@ int pgcn_plan_destroy(pgcn_plan* plan);
  * ring depth explicitly clears the tuned values, a non-zero "ring_tile_floats" overrides the tuned width. "hot_mb" (L2-resident hot set of H rows) is fixed at plan creation: environment variable PGCN_HOT_MB.
  * Split rows are always reduced in a fixed order: results are run-to-run deterministic.
  * Read-only names for pgcn_plan_get_option: "nccl", "blocks_fwd", "long_rows_fwd", "ring_blocks_fwd",
- * "ring_long_rows_fwd".
+ * "ring_long_rows_fwd", "retired_schedules" (see pgcn_plan_prepare), "epoch" (the peer transport's exchange epoch =
+ * fused calls over peer memory so far; a synchronous device read, not to be called while a stream is captured).
  */
 int pgcn_plan_set_option(pgcn_plan* plan, const char* name, int64_t value);
 int64_t pgcn_plan_get_option(const pgcn_plan* plan, const char* name);
@@ -130,6 +131,22 @@ int64_t pgcn_plan_get_option(const pgcn_plan* plan, const char* name);
  * GPU/PGCN.py:171-200). Synchronous. Returns the chosen value (>0) or a negative pgcn_status.
  */
 int pgcn_plan_autotune(pgcn_plan* plan, int32_t f);
+
+/*
+ * CUDA graphs. Synchronous set-up work for width f under the current options: builds every row-block schedule the
+ * fused calls can use at f (register and ring kernel: which one runs depends on the operands' alignment), sets every
+ * ring kernel instance's shared-memory attribute and occupancy, and loads the kernels. Afterwards pgcn_forward and
+ * pgcn_backward at width f make only stream-ordered CUDA calls and can be captured (cudaStreamBeginCapture,
+ * torch.cuda.graph). A call that would still need set-up work while its stream is being captured returns
+ * PGCN_ERR_STATE, before any unsafe call, and names this function; change f or an option, then prepare again.
+ * Schedules replaced after the first prepare (a new option, pgcn_plan_autotune) are kept until pgcn_plan_destroy,
+ * so a graph captured earlier never reads freed memory (read-only option "retired_schedules" counts them).
+ * A captured graph fixes f, the options, the "relu" epilogue and the operand addresses of the capture: replay it on
+ * new inputs by copying them into the captured buffers. The peer transport's exchange epoch lives in device memory
+ * and advances with every replay, so eager calls and replays may be mixed in any order, as long as all ranks make
+ * the same sequence of fused calls. pgcn_launch_count does not count replays.
+ */
+int pgcn_plan_prepare(pgcn_plan* plan, int32_t f);
 
 /*
  * Host-only (no GPU needed): the row-block schedule the SpMM walks, for inspection and tests.

@@ -16,7 +16,7 @@ NCCL_ID_BYTES = 128
 SYMBOLS = [
     "pgcn_version", "pgcn_device_count", "pgcn_last_error",
     "pgcn_plan_create", "pgcn_plan_destroy", "pgcn_plan_set_option", "pgcn_plan_get_option",
-    "pgcn_plan_autotune", "pgcn_debug_schedule", "pgcn_plan_slab", "pgcn_algorithmic_bytes", "pgcn_launch_count",
+    "pgcn_plan_autotune", "pgcn_plan_prepare", "pgcn_debug_schedule", "pgcn_plan_slab", "pgcn_algorithmic_bytes", "pgcn_launch_count",
     "pgcn_comm_unique_id", "pgcn_comm_init", "pgcn_comm_share", "pgcn_p2p_export", "pgcn_p2p_import",
     "pgcn_spmm", "pgcn_pack", "pgcn_exchange", "pgcn_unpack_add",
     "pgcn_forward", "pgcn_backward", "pgcn_forward_host", "pgcn_forward_host_async", "pgcn_forward_host_wait",
@@ -71,6 +71,8 @@ def load(build_if_missing=True):
     lib.pgcn_plan_get_option.argtypes = [vp, C.c_char_p]
     lib.pgcn_plan_autotune.restype = C.c_int
     lib.pgcn_plan_autotune.argtypes = [vp, i32]
+    lib.pgcn_plan_prepare.restype = C.c_int
+    lib.pgcn_plan_prepare.argtypes = [vp, i32]
     lib.pgcn_debug_schedule.restype = i64
     lib.pgcn_debug_schedule.argtypes = [vp, i32, i64, i64, vp, i64, vp, vp]
     lib.pgcn_plan_slab.restype = vp

@@ -171,7 +171,16 @@ struct pgcn_plan {
     void* peer_arena[kMaxPeers] = {nullptr};
     bool peer_local[kMaxPeers] = {false};   // peer lives in THIS process (same-process plans: no IPC mapping)
     P2PBlob peer_blob[kMaxPeers];
-    unsigned long long epoch = 0;
+    // exchange epoch of the peer transport, in device memory: advanced on the caller's stream by every fused multi-rank
+    // call over peer memory, read there by the kernels (flag value, parity of the double-buffered slabs), so a CUDA
+    // graph replay uses the epoch of the replay
+    unsigned long long* d_epoch = nullptr;
+
+    // pgcn_plan_prepare has run: schedules replaced from then on are retired instead of freed (a captured graph may
+    // still read them) and released by pgcn_plan_destroy
+    bool prepared = false;
+    std::vector<void*> retired;
+    int64_t nretired = 0;
 
     // host-buffer variant: two device slots, copy-in / compute / copy-out streams chained by events
     float* d_hostH[2] = {nullptr, nullptr}; float* d_hostZ[2] = {nullptr, nullptr}; int64_t host_cap = 0;
@@ -343,17 +352,28 @@ void make_schedule(const int* rp, int nrows_c, int64_t epb, int64_t long_row,
     close(nrows_c);
 }
 
+bool sched_ready(const DevCsr& c, int which, int64_t epb, int64_t long_row)
+{
+    return c.sched[which].epb == epb && c.sched[which].long_row == long_row;
+}
+
 int build_schedule(pgcn_plan* p, DevCsr& c, int which, int64_t epb, int64_t long_row)
 {
     DevCsr::Sched& sc = c.sched[which];
-    if (sc.epb == epb && sc.long_row == long_row) return 0;
+    if (sched_ready(c, which, epb, long_row)) return 0;
 
     std::vector<int4> blocks, longs;
     int nslots = 0;
     make_schedule(c.h_rowptr.data(), c.nrows_c, epb, long_row, blocks, longs, nslots,
                   which == 1 ? (1 << 30) : kMaxRowsPerBlock, c.row_base);
 
-    cudaFree(sc.d_blocks); cudaFree(sc.d_long); cudaFree(sc.d_partial);
+    if (p->prepared && sc.epb >= 0) {
+        // a graph captured after pgcn_plan_prepare may still launch the old schedule: keep it until pgcn_plan_destroy
+        p->retired.insert(p->retired.end(), {(void*)sc.d_blocks, (void*)sc.d_long, (void*)sc.d_partial});
+        ++p->nretired;
+    } else {
+        cudaFree(sc.d_blocks); cudaFree(sc.d_long); cudaFree(sc.d_partial);
+    }
     sc.d_blocks = nullptr; sc.d_long = nullptr; sc.d_partial = nullptr;
     int rc;
     if ((rc = upload(p, &sc.d_blocks, blocks.data(), blocks.size()))) return rc;
@@ -412,7 +432,7 @@ spmm_fn pick_lpe(int lpe, int vpl, bool halo)
 }
 
 typedef void (*ring_fn)(const SpmmArgs, const RingArgs);
-typedef void (*ring_tm_fn)(const SpmmArgs, const RingArgs, const CUtensorMap, const CUtensorMap);
+typedef void (*ring_tm_fn)(const SpmmArgs, const RingArgs, const CUtensorMap, const CUtensorMap, const CUtensorMap);
 
 // cuTensorMapEncodeTiled, resolved through the runtime (no link-time dependency on libcuda)
 typedef CUresult (*encode_tiled_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -511,7 +531,7 @@ void preload_kernels()
     touch_kernel(spmm_fixup_kernel<4>); touch_kernel(spmm_fixup_kernel<1>);
     touch_kernel(pack_rows_kernel<4>); touch_kernel(pack_rows_kernel<1>);
     touch_kernel(unpack_add_kernel<4>); touch_kernel(unpack_add_kernel<1>);
-    touch_kernel(put_rows_kernel<4>); touch_kernel(p2p_wait_kernel);
+    touch_kernel(put_rows_kernel<4>); touch_kernel(p2p_wait_kernel); touch_kernel(epoch_advance_kernel);
 }
 
 bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
@@ -524,21 +544,64 @@ bool use_ring(const pgcn_plan* p, const float* H0, const float* H1, int f)
     return f % 128 == 0 && aligned16(H0) && aligned16(H1);
 }
 
+// Block size and long-row threshold of matrix c's schedule for the ring (or register) kernel under the current options.
+void sched_params(const pgcn_plan* p, const DevCsr& c, bool ring, int64_t* epb, int64_t* long_row)
+{
+    if (ring) {
+        *epb = std::max<int64_t>(c.tuned_epb[1] > 0 ? c.tuned_epb[1] : p->opt_ring_epb, 64);
+        *long_row = p->opt_ring_long > 0 ? p->opt_ring_long : 2 * *epb;
+    } else {
+        *epb = std::max<int64_t>(c.tuned_epb[0] > 0 ? c.tuned_epb[0] : p->opt_epb, 8);
+        *long_row = p->opt_long > 0 ? p->opt_long : 4 * *epb;
+    }
+}
+
+// A stream under CUDA graph capture takes only stream-ordered work. Set-up that would allocate, copy synchronously or
+// set a function attribute is refused before any such call, so the caller's capture stays valid.
+int refuse_under_capture(pgcn_plan* p, cudaStream_t st)
+{
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    const cudaError_t e = cudaStreamIsCapturing(st, &cs);
+    if (e == cudaSuccess && cs == cudaStreamCaptureStatusNone) return 0;
+    if (e != cudaSuccess) cudaGetLastError();
+    return fail(p, PGCN_ERR_STATE, "this call needs set-up work (schedule upload or kernel attributes) that cannot run "
+                "while the stream is being captured into a CUDA graph: call pgcn_plan_prepare(plan, f) before capturing");
+}
+
+// Opt a ring kernel instance in to its dynamic shared memory (> 48 KB) and record its occupancy, once per plan.
+int ring_attr(pgcn_plan* p, int tf, int shape, int mode, bool halo, cudaStream_t st, int* slot_out, size_t* smem_out)
+{
+    const int g = kRingShapes[shape].g, ng = kRingShapes[shape].ng;
+    const size_t smem = ring_smem_bytes(tf, g * ng, ng);
+    const int tslot = tf == 64 ? 0 : (tf == 128 ? 1 : 2);
+    const int slot = ((tslot * 4 + shape) * 3 + mode) * 2 + (halo ? 1 : 0);
+    if (slot_out) *slot_out = slot;
+    if (smem_out) *smem_out = smem;
+    if (p->ring_attr_set[slot]) return 0;
+    int rc = refuse_under_capture(p, st);
+    if (rc) return rc;
+    const void* fptr = mode == 2 ? (const void*)pick_ring_tm(tf, shape, halo) : (const void*)pick_ring(tf, shape, mode, halo);
+    CU(p, cudaFuncSetAttribute(fptr, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int nb = 0;
+    CU(p, cudaOccupancyMaxActiveBlocksPerMultiprocessorWithFlags(&nb, fptr, kRingWarps * 32, smem, 0));
+    p->ring_ctas_per_sm[slot] = std::max(nb, 1);
+    p->ring_attr_set[slot] = true;
+    return 0;
+}
+
+// H_odd: the halo slab of odd exchange epochs when the operand that holds the halo slab (H1, or H0 without H1) is the
+// peer transport's double-buffered slab; the kernels then pick the buffer from the plan's device epoch.
 int launch_spmm(pgcn_plan* p, DevCsr& c, const float* H0, const float* H1, int split,
-                float* Z0, float* Z1, int zsplit, int f, int beta, cudaStream_t st, int relu = 0, bool use_final = false)
+                float* Z0, float* Z1, int zsplit, int f, int beta, cudaStream_t st, int relu = 0, bool use_final = false,
+                const float* H_odd = nullptr)
 {
     if (c.nrows == 0) return 0;
-    const bool ring = use_ring(p, H0, H1, f) && aligned16(Z0) && aligned16(Z1);
+    const bool ring = use_ring(p, H0, H1, f) && aligned16(Z0) && aligned16(Z1) && (!H_odd || aligned16(H_odd));
     int64_t epb, long_row;
-    if (ring) {
-        epb = std::max<int64_t>(c.tuned_epb[1] > 0 ? c.tuned_epb[1] : p->opt_ring_epb, 64);
-        long_row = p->opt_ring_long > 0 ? p->opt_ring_long : 2 * epb;
-    } else {
-        epb = std::max<int64_t>(c.tuned_epb[0] > 0 ? c.tuned_epb[0] : p->opt_epb, 8);
-        long_row = p->opt_long > 0 ? p->opt_long : 4 * epb;
-    }
-    int rc = build_schedule(p, c, ring ? 1 : 0, epb, long_row);
-    if (rc) return rc;
+    sched_params(p, c, ring, &epb, &long_row);
+    int rc;
+    if (!sched_ready(c, ring ? 1 : 0, epb, long_row) && (rc = refuse_under_capture(p, st))) return rc;
+    if ((rc = build_schedule(p, c, ring ? 1 : 0, epb, long_row))) return rc;
     const DevCsr::Sched& sc = c.sched[ring ? 1 : 0];
     const TileCfg t = choose_tile(p, f);
     if (c.nempty > 0 && !beta) {
@@ -558,6 +621,7 @@ int launch_spmm(pgcn_plan* p, DevCsr& c, const float* H0, const float* H1, int s
     a.rowids = c.d_rowids;
     a.partial = sc.d_partial; a.f = f; a.beta = beta;
     a.relu = relu; a.final = (relu && use_final) ? c.d_final : nullptr;
+    a.H_odd = H_odd; a.epoch = H_odd ? p->d_epoch : nullptr;
     if (sc.nblocks > 0 && ring) {
         int mode = p->opt_kernel == 6 ? 1 : (p->opt_kernel == 5 ? 0 : 2);   // default: 2-D tensor-map TMA
         // row tile: the option, else the tuned width, else the full width (256 floats when f allows, else 128);
@@ -570,31 +634,23 @@ int launch_spmm(pgcn_plan* p, DevCsr& c, const float* H0, const float* H1, int s
         // ring shape from the options: ring_slots = 16 | 32 | 64, ring_groups = 2 | 4 (only with 64 slots)
         const int64_t want_slots = c.tuned_slots > 0 ? c.tuned_slots : p->opt_ring_slots;
         int shape = want_slots <= 16 ? 0 : (want_slots <= 32 ? 1 : (p->opt_ring_groups == 4 ? 3 : 2));
-        CUtensorMap tm0, tm1;
+        CUtensorMap tm0, tm1, tm_odd;
         if (mode == 2) {
             // H0 holds the columns below `split` (all of them when there is no halo slab), H1 the rest
             bool ok = make_row_map(&tm0, H0, 1 << 30, f, tf, 1);
             if (ok && H1) ok = make_row_map(&tm1, H1, 1 << 30, f, tf, 1);
             else if (ok) tm1 = tm0;
+            if (ok && H_odd) ok = make_row_map(&tm_odd, H_odd, 1 << 30, f, tf, 1);
+            else if (ok) tm_odd = tm1;
             if (!ok) mode = 0;                                   // no driver entry point: 1-D bulk copies
         }
         if (mode == 1) shape = 0;
         if (mode == 0 && shape > 1) shape = 1;
-        const int g = kRingShapes[shape].g, ng = kRingShapes[shape].ng;
         ring_fn fn = mode == 2 ? nullptr : pick_ring(tf, shape, mode, halo);
         ring_tm_fn fn_tm = mode == 2 ? pick_ring_tm(tf, shape, halo) : nullptr;
-        const void* fptr = mode == 2 ? (const void*)fn_tm : (const void*)fn;
-        const size_t smem = ring_smem_bytes(tf, g * ng, ng);
-        // opt-in to > 48 KB of dynamic shared memory, once per kernel instance
-        const int tslot = tf == 64 ? 0 : (tf == 128 ? 1 : 2);
-        const int slot = ((tslot * 4 + shape) * 3 + mode) * 2 + (halo ? 1 : 0);
-        if (!p->ring_attr_set[slot]) {
-            CU(p, cudaFuncSetAttribute(fptr, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            int nb = 0;
-            CU(p, cudaOccupancyMaxActiveBlocksPerMultiprocessorWithFlags(&nb, fptr, kRingWarps * 32, smem, 0));
-            p->ring_ctas_per_sm[slot] = std::max(nb, 1);
-            p->ring_attr_set[slot] = true;
-        }
+        int slot = 0;
+        size_t smem = 0;
+        if ((rc = ring_attr(p, tf, shape, mode, halo, st, &slot, &smem))) return rc;
         RingArgs ra;
         ra.counter = nullptr; ra.hub = nullptr; ra.nhub = 0;
         dim3 grid((unsigned)((sc.nblocks + kRingWarps - 1) / kRingWarps), (unsigned)tiles);
@@ -612,7 +668,7 @@ int launch_spmm(pgcn_plan* p, DevCsr& c, const float* H0, const float* H1, int s
             grid.x = std::min<unsigned>(items, (unsigned)(p->num_sms * p->ring_ctas_per_sm[slot]));
             grid.y = 1;
         }
-        if (mode == 2) fn_tm<<<grid, kRingWarps * 32, smem, st>>>(a, ra, tm0, tm1);
+        if (mode == 2) fn_tm<<<grid, kRingWarps * 32, smem, st>>>(a, ra, tm0, tm1, tm_odd);
         else fn<<<grid, kRingWarps * 32, smem, st>>>(a, ra);
         ++p->launches;
     } else if (sc.nblocks > 0) {
@@ -665,12 +721,14 @@ int launch_pack(pgcn_plan* p, const float* H, float* slab, int f, cudaStream_t s
     return 0;
 }
 
-int launch_unpack(pgcn_plan* p, const float* recv, float* G, int f, cudaStream_t st)
+// recv_odd: the reverse slab of odd exchange epochs when `recv` is the peer transport's double-buffered slab
+int launch_unpack(pgcn_plan* p, const float* recv, float* G, int f, cudaStream_t st, const float* recv_odd = nullptr)
 {
     if (p->nb == 0) return 0;
     UnpackArgs a;
     a.brow = p->d_brow; a.bptr = p->d_bptr; a.bpos = p->d_bpos; a.nb = p->nb;
     a.recv = recv; a.G = G; a.f = f;
+    a.recv_odd = recv_odd; a.epoch = recv_odd ? p->d_epoch : nullptr;
     const int vw = (f % 4 == 0) ? 4 : 1;
     const long long total = (long long)p->nb * (f / vw);
     const unsigned grid = (unsigned)((total + 255) / 256);
@@ -709,21 +767,23 @@ unsigned long long* flag_slot(void* arena, int64_t off_flags, int slot)
 
 // Fused put of the rows bound for peer `dst` + epoch signal (peer-memory transport). `reverse`: halo partials of
 // A^T g back to their owner (rows already in wire order), else boundary rows of H gathered through send_idx.
-int p2p_put(pgcn_plan* p, int dst, const float* src, int f, bool reverse, int par, cudaStream_t st)
+int p2p_put(pgcn_plan* p, int dst, const float* src, int f, bool reverse, cudaStream_t st)
 {
     PutArgs a;
     const P2PBlob& pb = p->peer_blob[dst];
+    for (int par = 0; par < 2; ++par) {                 // the kernel picks the slab of this call's epoch parity
+        if (!reverse) a.dst[par] = arena_ptr(p->peer_arena[dst], pb.off_fwd[par]) + (size_t)pb.recv_off[p->rank] * f;
+        else a.dst[par] = arena_ptr(p->peer_arena[dst], pb.off_bwd[par]) + (size_t)pb.send_off[p->rank] * f;
+    }
     if (!reverse) {
         a.send_idx = p->d_send_idx; a.j0 = p->send_off[dst]; a.nrows = p->send_off[dst + 1] - p->send_off[dst];
-        a.dst = arena_ptr(p->peer_arena[dst], pb.off_fwd[par]) + (size_t)pb.recv_off[p->rank] * f;
     } else {
         a.send_idx = nullptr; a.j0 = p->recv_off[dst]; a.nrows = p->recv_off[dst + 1] - p->recv_off[dst];
-        a.dst = arena_ptr(p->peer_arena[dst], pb.off_bwd[par]) + (size_t)pb.send_off[p->rank] * f;
     }
     a.src = src; a.f = f;
     a.done = p->d_done + (reverse ? 32 : 0) + dst;     // kMaxPeers <= 16 destinations per direction
     a.flag = flag_slot(p->peer_arena[dst], pb.off_flags, p->rank);
-    a.epoch = p->epoch;
+    a.epoch = p->d_epoch;
     // enough CTAs to keep the NVLink store queues full, few enough not to crowd out the SpMM running beside it
     const long long items = a.nrows * (f / 4);
     const unsigned grid = (unsigned)std::max<long long>(1, std::min<long long>((items + 255) / 256, 4LL * p->num_sms));
@@ -735,7 +795,17 @@ int p2p_put(pgcn_plan* p, int dst, const float* src, int f, bool reverse, int pa
 
 int p2p_wait(pgcn_plan* p, int src, cudaStream_t st)
 {
-    p2p_wait_kernel<<<1, 32, 0, st>>>(flag_slot(p->arena, p->off_flags, src), p->epoch);
+    p2p_wait_kernel<<<1, 32, 0, st>>>(flag_slot(p->arena, p->off_flags, src), p->d_epoch);
+    ++p->launches;
+    CU(p, cudaGetLastError());
+    return 0;
+}
+
+// Start of a fused call over the peer transport: advance the device epoch on the caller's stream, ahead of every kernel
+// of the call (the exchange stream joins after it).
+int advance_epoch(pgcn_plan* p, cudaStream_t st)
+{
+    epoch_advance_kernel<<<1, 1, 0, st>>>(p->d_epoch);
     ++p->launches;
     CU(p, cudaGetLastError());
     return 0;
@@ -891,6 +961,8 @@ int pgcn_plan_create(const int32_t* rowptr, const int32_t* colidx, const float* 
         std::vector<unsigned int> zeros(64, 0u);
         TRY(upload(p, &p->d_counter, zeros.data(), zeros.size()));
         TRY(upload(p, &p->d_done, zeros.data(), zeros.size()));
+        const unsigned long long epoch0 = 0;
+        TRY(upload(p, &p->d_epoch, &epoch0, 1));
     }
     TRY(upload(p, &p->d_send_idx, send_idx, (size_t)S));
     // boundary CSR: for every owned row that appears in some send list, the slab positions
@@ -965,6 +1037,8 @@ int pgcn_plan_destroy(pgcn_plan* p)
     if (p->s_in) cudaStreamDestroy(p->s_in);
     if (p->s_out) cudaStreamDestroy(p->s_out);
     cudaFree(p->d_counter);
+    cudaFree(p->d_epoch);
+    for (void* q : p->retired) cudaFree(q);
     if (p->comm_stream) cudaStreamDestroy(p->comm_stream);
     if (p->host_stream) cudaStreamDestroy(p->host_stream);
     if (p->ev_a) cudaEventDestroy(p->ev_a);
@@ -1040,6 +1114,12 @@ int64_t pgcn_plan_get_option(const pgcn_plan* p, const char* name)
     if (n == "long_rows_fwd") return p->fwd.sched[0].nlong;
     if (n == "ring_blocks_fwd") return p->fwd.sched[1].nblocks;
     if (n == "ring_long_rows_fwd") return p->fwd.sched[1].nlong;
+    if (n == "retired_schedules") return p->nretired;
+    if (n == "epoch") {                                   // synchronous read (tests); not while a stream is captured
+        unsigned long long e = 0;
+        if (cudaMemcpy(&e, p->d_epoch, sizeof e, cudaMemcpyDeviceToHost) != cudaSuccess) { cudaGetLastError(); return PGCN_ERR_CUDA; }
+        return (int64_t)e;
+    }
     return PGCN_ERR_INVALID;
 }
 
@@ -1174,6 +1254,44 @@ int pgcn_plan_autotune(pgcn_plan* p, int32_t f)
     cleanup();
     const int which = use_ring(p, H0, nullptr, f) ? 1 : 0;     // H0 was cudaMalloc'ed: aligned
     return (int)(p->fwd.tuned_epb[which] > 0 ? p->fwd.tuned_epb[which] : (which ? p->opt_ring_epb : p->opt_epb));
+}
+
+// Everything a fused forward / backward at width f would otherwise set up on its first call: the schedules of every
+// matrix those calls launch, for the register kernel and (f a multiple of 128: the operands' alignment decides at
+// run time) the ring kernel; the shared-memory opt-in and occupancy of every ring instance; the kernel modules.
+int pgcn_plan_prepare(pgcn_plan* p, int32_t f)
+{
+    int rc = check_f(p, f);
+    if (rc) return rc;
+    CU(p, cudaSetDevice(p->device));
+    preload_kernels();
+    std::vector<DevCsr*> mats = {&p->fwd, &p->tr};
+    if (p->have_split) {
+        mats.push_back(&p->own);
+        mats.push_back(&p->tr_own);
+        for (auto& c : p->halo_q) mats.push_back(&c);
+        for (auto& c : p->tr_halo_q) mats.push_back(&c);
+    }
+    const bool ring = p->opt_kernel != 4 && f % 128 == 0;
+    for (DevCsr* c : mats) {
+        if (c->nrows == 0) continue;
+        for (int which = 0; which < (ring ? 2 : 1); ++which) {
+            int64_t epb, long_row;
+            sched_params(p, *c, which == 1, &epb, &long_row);
+            if ((rc = build_schedule(p, *c, which, epb, long_row))) return rc;
+        }
+    }
+    if (ring)
+        for (int tf = 64; tf <= 256; tf *= 2)
+            for (int halo = 0; halo < 2; ++halo) {
+                for (int shape = 0; shape < 4; ++shape)
+                    if ((rc = ring_attr(p, tf, shape, 2, halo != 0, p->host_stream, nullptr, nullptr))) return rc;
+                for (int shape = 0; shape < 2; ++shape)
+                    if ((rc = ring_attr(p, tf, shape, 0, halo != 0, p->host_stream, nullptr, nullptr))) return rc;
+                if (tf >= 128 && (rc = ring_attr(p, tf, 0, 1, halo != 0, p->host_stream, nullptr, nullptr))) return rc;
+            }
+    p->prepared = true;
+    return 0;
 }
 
 void* pgcn_plan_slab(pgcn_plan* p, int which)
@@ -1388,11 +1506,11 @@ int pgcn_forward(pgcn_plan* p, const float* H_own, float* Z, int32_t f, void* st
     const bool split = p->have_split && p->opt_overlap;
     const int k = p->k;
     float* halo = p->d_halo_slab;
-    int par = 0;
+    const float* halo_odd = nullptr;
     if (use_p2p) {
-        ++p->epoch;
-        par = (int)(p->epoch & 1);
-        halo = arena_ptr(p->arena, p->off_fwd[par]);
+        if ((rc = advance_epoch(p, st))) return rc;
+        halo = arena_ptr(p->arena, p->off_fwd[0]);
+        halo_odd = arena_ptr(p->arena, p->off_fwd[1]);
     }
     cudaStream_t cs = split ? p->comm_stream : st;
     if (split) {
@@ -1402,7 +1520,7 @@ int pgcn_forward(pgcn_plan* p, const float* H_own, float* Z, int32_t f, void* st
     // ---- send side (exchange stream): one peer after the other, in step order
     if (use_p2p) {
         for (int i = 1; i < k; ++i)
-            if ((rc = p2p_put(p, step_dst(p, i), H_own, f, false, par, cs))) return rc;
+            if ((rc = p2p_put(p, step_dst(p, i), H_own, f, false, cs))) return rc;
         if (split) CU(p, cudaEventRecord(p->ev_b, cs));                   // H_own is free for the caller after this
     } else {
         if ((rc = launch_pack(p, H_own, p->d_send_slab, f, cs))) return rc;
@@ -1416,7 +1534,8 @@ int pgcn_forward(pgcn_plan* p, const float* H_own, float* Z, int32_t f, void* st
         if (use_p2p)
             for (int i = 1; i < k; ++i)
                 if ((rc = p2p_wait(p, step_src(p, i), st))) return rc;
-        return launch_spmm(p, p->fwd, H_own, p->h > 0 ? halo : nullptr, p->m, Z, nullptr, p->m, f, 0, st, relu);
+        return launch_spmm(p, p->fwd, H_own, p->h > 0 ? halo : nullptr, p->m, Z, nullptr, p->m, f, 0, st, relu, false,
+                           p->h > 0 ? halo_odd : nullptr);
     }
     // ---- compute side: own columns while the rows travel, then each source's block as soon as it has landed
     if ((rc = launch_spmm(p, p->own, H_own, nullptr, p->m, Z, nullptr, p->m, f, 0, st, relu, true))) return rc;
@@ -1425,7 +1544,8 @@ int pgcn_forward(pgcn_plan* p, const float* H_own, float* Z, int32_t f, void* st
         if (use_p2p) { if ((rc = p2p_wait(p, src, st))) return rc; }
         else CU(p, cudaStreamWaitEvent(st, p->ev_step[(size_t)i], 0));
         if (p->halo_q[(size_t)src].nrows == 0) continue;
-        if ((rc = launch_spmm(p, p->halo_q[(size_t)src], halo, nullptr, p->h, Z, nullptr, p->m, f, 1, st, relu, true))) return rc;
+        if ((rc = launch_spmm(p, p->halo_q[(size_t)src], halo, nullptr, p->h, Z, nullptr, p->m, f, 1, st, relu, true, halo_odd)))
+            return rc;
     }
     if (use_p2p) CU(p, cudaStreamWaitEvent(st, p->ev_b, 0));
     return 0;
@@ -1445,22 +1565,22 @@ int pgcn_backward(pgcn_plan* p, const float* gZ, float* G_own, int32_t f, void* 
     const bool split = p->have_split && p->opt_overlap;
     const int k = p->k;
     float* rrecv = p->d_rrecv_slab;
-    int par = 0;
+    const float* rrecv_odd = nullptr;
     if (use_p2p) {
-        ++p->epoch;
-        par = (int)(p->epoch & 1);
-        rrecv = arena_ptr(p->arena, p->off_bwd[par]);
+        if ((rc = advance_epoch(p, st))) return rc;
+        rrecv = arena_ptr(p->arena, p->off_bwd[0]);
+        rrecv_odd = arena_ptr(p->arena, p->off_bwd[1]);
     }
     if (!split) {
         if ((rc = launch_spmm(p, p->tr, gZ, nullptr, p->m, G_own, p->d_hsend_slab, p->m, f, 0, st))) return rc;
         for (int i = 1; i < k; ++i) {
-            if (use_p2p) { if ((rc = p2p_put(p, step_dst(p, i), p->d_hsend_slab, f, true, par, st))) return rc; }
+            if (use_p2p) { if ((rc = p2p_put(p, step_dst(p, i), p->d_hsend_slab, f, true, st))) return rc; }
             else if ((rc = nccl_step(p, p->d_hsend_slab, rrecv, f, 1, i, st))) return rc;
         }
         if (use_p2p)
             for (int i = 1; i < k; ++i)
                 if ((rc = p2p_wait(p, step_src(p, i), st))) return rc;
-        return launch_unpack(p, rrecv, G_own, f, st);
+        return launch_unpack(p, rrecv, G_own, f, st, rrecv_odd);
     }
     // ---- pipelined: the partials owed to each peer are computed first (in step order) and leave on the exchange
     // stream while the next peer's rows, and finally the own rows of A^T g, are still being computed
@@ -1471,7 +1591,7 @@ int pgcn_backward(pgcn_plan* p, const float* gZ, float* G_own, int32_t f, void* 
             if ((rc = launch_spmm(p, p->tr_halo_q[(size_t)dst], gZ, nullptr, p->m, G_own, p->d_hsend_slab, p->m, f, 0, st))) return rc;
         CU(p, cudaEventRecord(p->ev_step[(size_t)i], st));
         CU(p, cudaStreamWaitEvent(cs, p->ev_step[(size_t)i], 0));
-        if (use_p2p) { if ((rc = p2p_put(p, dst, p->d_hsend_slab, f, true, par, cs))) return rc; }
+        if (use_p2p) { if ((rc = p2p_put(p, dst, p->d_hsend_slab, f, true, cs))) return rc; }
         else if ((rc = nccl_step(p, p->d_hsend_slab, rrecv, f, 1, i, cs))) return rc;
     }
     CU(p, cudaEventRecord(p->ev_b, cs));
@@ -1481,7 +1601,7 @@ int pgcn_backward(pgcn_plan* p, const float* gZ, float* G_own, int32_t f, void* 
             if ((rc = p2p_wait(p, step_src(p, i), st))) return rc;
     }
     CU(p, cudaStreamWaitEvent(st, p->ev_b, 0));      // NCCL: all blocks received; p2p: the send slab is free again
-    return launch_unpack(p, rrecv, G_own, f, st);
+    return launch_unpack(p, rrecv, G_own, f, st, rrecv_odd);
 }
 
 static int host_slots(pgcn_plan* p, int64_t need)

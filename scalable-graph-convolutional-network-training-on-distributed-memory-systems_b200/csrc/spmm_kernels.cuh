@@ -71,7 +71,17 @@ struct SpmmArgs {
     // (final == nullptr), else the rows whose byte in `final` (indexed by the walked row id) is non-zero
     int relu;
     const unsigned char* final;
+    // double-buffered halo slab of the peer-memory exchange: while the plan's exchange epoch (*epoch, device memory) is
+    // odd, H_odd replaces the operand that holds the slab (H1 with HALO, else H0). epoch == nullptr: no such operand.
+    const float* H_odd;
+    const unsigned long long* epoch;
 };
+
+// The exchange epoch lives on the device so that a captured CUDA graph sees the value of the replay, not the value of
+// the capture: a fused multi-rank call advances it on its stream, every kernel of the call reads it.
+__global__ void epoch_advance_kernel(unsigned long long* epoch) { ++*epoch; }
+
+__device__ __forceinline__ bool epoch_odd(const unsigned long long* epoch) { return epoch != nullptr && (*epoch & 1ull); }
 
 __device__ __forceinline__ float4 vrelu(const float4& a) { return make_float4(fmaxf(a.x, 0.f), fmaxf(a.y, 0.f), fmaxf(a.z, 0.f), fmaxf(a.w, 0.f)); }
 __device__ __forceinline__ float vrelu(const float& a) { return fmaxf(a, 0.f); }
@@ -207,8 +217,11 @@ spmm_rowblock_kernel(const SpmmArgs a)
     bool fok[VPL];
 #pragma unroll
     for (int v = 0; v < VPL; ++v) fok[v] = f0 + v * LPE * VW < a.f;  // f % VW == 0 (launcher)
-    const char* hb0 = reinterpret_cast<const char*>(a.H0) + (size_t)f0 * 4;
-    const char* hb1 = HALO ? reinterpret_cast<const char*>(a.H1) + (size_t)f0 * 4 - (size_t)a.split * pitch
+    const bool odd = epoch_odd(a.epoch);
+    const float* H0 = (!HALO && odd) ? a.H_odd : a.H0;
+    const float* H1 = (HALO && odd) ? a.H_odd : a.H1;
+    const char* hb0 = reinterpret_cast<const char*>(H0) + (size_t)f0 * 4;
+    const char* hb1 = HALO ? reinterpret_cast<const char*>(H1) + (size_t)f0 * 4 - (size_t)a.split * pitch
                            : hb0;
 
 #if PGCN_LDMODE >= 2
@@ -442,11 +455,11 @@ struct PutArgs {
     const int* send_idx;             // null: identity (row j0 + i of src)
     long long j0, nrows;
     const float* src;
-    float* dst;                      // "rows from me" inside the peer's slab
+    float* dst[2];                   // "rows from me" inside the peer's slab, per epoch parity
     int f;
     unsigned int* done;              // CTA completion counter of this destination (self-resetting)
     unsigned long long* flag;        // peer's flag slot for me
-    unsigned long long epoch;
+    const unsigned long long* epoch; // this plan's exchange epoch (already advanced for this call)
 };
 
 template <int VW>
@@ -454,6 +467,8 @@ __global__ void __launch_bounds__(256)
 put_rows_kernel(const PutArgs a)
 {
     typedef typename Vec<VW>::type vec_t;
+    const unsigned long long epoch = *a.epoch;
+    float* dst = (epoch & 1ull) ? a.dst[1] : a.dst[0];
     const int nvec = a.f / VW;
     const long long total = a.nrows * nvec;
     for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < total;
@@ -462,7 +477,7 @@ put_rows_kernel(const PutArgs a)
         const int v = (int)(t - i * nvec);
         const long long srow = a.send_idx ? (long long)__ldg(a.send_idx + a.j0 + i) : a.j0 + i;
         const vec_t val = ld_feat(reinterpret_cast<const vec_t*>(a.src + (size_t)srow * a.f) + v);
-        reinterpret_cast<vec_t*>(a.dst + (size_t)i * a.f)[v] = val;
+        reinterpret_cast<vec_t*>(dst + (size_t)i * a.f)[v] = val;
     }
     // last CTA out publishes the epoch: every CTA fences its own stores system-wide before it counts itself
     __syncthreads();
@@ -472,16 +487,17 @@ put_rows_kernel(const PutArgs a)
         if (t == gridDim.x - 1) {
             atomicExch(a.done, 0u);
             __threadfence_system();
-            asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(a.flag), "l"(a.epoch) : "memory");
+            asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(a.flag), "l"(epoch) : "memory");
         }
     }
 }
 
-// Spin until ONE peer's slot in my flag array has reached `epoch` (one tiny CTA: it never competes for SMs with
+// Spin until ONE peer's slot in my flag array has reached my epoch (one tiny CTA: it never competes for SMs with
 // the kernels whose stores it waits for).
-__global__ void p2p_wait_kernel(const unsigned long long* flag, unsigned long long epoch)
+__global__ void p2p_wait_kernel(const unsigned long long* flag, const unsigned long long* my_epoch)
 {
     if (threadIdx.x == 0) {
+        const unsigned long long epoch = *my_epoch;
         unsigned long long v;
         do {
             asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(flag) : "memory");
@@ -499,6 +515,8 @@ struct UnpackArgs {
     const float* recv;
     float* G;
     int f;
+    const float* recv_odd;               // the peer transport's reverse slab of odd epochs (with `epoch`, else null)
+    const unsigned long long* epoch;
 };
 
 template <int VW>
@@ -506,6 +524,7 @@ __global__ void __launch_bounds__(256)
 unpack_add_kernel(const UnpackArgs a)
 {
     typedef typename Vec<VW>::type vec_t;
+    const float* recv = epoch_odd(a.epoch) ? a.recv_odd : a.recv;
     const int nvec = a.f / VW;
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= (long long)a.nb * nvec) return;
@@ -516,7 +535,7 @@ unpack_add_kernel(const UnpackArgs a)
     vec_t s = *gp;
     const int q0 = __ldg(a.bptr + i), q1 = __ldg(a.bptr + i + 1);
     for (int q = q0; q < q1; ++q)
-        vadd(s, __ldcs(reinterpret_cast<const vec_t*>(a.recv + (size_t)__ldg(a.bpos + q) * a.f) + v));
+        vadd(s, __ldcs(reinterpret_cast<const vec_t*>(recv + (size_t)__ldg(a.bpos + q) * a.f) + v));
     *gp = s;
 }
 

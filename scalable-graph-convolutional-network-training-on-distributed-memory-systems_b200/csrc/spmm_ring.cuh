@@ -163,6 +163,10 @@ __device__ __forceinline__ void reg_set(uint32_t (&a)[N], int i, uint32_t v)
 // run one after the other: while tile t is gathered only that tile of H (TF / f of it) competes for L2, which
 // is what makes 64-float slices pay (a 256-byte slice of a row is twice as likely to still be in L2 as a 512-byte
 // row). Each output element sums the same products in the same order whatever TF is: results are bit-identical.
+// Double-buffered halo slab (a.epoch set): while the exchange epoch is odd, a.H_odd replaces the operand that holds the
+// slab (H1 with HALO, else H0). The tensor-map variant passes the maps of the call's buffers in tm0 / tm1; modes 0 and 1
+// read the parity with every work item (an L1 hit), because holding it for the whole CTA costs one of their instances a
+// register.
 template <int TF, int G, int NG, int MODE, bool HALO>
 __device__ __forceinline__ void ring_body(const SpmmArgs& a, const RingArgs& ra, const CUtensorMap* tm0, const CUtensorMap* tm1)
 {
@@ -224,8 +228,9 @@ __device__ __forceinline__ void ring_body(const SpmmArgs& a, const RingArgs& ra,
     while (w < nitems) {
         const int tile = w / a.nblocks, blk = w - tile * a.nblocks;
         const size_t toff = (size_t)tile * RB;
-        const char* hb0 = reinterpret_cast<const char*>(a.H0) + toff;
-        const char* hb1 = HALO ? reinterpret_cast<const char*>(a.H1) + toff - (size_t)a.split * pitch : hb0;
+        const bool odd = MODE != 2 && epoch_odd(a.epoch);
+        const char* hb0 = reinterpret_cast<const char*>((!HALO && odd) ? a.H_odd : a.H0) + toff;
+        const char* hb1 = HALO ? reinterpret_cast<const char*>(odd ? a.H_odd : a.H1) + toff - (size_t)a.split * pitch : hb0;
         const int4 b = __ldg(a.blocks + blk);
         const bool seg = b.y < 0;
         const int e0 = b.z, e1 = b.w;
@@ -431,13 +436,15 @@ spmm_ring_kernel(const SpmmArgs a, const RingArgs ra)
     ring_body<TF, G, NG, MODE, HALO>(a, ra, nullptr, nullptr);
 }
 
-// tensor-map variant: the tensor maps of H_own (tm0) and of the halo slab (tm1) travel as __grid_constant__ parameters
+// tensor-map variant: the tensor maps of H_own (tm0) and of the halo slab (tm1) travel as __grid_constant__ parameters;
+// tm_odd maps the halo slab of odd exchange epochs (it replaces tm1 with HALO, else tm0; unused when a.epoch is null)
 template <int TF, int G, int NG, bool HALO>
 __global__ void __launch_bounds__(kRingWarps * 32)
 spmm_ring_tm_kernel(const SpmmArgs a, const RingArgs ra, const __grid_constant__ CUtensorMap tm0,
-                    const __grid_constant__ CUtensorMap tm1)
+                    const __grid_constant__ CUtensorMap tm1, const __grid_constant__ CUtensorMap tm_odd)
 {
-    ring_body<TF, G, NG, 2, HALO>(a, ra, &tm0, &tm1);
+    const bool odd = epoch_odd(a.epoch);
+    ring_body<TF, G, NG, 2, HALO>(a, ra, (!HALO && odd) ? &tm_odd : &tm0, (HALO && odd) ? &tm_odd : &tm1);
 }
 
 }  // namespace pgcn

@@ -58,8 +58,14 @@ def batch_local_plans(A, partvec, rank, size, batch_size, seed=1, index_sets=Non
 
 # ---- training driver ---------------------------------------------------------------------------------------------
 
-def run(rank, size, nlayers, nfeatures, path_A, path_partvec, backend, batch_size, out=None, seed=None):
-    """GPU/PGCN-Mini-batch.py:199-310 on the H100 path. Returns {"losses", "elapsed", "total_vol", "total_nmsg"}."""
+def run(rank, size, nlayers, nfeatures, path_A, path_partvec, backend, batch_size, out=None, seed=None,
+        cuda_graph=False):
+    """GPU/PGCN-Mini-batch.py:199-310 on the H100 path. Returns {"losses", "elapsed", "total_vol", "total_nmsg"}.
+
+    cuda_graph=True: after the (eager) warm-up epoch, the forward and backward of every batch plan are captured once
+    in a CUDA graph (all graphs share one memory pool) and replayed in the eager step order; the gradient average and
+    the optimizer step stay eager, so the losses are the eager ones. A step of a small batch is launch-bound: the
+    replay saves the per-kernel launch and the Python autograd overhead."""
     import sys
     import time
     import torch
@@ -106,20 +112,31 @@ def run(rank, size, nlayers, nfeatures, path_A, path_partvec, backend, batch_siz
         initialize_parameters(layers, size)
     optimizer = torch.optim.Adam(layers.parameters(), lr=1e-3)                 # :249
 
-    def step(plan):
+    def forward_loss(plan):
         X = H
         for layer in layers:
             X = layer(plan, X)
-        loss = reference_loss(X, labels, n)                         # nll over all n rows (:262-263)
-        optimizer.zero_grad()
-        loss.backward()
+        return reference_loss(X, labels, n)                         # nll over all n rows (:262-263)
+
+    def update():
         if size > 1:
             average_gradients(layers, size)
         optimizer.step()
+
+    def step(plan):
+        loss = forward_loss(plan)
+        optimizer.zero_grad()
+        loss.backward()
+        update()
         return loss.detach()
 
+    if cuda_graph:
+        for plan in plans:
+            plan.prepare(nfeatures)
     for plan in plans:                                                         # warm-up epoch (:251-268)
         step(plan)
+    if cuda_graph:
+        step = _graphed_steps(plans, forward_loss, update, optimizer, layers)
     torch.cuda.synchronize()
     start = time.time()
     losses = []
@@ -149,8 +166,44 @@ def run(rank, size, nlayers, nfeatures, path_A, path_partvec, backend, batch_siz
     return res
 
 
+def _graphed_steps(plans, forward_loss, update, optimizer, layers):
+    """Capture forward + backward of every batch plan in a CUDA graph of its own, all graphs in one memory pool.
+    Returns step(plan): replay that plan's graph, add the exchange stats its capture recorded, run `update` (gradient
+    average and optimizer step) eagerly, and return the graph's loss tensor (read it before the next replay: the next
+    graph may reuse its memory)."""
+    import torch
+    params = list(layers.parameters())
+    grads = [p.grad if p.grad is not None else torch.zeros_like(p) for p in params]
+    for p, g in zip(params, grads):
+        p.grad = g                       # static gradient buffers: backward inside the graph accumulates into them
+    pool = torch.cuda.graph_pool_handle()
+    graphs = {}
+    for plan in plans:
+        before = dict(plan.stats)
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g, pool=pool):
+            optimizer.zero_grad(set_to_none=False)
+            loss = forward_loss(plan)
+            loss.backward()
+        # the capture ran no kernel: its exchange counts belong to every replay instead
+        delta = {k: plan.stats[k] - before[k] for k in before}
+        plan.stats.update(before)
+        if any(p.grad is None or p.grad.data_ptr() != g_.data_ptr() for p, g_ in zip(params, grads)):
+            raise RuntimeError("backward inside the CUDA graph replaced a gradient buffer instead of accumulating")
+        graphs[id(plan)] = (g, loss.detach(), delta)
+
+    def step(plan):
+        g, loss, delta = graphs[id(plan)]
+        g.replay()
+        for k, v in delta.items():
+            plan.stats[k] += v
+        update()
+        return loss
+    return step
+
+
 def main(argv):
-    """python -m pgcn_b200.minibatch -a A.mtx -p partvec.pkl -b nccl -s k -l 3 -f F -n batch_size
+    """python -m pgcn_b200.minibatch -a A.mtx -p partvec.pkl -b nccl -s k -l 3 -f F -n batch_size [--cuda-graph]
     (SLURM_NPROCS / SLURM_PROCID or WORLD_SIZE / RANK, MASTER_ADDR / MASTER_PORT as the reference)."""
     import getopt
     import os
@@ -159,11 +212,12 @@ def main(argv):
     size = int(os.environ.get("SLURM_NPROCS", os.environ.get("WORLD_SIZE", "1")))
     rank = int(os.environ.get("SLURM_PROCID", os.environ.get("RANK", "0")))
     try:
-        opts, _ = getopt.getopt(argv, "a:p:b:s:l:f:n:", ["seed="])
+        opts, _ = getopt.getopt(argv, "a:p:b:s:l:f:n:", ["seed=", "cuda-graph"])
     except getopt.GetoptError:
         print("a:p:b:", flush=True)
         sys.exit(2)
-    kw = dict(path_A=None, path_partvec=None, backend="nccl", nlayers=3, nfeatures=None, batch_size=None, seed=None)
+    kw = dict(path_A=None, path_partvec=None, backend="nccl", nlayers=3, nfeatures=None, batch_size=None, seed=None,
+              cuda_graph=False)
     for opt, arg in opts:
         if opt == "-a": kw["path_A"] = arg
         elif opt == "-p": kw["path_partvec"] = arg
@@ -173,6 +227,7 @@ def main(argv):
         elif opt == "-f": kw["nfeatures"] = int(arg)
         elif opt == "-n": kw["batch_size"] = int(arg)
         elif opt == "--seed": kw["seed"] = int(arg)
+        elif opt == "--cuda-graph": kw["cuda_graph"] = True
     if None in (kw["path_A"], kw["path_partvec"], kw["nfeatures"], kw["batch_size"]):
         print("usage: minibatch -a <A.mtx> -p <partvec.pkl> -b nccl -s <nparts> -l <nlayers> -f <nfeatures> -n <batch_size>", flush=True)
         sys.exit(2)
@@ -184,7 +239,7 @@ def main(argv):
                             device_id=torch.device("cuda", rank % max(torch.cuda.device_count(), 1)))
     try:
         return run(rank, size, kw["nlayers"], kw["nfeatures"], kw["path_A"], kw["path_partvec"], kw["backend"],
-                   kw["batch_size"], seed=kw["seed"])
+                   kw["batch_size"], seed=kw["seed"], cuda_graph=kw["cuda_graph"])
     finally:
         dist.destroy_process_group()
 

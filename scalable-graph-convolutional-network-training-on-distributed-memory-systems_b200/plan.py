@@ -276,6 +276,15 @@ class PgcnPlan:
         with torch.cuda.device(self.device):
             return cabi.check(self._lib.pgcn_plan_autotune(self.handle, int(f)), self._h)
 
+    def prepare(self, f):
+        """Set-up work for width f under the current options (pgcn_plan_prepare), so that PSpMM / PSpMMRelu on this
+        plan can be captured in a CUDA graph (torch.cuda.graph, torch.cuda.make_graphed_callables). Synchronous. Call it
+        again after changing f or an option."""
+        import torch
+        self.owned_index()                # the "global" layout's index tensor: a host-to-device copy, not capturable
+        with torch.cuda.device(self.device):
+            cabi.check(self._lib.pgcn_plan_prepare(self.handle, int(f)), self._h)
+
     def algorithmic_bytes(self, f):
         b = cabi.PgcnBytes()
         cabi.check(self._lib.pgcn_algorithmic_bytes(self.handle, int(f), C.byref(b)), self._h)
