@@ -573,6 +573,7 @@ int ring_attr(pgcn_plan* p, int tf, int shape, int mode, bool halo, cudaStream_t
 {
     const int g = kRingShapes[shape].g, ng = kRingShapes[shape].ng;
     const size_t smem = ring_smem_bytes(tf, g * ng, ng);
+    const int warps = ring_cta_warps(tf, g * ng, ng);
     const int tslot = tf == 64 ? 0 : (tf == 128 ? 1 : 2);
     const int slot = ((tslot * 4 + shape) * 3 + mode) * 2 + (halo ? 1 : 0);
     if (slot_out) *slot_out = slot;
@@ -583,7 +584,7 @@ int ring_attr(pgcn_plan* p, int tf, int shape, int mode, bool halo, cudaStream_t
     const void* fptr = mode == 2 ? (const void*)pick_ring_tm(tf, shape, halo) : (const void*)pick_ring(tf, shape, mode, halo);
     CU(p, cudaFuncSetAttribute(fptr, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int nb = 0;
-    CU(p, cudaOccupancyMaxActiveBlocksPerMultiprocessorWithFlags(&nb, fptr, kRingWarps * 32, smem, 0));
+    CU(p, cudaOccupancyMaxActiveBlocksPerMultiprocessorWithFlags(&nb, fptr, warps * 32, smem, 0));
     p->ring_ctas_per_sm[slot] = std::max(nb, 1);
     p->ring_attr_set[slot] = true;
     return 0;
@@ -653,7 +654,8 @@ int launch_spmm(pgcn_plan* p, DevCsr& c, const float* H0, const float* H1, int s
         if ((rc = ring_attr(p, tf, shape, mode, halo, st, &slot, &smem))) return rc;
         RingArgs ra;
         ra.counter = nullptr; ra.hub = nullptr; ra.nhub = 0;
-        dim3 grid((unsigned)((sc.nblocks + kRingWarps - 1) / kRingWarps), (unsigned)tiles);
+        const int warps = ring_cta_warps(tf, kRingShapes[shape].g * kRingShapes[shape].ng, kRingShapes[shape].ng);
+        dim3 grid((unsigned)((sc.nblocks + warps - 1) / warps), (unsigned)tiles);
         // Persistent CTAs own their SM (shared memory + registers) until the whole launch is done; a put / NCCL kernel
         // of the exchange stream would then wait behind the SpMM it is supposed to overlap (measured at 8 GPUs: step =
         // sum of puts + sum of SpMMs). Multi-rank plans with overlap therefore run one block per warp (CTAs retire
@@ -664,12 +666,12 @@ int launch_spmm(pgcn_plan* p, DevCsr& c, const float* H0, const float* H1, int s
             // one counter over all (tile, row block) items, tile-major: the tiles run one after the other
             CU(p, cudaMemsetAsync(p->d_counter, 0, sizeof(unsigned int), st));
             ra.counter = p->d_counter;
-            const unsigned items = (unsigned)(((int64_t)sc.nblocks * tiles + kRingWarps - 1) / kRingWarps);
+            const unsigned items = (unsigned)(((int64_t)sc.nblocks * tiles + warps - 1) / warps);
             grid.x = std::min<unsigned>(items, (unsigned)(p->num_sms * p->ring_ctas_per_sm[slot]));
             grid.y = 1;
         }
-        if (mode == 2) fn_tm<<<grid, kRingWarps * 32, smem, st>>>(a, ra, tm0, tm1, tm_odd);
-        else fn<<<grid, kRingWarps * 32, smem, st>>>(a, ra);
+        if (mode == 2) fn_tm<<<grid, warps * 32, smem, st>>>(a, ra, tm0, tm1, tm_odd);
+        else fn<<<grid, warps * 32, smem, st>>>(a, ra);
         ++p->launches;
     } else if (sc.nblocks > 0) {
         const int groups_per_cta = kSpmmThreads / t.lpe;

@@ -100,11 +100,10 @@ __device__ __noinline__ void ring_store_row(V a0, V a1, const int* rowids, int r
     }
 }
 
-constexpr int kRingWarps = 2;        // warps per CTA (each fully independent: CTA size only sets the smem granule)
 constexpr int kRingPieces = 4;       // index pieces (32 entries, kPieceBytes each) resident per warp
 
 struct RingArgs {
-    unsigned int* counter;   // null: block blockIdx.x * kRingWarps + warp of tile blockIdx.y; else the next
+    unsigned int* counter;   // null: block blockIdx.x * warps per CTA + warp of tile blockIdx.y; else the next
                              // (tile, block) work item, tile-major (persistent CTAs)
     const float* hub;        // reserved (hub rows resident in shared memory)
     int nhub;
@@ -115,9 +114,23 @@ __host__ __device__ constexpr size_t ring_warp_bytes(int tf, int ns, int ng)
 {
     return ((size_t)ns * tf * 4 + (size_t)kRingPieces * kPieceBytes + (size_t)(ng + kRingPieces) * 8 + 127) / 128 * 128;
 }
+// Warps per CTA. The warps are fully independent, so the CTA size only sets the shared-memory granule, and every CTA
+// also costs the SM 1 KB of reserved shared memory (sm_90: 228 KB per SM, at most 227 KB per CTA). Where the ring is
+// bounded by shared memory, 4-warp CTAs fit more warps per SM than 2-warp CTAs: 24 instead of 22 for the 64-float,
+// 32-slot ring (9.1 KB per warp). Otherwise (a tie, or a CTA over 227 KB) CTAs keep 2 warps.
+constexpr size_t kSmemPerSm = 228 * 1024, kSmemPerCtaMax = 227 * 1024, kSmemReservedPerCta = 1024;
+__host__ __device__ constexpr int ring_resident_warps(size_t warp_bytes, int warps)
+{
+    return (int)(kSmemPerSm / (warp_bytes * warps + 128 + kSmemReservedPerCta)) * warps;
+}
+__host__ __device__ constexpr int ring_cta_warps(int tf, int ns, int ng)
+{
+    return (ring_warp_bytes(tf, ns, ng) * 4 + 128 <= kSmemPerCtaMax &&
+            ring_resident_warps(ring_warp_bytes(tf, ns, ng), 4) > ring_resident_warps(ring_warp_bytes(tf, ns, ng), 2)) ? 4 : 2;
+}
 __host__ __device__ constexpr size_t ring_smem_bytes(int tf, int ns, int ng)
 {
-    return ring_warp_bytes(tf, ns, ng) * kRingWarps + 128;
+    return ring_warp_bytes(tf, ns, ng) * ring_cta_warps(tf, ns, ng) + 128;
 }
 
 // What one lane holds of a row tile of TF floats: one float2 (64-float slices, 256 B), one float4 (128 floats) or
@@ -218,7 +231,7 @@ __device__ __forceinline__ void ring_body(const SpmmArgs& a, const RingArgs& ra,
     for (int v = 0; v < NV; ++v) acc[v] = vzero((V*)nullptr);
 
     // without a counter: one item per warp, tile blockIdx.y
-    int w = (int)(blockIdx.x * kRingWarps + warp);
+    int w = (int)(blockIdx.x * ring_cta_warps(TF, NS, NG) + warp);
     w = w < a.nblocks ? (int)blockIdx.y * a.nblocks + w : nitems;
     if (counter) {
         if (lane == 0) w = (int)atomicAdd(counter, 1u);
@@ -430,7 +443,7 @@ __device__ __forceinline__ void ring_body(const SpmmArgs& a, const RingArgs& ra,
 }
 
 template <int TF, int G, int NG, int MODE, bool HALO>
-__global__ void __launch_bounds__(kRingWarps * 32)
+__global__ void __launch_bounds__(ring_cta_warps(TF, G * NG, NG) * 32)
 spmm_ring_kernel(const SpmmArgs a, const RingArgs ra)
 {
     ring_body<TF, G, NG, MODE, HALO>(a, ra, nullptr, nullptr);
@@ -439,7 +452,7 @@ spmm_ring_kernel(const SpmmArgs a, const RingArgs ra)
 // tensor-map variant: the tensor maps of H_own (tm0) and of the halo slab (tm1) travel as __grid_constant__ parameters;
 // tm_odd maps the halo slab of odd exchange epochs (it replaces tm1 with HALO, else tm0; unused when a.epoch is null)
 template <int TF, int G, int NG, bool HALO>
-__global__ void __launch_bounds__(kRingWarps * 32)
+__global__ void __launch_bounds__(ring_cta_warps(TF, G * NG, NG) * 32)
 spmm_ring_tm_kernel(const SpmmArgs a, const RingArgs ra, const __grid_constant__ CUtensorMap tm0,
                     const __grid_constant__ CUtensorMap tm1, const __grid_constant__ CUtensorMap tm_odd)
 {

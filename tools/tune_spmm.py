@@ -5,6 +5,7 @@
     python tools/tune_spmm.py --config C2 --sweep default
     python tools/tune_spmm.py --config C2 --single edges_per_block=256,tile_floats=0 --iters 5   (for ncu)
     python tools/tune_spmm.py --gather-sweep        (L2 capacity / bandwidth probe with windowed columns)
+    python tools/tune_spmm.py --gather-sweep --mixed   (0-40 % of the columns from a 512 MB window, the rest from 16 MB)
     python tools/tune_spmm.py --config C2 --sweep slices   (ring row tile: full width vs 64-float slices)
 """
 import argparse
@@ -42,6 +43,7 @@ def main():
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--baselines", action="store_true")
     ap.add_argument("--gather-sweep", action="store_true")
+    ap.add_argument("--mixed", action="store_true", help="with --gather-sweep: mix a 512 MB and a 16 MB window of columns")
     ap.add_argument("--transpose", action="store_true")
     ap.add_argument("--cache", default="/tmp/pgcn_b200_cache")
     ap.add_argument("--out", default="")
@@ -66,6 +68,28 @@ def main():
         print(s, flush=True)
         if outf:
             outf.write(s + "\n"); outf.flush()
+
+    if args.gather_sweep and args.mixed:
+        # a fraction of the columns uniform over a 512 MB window (1 M rows: they miss L2), the rest over a 16 MB window
+        # (32 K rows: they hit); the plan marks the wide-window columns cold. Shows what a given share of L2-missing
+        # gathers costs the ring at each row tile and ring depth (DESIGN §6, cold look-ahead).
+        n, d, f, hot_rows = 1_000_000, 16, 128, 32_000
+        rng = np.random.default_rng(0)
+        for frac in (0.0, 0.1, 0.2, 0.4):
+            wide = rng.random(n * d) < frac
+            col = np.where(wide, rng.integers(0, n, size=n * d), rng.integers(0, hot_rows, size=n * d))
+            row = np.repeat(np.arange(n, dtype=np.int64), d)
+            A = sp.coo_matrix((np.ones(n * d, dtype=np.float32), (row, col)), shape=(n, n))
+            p = planmod.build_plan(A, np.zeros(n, dtype=np.int64), 0, 1, f, device=dev)
+            H = torch.rand((n, f), device=dev); Z = torch.empty((n, f), device=dev)
+            for tile, slots in itertools.product((0, 64), (16, 32)):
+                p.set_option("ring_tile_floats", tile)
+                p.set_option("ring_slots", slots)
+                med, mn = timed(lambda: cabi.check(lib.pgcn_spmm(p.handle, 0, H.data_ptr(), None, Z.data_ptr(), None, f, stream), p.handle), args.iters, warm=20)
+                emit({"probe": "gather-mixed", "wide_frac": frac, "ring_tile_floats": tile, "ring_slots": slots, "ms": med,
+                      "gather_GBs": p.lp.nnz() * f * 4 / med / 1e6})
+            p.close()
+        return
 
     if args.gather_sweep:
         # n rows, degree d, columns uniform in a window of W rows: working set W*f*4 bytes
