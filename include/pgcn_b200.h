@@ -236,6 +236,43 @@ int pgcn_unpack_add(pgcn_plan* plan, const float* recv_slab, float* G_own, int32
 int pgcn_forward(pgcn_plan* plan, const float* H_own, float* Z, int32_t f, void* stream);
 int pgcn_backward(pgcn_plan* plan, const float* gZ, float* G_own, int32_t f, void* stream);
 
+/* ---- edge values: the aggregation's values set per call, and their gradient ------------------ */
+/*
+ * torch.sparse.mm(A, H) (GPU/PGCN.py:127) takes new values of A on every call and, when they require grad, returns
+ * dA.values = < gZ[row(e)], H[col(e)] >. These entry points give the plan the same two abilities (learned edge
+ * weights, per-step edge masks such as DropEdge, attention scores), without changing the exchange or the kernels.
+ *
+ * pgcn_plan_bind_values: synchronous set-up, like pgcn_plan_autotune and pgcn_plan_prepare. For every record set of
+ *   the plan (forward, transposed, and on split multi-rank plans the own-column block and each peer's block) it builds
+ *   a device map from each stored entry to its forward entry (an index into the colidx / vals arrays given to
+ *   pgcn_plan_create), reading the plan's own records back; it also keeps a device copy of the creation values.
+ *   Transposed entries are matched to the forward entry of the same (row, column), duplicates in order of appearance;
+ *   a transposed CSR that does not hold the same entries with the same values returns PGCN_ERR_INVALID and names the
+ *   first mismatch. Cost: 4 B per entry per record set that is not the forward matrix itself, plus 4 B per entry of
+ *   creation values: 12 B per edge on a split multi-rank plan, 8 B on one rank. Plans that are never bound pay nothing.
+ *   Binding twice is a no-op. Its copies run on a stream of the plan and wait for that stream only (never for the
+ *   device), so it may be called while other plans of the process have exchange kernels waiting on the device.
+ * pgcn_plan_set_values: `vals` is a DEVICE array of nnz floats in forward CSR order; NULL restores the creation values.
+ *   One kernel rewrites the value words of every record set, stream-ordered on `stream`: every later compute call on
+ *   that stream (pgcn_spmm, pgcn_forward / pgcn_backward, the _host variants, every kernel and layout) aggregates with
+ *   these values. Masks, schedules and the hot / cold marking do not depend on values and do not change. Capturable.
+ *   Before pgcn_plan_bind_values it returns PGCN_ERR_STATE.
+ * pgcn_sddmm: dvals[e] = sum_c gZ[row(e), c] * [H_own ; H_halo][col(e), c] for every forward entry e, written in
+ *   forward CSR order (nnz floats). gZ and H_own are m x f, H_halo h x f (may be NULL when h == 0): the halo rows of
+ *   the forward, see pgcn_forward_keep_halo. Local only (no exchange); every output is reduced in one fixed order, so
+ *   runs are bit-identical. Needs no binding. f = 128, 256, 384 or 512 with 16-byte aligned operands takes a
+ *   shared-memory ring kernel fed by TMA bulk copies, every other case a plain kernel. Like pgcn_forward it refuses,
+ *   with PGCN_ERR_STATE, set-up work while its stream is being captured: pgcn_plan_prepare(plan, f) does that set-up.
+ * pgcn_forward_keep_halo: pgcn_forward, and in addition the h halo rows this call received are copied into
+ *   H_halo_out (h x f, caller-owned) on `stream` before it returns, out of the slab of the call's exchange parity (the
+ *   next fused call of the same parity overwrites that slab). With k == 1 it is pgcn_forward (H_halo_out unused).
+ */
+int pgcn_plan_bind_values(pgcn_plan* plan);
+int pgcn_plan_set_values(pgcn_plan* plan, const float* vals, void* stream);
+int pgcn_sddmm(pgcn_plan* plan, const float* gZ, const float* H_own, const float* H_halo, float* dvals, int32_t f,
+               void* stream);
+int pgcn_forward_keep_halo(pgcn_plan* plan, const float* H_own, float* Z, float* H_halo_out, int32_t f, void* stream);
+
 /* ---- host-buffer variant: what a non-torch host (the reference's C path) would bind -------- */
 /*
  * Same as pgcn_forward but H and Z are HOST pointers (pinned or pageable): copies H to the

@@ -20,6 +20,7 @@ SYMBOLS = [
     "pgcn_comm_unique_id", "pgcn_comm_init", "pgcn_comm_share", "pgcn_p2p_export", "pgcn_p2p_import",
     "pgcn_spmm", "pgcn_pack", "pgcn_exchange", "pgcn_unpack_add",
     "pgcn_forward", "pgcn_backward", "pgcn_forward_host", "pgcn_forward_host_async", "pgcn_forward_host_wait",
+    "pgcn_plan_bind_values", "pgcn_plan_set_values", "pgcn_sddmm", "pgcn_forward_keep_halo",
 ]
 
 
@@ -109,6 +110,14 @@ def load(build_if_missing=True):
     lib.pgcn_forward_host_async.argtypes = [vp, vp, vp, i32]
     lib.pgcn_forward_host_wait.restype = C.c_int
     lib.pgcn_forward_host_wait.argtypes = [vp]
+    lib.pgcn_plan_bind_values.restype = C.c_int
+    lib.pgcn_plan_bind_values.argtypes = [vp]
+    lib.pgcn_plan_set_values.restype = C.c_int
+    lib.pgcn_plan_set_values.argtypes = [vp, vp, vp]
+    lib.pgcn_sddmm.restype = C.c_int
+    lib.pgcn_sddmm.argtypes = [vp, vp, vp, vp, vp, i32, vp]
+    lib.pgcn_forward_keep_halo.restype = C.c_int
+    lib.pgcn_forward_keep_halo.argtypes = [vp, vp, vp, vp, i32, vp]
     _lib = lib
     return lib
 

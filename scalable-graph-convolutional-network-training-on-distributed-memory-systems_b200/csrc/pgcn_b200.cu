@@ -8,6 +8,7 @@
 #include "../../include/pgcn_b200.h"
 #include "spmm_kernels.cuh"
 #include "spmm_ring.cuh"
+#include "sddmm.cuh"
 
 #include <dlfcn.h>
 #include <unistd.h>
@@ -86,6 +87,7 @@ struct DevCsr {
     int row_base = 0;               // compact id of the first walked row (views: offset into the parent's numbering)
     std::vector<int> h_rowids, h_empty;   // host copies (parents of views only)
     unsigned char* d_final = nullptr;     // per walked row: this matrix is the LAST launch of the forward that writes it
+    int* d_vmap = nullptr;          // pgcn_plan_bind_values: entry -> forward entry (null for the forward matrix itself)
     int64_t tuned_epb[2] = {0, 0};  // per-matrix autotune results (0: use the plan option): [0] register, [1] ring
     int tuned_slots = 0;
     int tuned_tile = 0;             // ring row tile in floats (0: the full width 128 or 256)
@@ -181,6 +183,15 @@ struct pgcn_plan {
     bool prepared = false;
     std::vector<void*> retired;
     int64_t nretired = 0;
+
+    // pgcn_plan_bind_values: the record sets whose value words pgcn_plan_set_values rewrites, and the creation values
+    bool bound = false;
+    float* d_vals0 = nullptr;              // nnz, forward CSR order
+    ValueSet* d_vsets = nullptr;
+    int nvsets = 0;
+    long long vtotal = 0;                  // entries over all sets
+    bool sddmm_attr_set[5] = {false};      // per f / 128 of the SDDMM ring kernel
+    int sddmm_ctas_per_sm[5] = {0};
 
     // host-buffer variant: two device slots, copy-in / compute / copy-out streams chained by events
     float* d_hostH[2] = {nullptr, nullptr}; float* d_hostZ[2] = {nullptr, nullptr}; int64_t host_cap = 0;
@@ -304,7 +315,7 @@ void csr_view(const DevCsr& base, DevCsr& v, int r0, int r1)
 
 void csr_free(DevCsr& c)
 {
-    if (!c.view) { cudaFree(c.d_cw); cudaFree(c.d_rowids); cudaFree(c.d_empty); }
+    if (!c.view) { cudaFree(c.d_cw); cudaFree(c.d_rowids); cudaFree(c.d_empty); cudaFree(c.d_vmap); }
     cudaFree(c.d_final);
     for (auto& sc : c.sched) { cudaFree(sc.d_blocks); cudaFree(sc.d_long); cudaFree(sc.d_partial); }
     c = DevCsr();
@@ -532,6 +543,9 @@ void preload_kernels()
     touch_kernel(pack_rows_kernel<4>); touch_kernel(pack_rows_kernel<1>);
     touch_kernel(unpack_add_kernel<4>); touch_kernel(unpack_add_kernel<1>);
     touch_kernel(put_rows_kernel<4>); touch_kernel(p2p_wait_kernel); touch_kernel(epoch_advance_kernel);
+    touch_kernel(set_values_kernel); touch_kernel(copy_halo_kernel); touch_kernel(sddmm_plain_kernel);
+    touch_kernel(sddmm_ring_kernel<1>); touch_kernel(sddmm_ring_kernel<2>);
+    touch_kernel(sddmm_ring_kernel<3>); touch_kernel(sddmm_ring_kernel<4>);
 }
 
 bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
@@ -738,6 +752,125 @@ int launch_unpack(pgcn_plan* p, const float* recv, float* G, int f, cudaStream_t
     else unpack_add_kernel<1><<<grid, 256, 0, st>>>(a);
     ++p->launches;
     CU(p, cudaGetLastError());
+    return 0;
+}
+
+// ---- edge values -----------------------------------------------------------------------------
+
+typedef void (*sddmm_fn)(const SddmmArgs);
+
+sddmm_fn pick_sddmm(int nv)
+{
+    switch (nv) {
+        case 1: return sddmm_ring_kernel<1>;
+        case 2: return sddmm_ring_kernel<2>;
+        case 3: return sddmm_ring_kernel<3>;
+        default: return sddmm_ring_kernel<4>;
+    }
+}
+
+// The SDDMM ring kernel serves f = 128 .. 512 in steps of 128 with 16-byte aligned operands, like the SpMM ring
+bool sddmm_use_ring(const pgcn_plan* p, const float* gZ, const float* H0, const float* H1, int f)
+{
+    return use_ring(p, gZ, H0, f) && f <= 512 && (!H1 || aligned16(H1));
+}
+
+// Opt the SDDMM ring instance of width f in to its dynamic shared memory and record its occupancy, once per plan.
+int sddmm_attr(pgcn_plan* p, int f, cudaStream_t st)
+{
+    const int nv = f / 128;
+    if (p->sddmm_attr_set[nv]) return 0;
+    int rc = refuse_under_capture(p, st);
+    if (rc) return rc;
+    const void* fptr = (const void*)pick_sddmm(nv);
+    const size_t smem = sddmm_smem_bytes(nv);
+    CU(p, cudaFuncSetAttribute(fptr, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int nb = 0;
+    CU(p, cudaOccupancyMaxActiveBlocksPerMultiprocessorWithFlags(&nb, fptr, kSddmmWarps * 32, smem, 0));
+    p->sddmm_ctas_per_sm[nv] = std::max(nb, 1);
+    p->sddmm_attr_set[nv] = true;
+    return 0;
+}
+
+// dvals = SDDMM over the forward matrix (H1: the halo rows, columns >= m)
+int launch_sddmm(pgcn_plan* p, const float* gZ, const float* H0, const float* H1, float* dvals, int f, cudaStream_t st)
+{
+    DevCsr& c = p->fwd;
+    if (c.nnz == 0 || c.nrows == 0) return 0;
+    const bool ring = sddmm_use_ring(p, gZ, H0, H1, f);
+    int64_t epb, long_row;
+    sched_params(p, c, ring, &epb, &long_row);
+    int rc;
+    if (!sched_ready(c, ring ? 1 : 0, epb, long_row) && (rc = refuse_under_capture(p, st))) return rc;
+    if ((rc = build_schedule(p, c, ring ? 1 : 0, epb, long_row))) return rc;
+    const DevCsr::Sched& sc = c.sched[ring ? 1 : 0];
+    SddmmArgs a;
+    a.blocks = sc.d_blocks; a.nblocks = sc.nblocks;
+    a.pieces = c.d_cw;
+    a.gZ = gZ; a.H0 = H0; a.H1 = H1; a.split = p->m;
+    a.rowids = c.d_rowids;
+    a.dvals = dvals; a.f = f;
+    a.counter = nullptr;
+    if (sc.nblocks == 0) return 0;
+    if (ring) {
+        if ((rc = sddmm_attr(p, f, st))) return rc;
+        CU(p, cudaMemsetAsync(p->d_counter, 0, sizeof(unsigned int), st));
+        a.counter = p->d_counter;
+        const unsigned ctas = (unsigned)((sc.nblocks + kSddmmWarps - 1) / kSddmmWarps);
+        const unsigned grid = std::min<unsigned>(ctas, (unsigned)(p->num_sms * p->sddmm_ctas_per_sm[f / 128]));
+        pick_sddmm(f / 128)<<<grid, kSddmmWarps * 32, sddmm_smem_bytes(f / 128), st>>>(a);
+    } else {
+        sddmm_plain_kernel<<<(unsigned)((sc.nblocks + 7) / 8), 256, 0, st>>>(a);
+    }
+    ++p->launches;
+    CU(p, cudaGetLastError());
+    return 0;
+}
+
+// Set-up copies of pgcn_plan_bind_values. They run on the plan's own non-blocking stream and wait for that stream only:
+// a device-wide (or legacy-stream) synchronisation could wait for another rank's spinning p2p_wait_kernel when several
+// ranks' plans share this process, and that rank's puts would then never be enqueued. No compute call writes the
+// records (only pgcn_plan_set_values does, and it needs the binding), so nothing has to be waited for.
+int copy_setup(pgcn_plan* p, void* dst, const void* src, size_t bytes, cudaMemcpyKind kind)
+{
+    if (bytes == 0) return 0;
+    CU(p, cudaMemcpyAsync(dst, src, bytes, kind, p->host_stream));
+    CU(p, cudaStreamSynchronize(p->host_stream));
+    return 0;
+}
+
+template <class T>
+int upload_setup(pgcn_plan* p, T** dst, const T* src, size_t n)
+{
+    *dst = nullptr;
+    CU(p, cudaMalloc((void**)dst, std::max<size_t>(n, 1) * sizeof(T)));
+    return copy_setup(p, *dst, src, n * sizeof(T), cudaMemcpyHostToDevice);
+}
+
+// Download the records of a matrix and decode, per entry: its column, its value bits and its output row.
+int decode_records(pgcn_plan* p, const DevCsr& c, std::vector<int>& col, std::vector<int>& val, std::vector<int>& row)
+{
+    const int64_t nnz = c.nnz;
+    col.resize((size_t)nnz); val.resize((size_t)nnz); row.resize((size_t)nnz);
+    if (nnz == 0) return 0;
+    const size_t npieces = (size_t)((nnz + 31) / 32);
+    std::vector<int> cw(npieces * kPieceInts);
+    int rc;
+    if ((rc = copy_setup(p, cw.data(), c.d_cw, cw.size() * sizeof(int), cudaMemcpyDeviceToHost))) return rc;
+    std::vector<int> rowids;
+    if (c.d_rowids) {
+        rowids.resize((size_t)c.nrows_c);
+        if ((rc = copy_setup(p, rowids.data(), c.d_rowids, rowids.size() * sizeof(int), cudaMemcpyDeviceToHost))) return rc;
+    }
+    int r = 0;
+    for (int64_t e = 0; e < nnz; ++e) {
+        const int* pc = cw.data() + (size_t)(e >> 5) * kPieceInts;
+        const int i = (int)(e & 31);
+        col[(size_t)e] = pc[i];
+        val[(size_t)e] = pc[32 + i];
+        row[(size_t)e] = rowids.empty() ? r : rowids[(size_t)r];
+        if (((unsigned)pc[64] >> i) & 1u) ++r;
+    }
     return 0;
 }
 
@@ -1040,6 +1173,7 @@ int pgcn_plan_destroy(pgcn_plan* p)
     if (p->s_out) cudaStreamDestroy(p->s_out);
     cudaFree(p->d_counter);
     cudaFree(p->d_epoch);
+    cudaFree(p->d_vals0); cudaFree(p->d_vsets);
     for (void* q : p->retired) cudaFree(q);
     if (p->comm_stream) cudaStreamDestroy(p->comm_stream);
     if (p->host_stream) cudaStreamDestroy(p->host_stream);
@@ -1292,7 +1426,110 @@ int pgcn_plan_prepare(pgcn_plan* p, int32_t f)
                     if ((rc = ring_attr(p, tf, shape, 0, halo != 0, p->host_stream, nullptr, nullptr))) return rc;
                 if (tf >= 128 && (rc = ring_attr(p, tf, 0, 1, halo != 0, p->host_stream, nullptr, nullptr))) return rc;
             }
+    // pgcn_sddmm walks the forward matrix's schedules (built above); its ring instance of width f needs its attribute
+    if (ring && f <= 512 && (rc = sddmm_attr(p, f, p->host_stream))) return rc;
     p->prepared = true;
+    return 0;
+}
+
+int pgcn_plan_bind_values(pgcn_plan* p)
+{
+    if (!p) return fail(nullptr, PGCN_ERR_INVALID, "null plan");
+    if (p->bound) return 0;
+    CU(p, cudaSetDevice(p->device));
+    const int64_t nnz = p->fwd.nnz;
+    const int64_t ncol = (int64_t)p->m + p->h;
+    std::vector<int> fcol, fval, frow, tcol, tval, trow;
+    int rc;
+    if ((rc = decode_records(p, p->fwd, fcol, fval, frow))) return rc;
+    if ((rc = decode_records(p, p->tr, tcol, tval, trow))) return rc;
+    if (p->tr.nnz != nnz) return fail(p, PGCN_ERR_INVALID, "transposed CSR holds %lld entries, the forward CSR %lld",
+                                      (long long)p->tr.nnz, (long long)nnz);
+    // forward entries in (column, row) order: a stable counting sort by column of the row-major entries (duplicates
+    // keep their order of appearance)
+    std::vector<int64_t> cstart((size_t)ncol + 1, 0);
+    for (int64_t e = 0; e < nnz; ++e) ++cstart[(size_t)fcol[(size_t)e] + 1];
+    for (int64_t c = 0; c < ncol; ++c) cstart[(size_t)c + 1] += cstart[(size_t)c];
+    std::vector<int> fsorted((size_t)nnz);
+    {
+        std::vector<int64_t> pos(cstart.begin(), cstart.end() - 1);
+        for (int64_t e = 0; e < nnz; ++e) fsorted[(size_t)pos[(size_t)fcol[(size_t)e]]++] = (int)e;
+    }
+    // transposed entries: row-major over the forward columns already; order each row by forward row (stable)
+    std::vector<int> tsorted((size_t)nnz);
+    for (int64_t e = 0; e < nnz; ++e) tsorted[(size_t)e] = (int)e;
+    for (int64_t s = 0; s < nnz;) {
+        int64_t t = s + 1;
+        while (t < nnz && trow[(size_t)t] == trow[(size_t)s]) ++t;
+        std::stable_sort(tsorted.begin() + s, tsorted.begin() + t, [&](int x, int y) { return tcol[(size_t)x] < tcol[(size_t)y]; });
+        s = t;
+    }
+    std::vector<int> tmap((size_t)nnz);
+    for (int64_t i = 0; i < nnz; ++i) {
+        const int fe = fsorted[(size_t)i], te = tsorted[(size_t)i];
+        if (fcol[(size_t)fe] != trow[(size_t)te] || frow[(size_t)fe] != tcol[(size_t)te])
+            return fail(p, PGCN_ERR_INVALID, "the transposed CSR does not hold the forward entries: transposed entry %d (row %d, "
+                        "column %d) has no forward entry (row %d, column %d) to match", te, trow[(size_t)te], tcol[(size_t)te],
+                        tcol[(size_t)te], trow[(size_t)te]);
+        if (fval[(size_t)fe] != tval[(size_t)te])
+            return fail(p, PGCN_ERR_INVALID, "transposed entry %d (row %d, column %d) has another value than its forward entry %d",
+                        te, trow[(size_t)te], tcol[(size_t)te], fe);
+        tmap[(size_t)te] = fe;
+    }
+    // own-column and per-peer blocks: the forward entries in forward order, split by column (as pgcn_plan_create did)
+    std::vector<int> omap;
+    std::vector<std::vector<int>> qmap;
+    if (p->have_split) {
+        std::vector<int> col_peer((size_t)p->h);
+        for (int q = 0; q < p->k; ++q)
+            for (int64_t c = p->recv_off[(size_t)q]; c < p->recv_off[(size_t)q + 1]; ++c) col_peer[(size_t)c] = q;
+        qmap.resize((size_t)p->k);
+        for (int64_t e = 0; e < nnz; ++e) {
+            const int c = fcol[(size_t)e];
+            if (c < p->m) omap.push_back((int)e);
+            else qmap[(size_t)col_peer[(size_t)(c - p->m)]].push_back((int)e);
+        }
+        if ((int64_t)omap.size() != p->own.nnz) return fail(p, PGCN_ERR_STATE, "own-column block does not match the forward CSR");
+        for (int q = 0; q < p->k; ++q)
+            if ((int64_t)qmap[(size_t)q].size() != p->halo_q[(size_t)q].nnz)
+                return fail(p, PGCN_ERR_STATE, "halo block of peer %d does not match the forward CSR", q);
+    }
+    // device side: maps, creation values, the set table of the rewrite kernel
+    std::vector<ValueSet> sets;
+    long long total = 0;
+    auto add = [&](DevCsr& c, const std::vector<int>* map) -> int {
+        if (c.nnz == 0) return 0;
+        if (map) { int r2 = upload_setup(p, &c.d_vmap, map->data(), map->size()); if (r2) return r2; }
+        ValueSet s;
+        s.cw = c.d_cw; s.map = map ? c.d_vmap : nullptr; s.nnz = c.nnz; s.start = total;
+        total += c.nnz;
+        sets.push_back(s);
+        return 0;
+    };
+    if ((rc = add(p->fwd, nullptr))) return rc;
+    if ((rc = add(p->tr, &tmap))) return rc;
+    if (p->have_split) {
+        if ((rc = add(p->own, &omap))) return rc;
+        for (int q = 0; q < p->k; ++q)
+            if ((rc = add(p->halo_q[(size_t)q], &qmap[(size_t)q]))) return rc;
+    }
+    if ((rc = upload_setup(p, &p->d_vals0, reinterpret_cast<const float*>(fval.data()), fval.size()))) return rc;
+    if ((rc = upload_setup(p, &p->d_vsets, sets.data(), sets.size()))) return rc;
+    p->nvsets = (int)sets.size();
+    p->vtotal = total;
+    p->bound = true;
+    return 0;
+}
+
+int pgcn_plan_set_values(pgcn_plan* p, const float* vals, void* stream)
+{
+    if (!p) return fail(nullptr, PGCN_ERR_INVALID, "null plan");
+    if (!p->bound) return fail(p, PGCN_ERR_STATE, "pgcn_plan_set_values needs the value maps: call pgcn_plan_bind_values first");
+    if (p->vtotal == 0) return 0;
+    cudaStream_t st = (cudaStream_t)stream;
+    set_values_kernel<<<grid_for(p->vtotal, p->num_sms), 256, 0, st>>>(p->d_vsets, p->nvsets, p->vtotal, vals ? vals : p->d_vals0);
+    ++p->launches;
+    CU(p, cudaGetLastError());
     return 0;
 }
 
@@ -1604,6 +1841,35 @@ int pgcn_backward(pgcn_plan* p, const float* gZ, float* G_own, int32_t f, void* 
     }
     CU(p, cudaStreamWaitEvent(st, p->ev_b, 0));      // NCCL: all blocks received; p2p: the send slab is free again
     return launch_unpack(p, rrecv, G_own, f, st, rrecv_odd);
+}
+
+int pgcn_forward_keep_halo(pgcn_plan* p, const float* H_own, float* Z, float* H_halo_out, int32_t f, void* stream)
+{
+    int rc = check_f(p, f);
+    if (rc) return rc;
+    if (p->k > 1 && p->h > 0 && !H_halo_out) return fail(p, PGCN_ERR_INVALID, "h=%d but H_halo_out is null", p->h);
+    if ((rc = pgcn_forward(p, H_own, Z, f, stream))) return rc;
+    if (p->k == 1 || p->h == 0) return 0;
+    // the stream has waited for every source's rows; the peer transport's rows sit in the slab of this call's parity,
+    // which the next fused call of the same parity overwrites: copy them now, picking the slab from the device epoch
+    cudaStream_t st = (cudaStream_t)stream;
+    const bool use_p2p = p->p2p && (f % 4 == 0);
+    const float* src = use_p2p ? arena_ptr(p->arena, p->off_fwd[0]) : p->d_halo_slab;
+    const float* src_odd = use_p2p ? arena_ptr(p->arena, p->off_fwd[1]) : nullptr;
+    const long long n = (long long)p->h * f;
+    copy_halo_kernel<<<grid_for(n, p->num_sms), 256, 0, st>>>(src, src_odd, use_p2p ? p->d_epoch : nullptr, H_halo_out, n);
+    ++p->launches;
+    CU(p, cudaGetLastError());
+    return 0;
+}
+
+int pgcn_sddmm(pgcn_plan* p, const float* gZ, const float* H_own, const float* H_halo, float* dvals, int32_t f, void* stream)
+{
+    int rc = check_f(p, f);
+    if (rc) return rc;
+    if (p->fwd.nnz > 0 && (!gZ || !H_own || !dvals)) return fail(p, PGCN_ERR_INVALID, "null gZ/H_own/dvals");
+    if (p->h > 0 && !H_halo) return fail(p, PGCN_ERR_INVALID, "h=%d but H_halo is null", p->h);
+    return launch_sddmm(p, gZ, H_own, p->h > 0 ? H_halo : nullptr, dvals, f, (cudaStream_t)stream);
 }
 
 static int host_slots(pgcn_plan* p, int64_t need)

@@ -44,6 +44,7 @@ def aggregate_forward(plan, H_own, relu=False):
     Z = torch.empty((plan.m, f), dtype=torch.float32, device=H_own.device)
     lib = cabi.load()
     with torch.cuda.device(H_own.device):
+        plan.use_values(None)             # PSpMM / PSpMMRelu aggregate with the plan's own values
         if relu:
             plan.set_option("relu", 1)
         try:
@@ -63,6 +64,7 @@ def aggregate_backward(plan, gZ_own):
     G = torch.empty((plan.m, f), dtype=torch.float32, device=gZ_own.device)
     lib = cabi.load()
     with torch.cuda.device(gZ_own.device):
+        plan.use_values(None)
         cabi.check(lib.pgcn_backward(plan.handle, gZ_own.data_ptr(), G.data_ptr(), f, _stream_ptr()), plan.handle)
     if plan.lp.k > 1:
         plan.count_exchange(backward=True)
@@ -112,6 +114,88 @@ class PSpMMRelu(torch.autograd.Function):
     def backward(ctx, grad_output):
         (out,) = ctx.saved_tensors
         return None, aggregate_backward(ctx.plan, grad_output * (out > 0))
+
+
+class PSpMMWeighted(torch.autograd.Function):
+    """Z = A(vals) * H with the edge values given per call, like torch.sparse.mm(A, H) on a sparse A whose values
+    require grad (GPU/PGCN.py:127 with learned edge weights, an edge mask or attention scores).
+
+        PSpMMWeighted.apply(A, vals, H)     vals = fp32 CUDA [nnz] in A's local forward CSR order (A.edge_index())
+
+    Backward returns (None, dvals, dH): dH = A(vals)^T gZ with the exchange (pgcn_backward, vals resident), and, when
+    vals needs grad, dvals[e] = <gZ[row(e)], [H_own; H_halo][col(e)]> from the SDDMM kernel (pgcn_sddmm); on k > 1 the
+    forward keeps the halo rows it received for it (pgcn_forward_keep_halo). Several layers may share one plan with
+    different values: each launch first makes its own values resident (PgcnPlan.use_values). Layouts as PSpMM.
+
+    The plan must be bound first (PgcnPlan.bind_values, synchronous set-up). A rewrite is skipped when `vals` is the
+    tensor set last and its version counter has not moved: in-place updates through autograd-visible ops (optimizer
+    steps, `with torch.no_grad(): w.mul_(...)`) are seen, writes through `w.data` or raw pointers are not — call
+    A.set_values(w) after those."""
+
+    @staticmethod
+    def forward(ctx, A, vals, H):
+        from .plan import check_values
+        check_values(A, vals)
+        ctx.plan = A
+        ctx.glob = A.layout == "global"
+        if ctx.glob:
+            _check_feat(A, H, A.n, "H")
+            H_own = H.index_select(0, A.owned_index())
+        else:
+            H_own = _check_feat(A, H, A.m, "H")
+        lp = A.lp
+        f = H_own.shape[1]
+        want_dvals = ctx.needs_input_grad[1]
+        keep = want_dvals and lp.k > 1 and lp.h > 0
+        Z = torch.empty((lp.m, f), dtype=torch.float32, device=H_own.device)
+        H_halo = torch.empty((lp.h, f), dtype=torch.float32, device=H_own.device) if keep else None
+        lib = cabi.load()
+        with torch.cuda.device(H_own.device):
+            A.use_values(vals)
+            if keep:
+                cabi.check(lib.pgcn_forward_keep_halo(A.handle, H_own.data_ptr(), Z.data_ptr(), H_halo.data_ptr(), f,
+                                                      _stream_ptr()), A.handle)
+            else:
+                cabi.check(lib.pgcn_forward(A.handle, H_own.data_ptr(), Z.data_ptr(), f, _stream_ptr()), A.handle)
+        if lp.k > 1:
+            A.count_exchange(backward=False)
+        ctx.save_for_backward(vals, H_own if want_dvals else None, H_halo)
+        if ctx.glob:
+            Zg = torch.zeros((A.n, f), dtype=torch.float32, device=H.device)
+            Zg.index_copy_(0, A.owned_index(), Z)
+            return Zg
+        return Z
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        A = ctx.plan
+        vals, H_own, H_halo = ctx.saved_tensors
+        if ctx.glob:
+            g = _check_feat(A, grad_output, A.n, "grad_output").index_select(0, A.owned_index())
+        else:
+            g = _check_feat(A, grad_output, A.m, "grad_output")
+        lp = A.lp
+        f = g.shape[1]
+        lib = cabi.load()
+        dvals = dH = None
+        with torch.cuda.device(g.device):
+            if ctx.needs_input_grad[2]:
+                A.use_values(vals)
+                G = torch.empty((lp.m, f), dtype=torch.float32, device=g.device)
+                cabi.check(lib.pgcn_backward(A.handle, g.data_ptr(), G.data_ptr(), f, _stream_ptr()), A.handle)
+                if lp.k > 1:
+                    A.count_exchange(backward=True)
+                if ctx.glob:
+                    dH = torch.zeros((A.n, f), dtype=torch.float32, device=g.device)
+                    dH.index_copy_(0, A.owned_index(), G)
+                else:
+                    dH = G
+            if ctx.needs_input_grad[1]:
+                dvals = torch.empty((lp.nnz(),), dtype=torch.float32, device=g.device)
+                cabi.check(lib.pgcn_sddmm(A.handle, g.data_ptr(), H_own.data_ptr(),
+                                          H_halo.data_ptr() if H_halo is not None else None, dvals.data_ptr(), f,
+                                          _stream_ptr()), A.handle)
+        return None, dvals, dH
 
 
 # ---- the pieces, individually callable (NCCL transport), mirroring communicate_fgm ----------------

@@ -230,6 +230,12 @@ class PgcnPlan:
                 lp.k, lp.rank, self.f_max, C.byref(self._h))
         cabi.check(rc, None)
         self._owned_t = None
+        self._edge_index = None
+        # edge values (bind_values / set_values): which values the records hold, as far as this process knows
+        self._bound = False
+        self._resident = "creation"      # "creation", a key of the tensor set last, or None: unknown
+        self._resident_ref = None        # that tensor, kept alive so that its key cannot be reused
+        self._captured = False           # values were set inside a CUDA-graph capture: replays change them unseen
 
     # -- lifetime ------------------------------------------------------------------------------
     def close(self):
@@ -284,6 +290,72 @@ class PgcnPlan:
         self.owned_index()                # the "global" layout's index tensor: a host-to-device copy, not capturable
         with torch.cuda.device(self.device):
             cabi.check(self._lib.pgcn_plan_prepare(self.handle, int(f)), self._h)
+
+    # -- edge values ---------------------------------------------------------------------------
+    def bind_values(self):
+        """Build the maps set_values needs (pgcn_plan_bind_values): synchronous set-up, not capturable; 4 B per edge and
+        record set, about 8 B per edge on one rank and 12 B on a split multi-rank plan. Idempotent."""
+        import torch
+        if self._bound:
+            return
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("PgcnPlan.bind_values is set-up work and cannot run while a CUDA graph is being captured: "
+                               "call it before the capture")
+        with torch.cuda.device(self.device):
+            cabi.check(self._lib.pgcn_plan_bind_values(self.handle), self._h)
+        self._bound = True
+
+    def set_values(self, vals):
+        """Aggregate with `vals` (fp32 CUDA [nnz], this plan's local forward CSR order, i.e. lp.colidx's order) from now on,
+        stream-ordered on the current stream; None restores the values the plan was created with. Needs bind_values."""
+        import torch
+        ptr = None
+        if vals is not None:
+            ptr = check_values(self, vals).data_ptr()
+        with torch.cuda.device(self.device):
+            cabi.check(self._lib.pgcn_plan_set_values(self.handle, ptr, torch.cuda.current_stream().cuda_stream), self._h)
+        if torch.cuda.is_current_stream_capturing():
+            # what the device holds after the capture depends on which graphs are replayed: never trust a record again
+            self._captured = True
+            self._resident, self._resident_ref = None, None
+        elif vals is None:
+            self._resident, self._resident_ref = "creation", None
+        else:
+            self._resident, self._resident_ref = _values_key(vals), vals
+
+    def use_values(self, vals):
+        """Make `vals` (None: the creation values) the resident values before a launch on the current stream.
+
+        Skips the rewrite when this plan last set the same tensor eagerly and its version counter has not moved since.
+        Writes that bypass the counter (`w.data.copy_(...)`, assigning `w.data`, DLPack or raw-pointer kernels) are not
+        seen: after such a write call set_values(w) yourself. On a plan that was never bound, None costs nothing and a
+        tensor raises (bind_values is synchronous set-up and is not done implicitly). Under CUDA-graph capture, and on a
+        plan whose values were ever set inside a capture, it always rewrites, so that a graph never depends on what was
+        resident when it was captured or replayed; such a plan pays one set_values launch (0.34 ms on C2, DESIGN.md §6)
+        before every later PSpMM / PSpMMRelu forward and backward as well."""
+        import torch
+        if not self._bound:
+            if vals is None:
+                return
+            raise RuntimeError("edge values need the plan's value maps: call PgcnPlan.bind_values() once (set-up, "
+                               "before any CUDA-graph capture) before PSpMMWeighted or set_values")
+        if not torch.cuda.is_current_stream_capturing() and not self._captured:
+            if vals is None and self._resident == "creation":
+                return
+            if vals is not None and self._resident_ref is vals and self._resident == _values_key(vals):
+                return
+        self.set_values(vals)
+
+    def edge_index(self):
+        """(row, col) of every forward entry, int64 CUDA tensors in the order of the values set_values takes: rows in
+        [0, m) (global id lp.owned[row]), columns in [0, m + h) (own rows, then the halo rows lp.halo[col - m])."""
+        import torch
+        if self._edge_index is None:
+            lp = self.lp
+            rows = np.repeat(np.arange(lp.m, dtype=np.int64), np.diff(lp.rowptr.astype(np.int64)))
+            self._edge_index = (torch.from_numpy(rows).to(self.device),
+                                torch.from_numpy(lp.colidx.astype(np.int64)).to(self.device))
+        return self._edge_index
 
     def algorithmic_bytes(self, f):
         b = cabi.PgcnBytes()
@@ -363,6 +435,25 @@ class PgcnPlan:
         self.stats["recv_volume"] += int(in_rows)
         self.stats["send_nmsg"] += lp.k - 1
         self.stats["recv_nmsg"] += lp.k - 1
+
+
+def _values_key(vals):
+    return (id(vals), vals.data_ptr(), vals._version)
+
+
+def check_values(plan, vals):
+    """Edge values for `plan`: fp32 CUDA [nnz] on the plan's device. Returns them contiguous."""
+    import torch
+    if not torch.is_tensor(vals) or not vals.is_cuda:
+        raise RuntimeError("edge values must be a CUDA tensor: the PGCN H100 path has no CPU fallback")
+    if vals.dtype != torch.float32:
+        raise TypeError("edge values must be float32, got %s" % vals.dtype)
+    nnz = plan.lp.nnz()
+    if vals.dim() != 1 or vals.shape[0] != nnz:
+        raise ValueError("edge values must be [%d] (the plan's nnz), got %s" % (nnz, tuple(vals.shape)))
+    if vals.device != plan.device:
+        raise ValueError("edge values live on %s, the plan on %s" % (vals.device, plan.device))
+    return vals.detach().contiguous()
 
 
 def link_local_plans(plans):
