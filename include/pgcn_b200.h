@@ -273,6 +273,33 @@ int pgcn_sddmm(pgcn_plan* plan, const float* gZ, const float* H_own, const float
                void* stream);
 int pgcn_forward_keep_halo(pgcn_plan* plan, const float* H_own, float* Z, float* H_halo_out, int32_t f, void* stream);
 
+/* ---- sparse graph attention: the edge softmax of GPU/PGAT.py:139-148 over the stored pattern ---------------------- */
+/*
+ * With el (m floats, one per owned row) and er (one per column: er_own, m floats, then er_halo, h floats, the halo
+ * rows' values from pgcn_halo_rows; er_halo may be NULL when h == 0):
+ *   s_e = LeakyReLU(el[row(e)] + er[col(e)], negative_slope)          for every forward entry e
+ *   alpha_e = exp(s_e - max_row s) / sum_row exp(s - max_row s)        over the stored entries of row(e) only
+ * pgcn_edge_softmax writes alpha (nnz floats, forward CSR order: what pgcn_plan_set_values takes). Rows without entries
+ *   write nothing. Full-precision expf with the row maximum subtracted: no overflow for any row length or score.
+ * pgcn_edge_softmax_backward: given alpha and dalpha (nnz, e.g. pgcn_sddmm of the output gradient against the
+ *   aggregated rows), writes dpre_e = alpha_e (dalpha_e - sum_row alpha dalpha) * (s_e > 0 ? 1 : negative_slope)
+ *   (nnz floats) and d_el[i] = sum over row i of dpre (m floats, 0 for empty rows). The gradient of er is the column
+ *   sum of dpre over all ranks: pgcn_plan_set_values(dpre), then pgcn_backward on an m x 4 matrix of ones (column 0).
+ *   Both kernels give a warp to each row and a CTA to each row of more than 1024 entries; every output is reduced in
+ *   one fixed order, so runs are bit-identical.
+ * pgcn_halo_rows: the forward exchange of pgcn_forward without the SpMM. X_own is m x w (this rank's owned rows), the
+ *   h halo rows it receives are copied into X_halo_out (h x w) on `stream`. Peer transport when imported and
+ *   w % 4 == 0 (the device epoch advances as in every fused call), NCCL otherwise. k == 1: nothing to do.
+ * All three need pgcn_plan_bind_values (PGCN_ERR_STATE before) and do no set-up work of their own: they are capturable
+ *   once the plan is bound (and, for the exchange, wired). A null plan or a null argument returns PGCN_ERR_INVALID.
+ */
+int pgcn_edge_softmax(pgcn_plan* plan, const float* el, const float* er_own, const float* er_halo, float negative_slope,
+                      float* alpha, void* stream);
+int pgcn_edge_softmax_backward(pgcn_plan* plan, const float* el, const float* er_own, const float* er_halo,
+                               const float* alpha, const float* dalpha, float negative_slope, float* dpre, float* d_el,
+                               void* stream);
+int pgcn_halo_rows(pgcn_plan* plan, const float* X_own, float* X_halo_out, int32_t w, void* stream);
+
 /* ---- host-buffer variant: what a non-torch host (the reference's C path) would bind -------- */
 /*
  * Same as pgcn_forward but H and Z are HOST pointers (pinned or pageable): copies H to the

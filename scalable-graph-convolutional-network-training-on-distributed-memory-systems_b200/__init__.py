@@ -16,10 +16,10 @@ __version__ = "0.1"
 
 def __getattr__(name):
     # torch-dependent pieces are imported lazily so `import pgcn_b200` stays cheap
-    if name in ("op", "pgcn", "minibatch"):
+    if name in ("op", "pgcn", "pgat", "minibatch"):
         import importlib
         return importlib.import_module("." + name, __name__)
-    if name in ("PSpMM", "PSpMMWeighted", "aggregate_forward", "aggregate_backward"):
+    if name in ("PSpMM", "PSpMMWeighted", "PGATAttention", "aggregate_forward", "aggregate_backward"):
         from . import op
         return getattr(op, name)
     raise AttributeError(name)

@@ -21,6 +21,7 @@ SYMBOLS = [
     "pgcn_spmm", "pgcn_pack", "pgcn_exchange", "pgcn_unpack_add",
     "pgcn_forward", "pgcn_backward", "pgcn_forward_host", "pgcn_forward_host_async", "pgcn_forward_host_wait",
     "pgcn_plan_bind_values", "pgcn_plan_set_values", "pgcn_sddmm", "pgcn_forward_keep_halo",
+    "pgcn_edge_softmax", "pgcn_edge_softmax_backward", "pgcn_halo_rows",
 ]
 
 
@@ -118,6 +119,12 @@ def load(build_if_missing=True):
     lib.pgcn_sddmm.argtypes = [vp, vp, vp, vp, vp, i32, vp]
     lib.pgcn_forward_keep_halo.restype = C.c_int
     lib.pgcn_forward_keep_halo.argtypes = [vp, vp, vp, vp, i32, vp]
+    lib.pgcn_edge_softmax.restype = C.c_int
+    lib.pgcn_edge_softmax.argtypes = [vp, vp, vp, vp, C.c_float, vp, vp]
+    lib.pgcn_edge_softmax_backward.restype = C.c_int
+    lib.pgcn_edge_softmax_backward.argtypes = [vp, vp, vp, vp, vp, vp, C.c_float, vp, vp, vp]
+    lib.pgcn_halo_rows.restype = C.c_int
+    lib.pgcn_halo_rows.argtypes = [vp, vp, vp, i32, vp]
     _lib = lib
     return lib
 

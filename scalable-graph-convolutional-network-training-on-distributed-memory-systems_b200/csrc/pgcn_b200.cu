@@ -9,6 +9,7 @@
 #include "spmm_kernels.cuh"
 #include "spmm_ring.cuh"
 #include "sddmm.cuh"
+#include "attention.cuh"
 
 #include <dlfcn.h>
 #include <unistd.h>
@@ -192,6 +193,9 @@ struct pgcn_plan {
     long long vtotal = 0;                  // entries over all sets
     bool sddmm_attr_set[5] = {false};      // per f / 128 of the SDDMM ring kernel
     int sddmm_ctas_per_sm[5] = {0};
+    int* d_rowptr = nullptr;               // m + 1, the forward rowptr (edge softmax)
+    int* d_long_rows = nullptr;            // rows of more than kAttnLongRow entries (one CTA each in the edge softmax)
+    int nlong_rows = 0;
 
     // host-buffer variant: two device slots, copy-in / compute / copy-out streams chained by events
     float* d_hostH[2] = {nullptr, nullptr}; float* d_hostZ[2] = {nullptr, nullptr}; int64_t host_cap = 0;
@@ -546,6 +550,7 @@ void preload_kernels()
     touch_kernel(set_values_kernel); touch_kernel(copy_halo_kernel); touch_kernel(sddmm_plain_kernel);
     touch_kernel(sddmm_ring_kernel<1>); touch_kernel(sddmm_ring_kernel<2>);
     touch_kernel(sddmm_ring_kernel<3>); touch_kernel(sddmm_ring_kernel<4>);
+    touch_kernel(edge_softmax_kernel); touch_kernel(edge_softmax_backward_kernel);
 }
 
 bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
@@ -1173,7 +1178,7 @@ int pgcn_plan_destroy(pgcn_plan* p)
     if (p->s_out) cudaStreamDestroy(p->s_out);
     cudaFree(p->d_counter);
     cudaFree(p->d_epoch);
-    cudaFree(p->d_vals0); cudaFree(p->d_vsets);
+    cudaFree(p->d_vals0); cudaFree(p->d_vsets); cudaFree(p->d_rowptr); cudaFree(p->d_long_rows);
     for (void* q : p->retired) cudaFree(q);
     if (p->comm_stream) cudaStreamDestroy(p->comm_stream);
     if (p->host_stream) cudaStreamDestroy(p->host_stream);
@@ -1515,6 +1520,16 @@ int pgcn_plan_bind_values(pgcn_plan* p)
     }
     if ((rc = upload_setup(p, &p->d_vals0, reinterpret_cast<const float*>(fval.data()), fval.size()))) return rc;
     if ((rc = upload_setup(p, &p->d_vsets, sets.data(), sets.size()))) return rc;
+    // the edge softmax walks the forward rows: their rowptr, and the rows long enough for a CTA each
+    std::vector<int> rowptr((size_t)p->m + 1, 0), long_rows;
+    for (int64_t e = 0; e < nnz; ++e) ++rowptr[(size_t)frow[(size_t)e] + 1];
+    for (int i = 0; i < p->m; ++i) {
+        if (rowptr[(size_t)i + 1] > kAttnLongRow) long_rows.push_back(i);
+        rowptr[(size_t)i + 1] += rowptr[(size_t)i];
+    }
+    if ((rc = upload_setup(p, &p->d_rowptr, rowptr.data(), rowptr.size()))) return rc;
+    if ((rc = upload_setup(p, &p->d_long_rows, long_rows.data(), long_rows.size()))) return rc;
+    p->nlong_rows = (int)long_rows.size();
     p->nvsets = (int)sets.size();
     p->vtotal = total;
     p->bound = true;
@@ -1730,6 +1745,44 @@ static int nccl_step(pgcn_plan* p, const float* send, float* recv, int f, int re
     return 0;
 }
 
+// Send half of the forward exchange, shared by pgcn_forward and pgcn_halo_rows: the owned rows leave for every peer in
+// step order. Peer transport: the device epoch advances on `st` (every call of the plan that exchanges does this once,
+// which is what picks the slab parity) and the rows are stored into each peer's slab of the new parity. NCCL: they are
+// packed and sent, and each source's block is received into the halo slab. With `split` the sends run on the exchange
+// stream, after `st`'s earlier work; ev_step[i] (NCCL) and ev_b (peer transport) mark their progress.
+static int forward_send(pgcn_plan* p, const float* H_own, int f, bool use_p2p, bool split, cudaStream_t st)
+{
+    int rc;
+    if (use_p2p && (rc = advance_epoch(p, st))) return rc;
+    cudaStream_t cs = split ? p->comm_stream : st;
+    if (split) {
+        CU(p, cudaEventRecord(p->ev_a, st));
+        CU(p, cudaStreamWaitEvent(cs, p->ev_a, 0));
+    }
+    if (use_p2p) {
+        for (int i = 1; i < p->k; ++i)
+            if ((rc = p2p_put(p, step_dst(p, i), H_own, f, false, cs))) return rc;
+        if (split) CU(p, cudaEventRecord(p->ev_b, cs));                   // H_own is free for the caller after this
+    } else {
+        if ((rc = launch_pack(p, H_own, p->d_send_slab, f, cs))) return rc;
+        for (int i = 1; i < p->k; ++i) {
+            if ((rc = nccl_step(p, p->d_send_slab, p->d_halo_slab, f, 0, i, cs))) return rc;
+            if (split) CU(p, cudaEventRecord(p->ev_step[(size_t)i], cs));
+        }
+    }
+    return 0;
+}
+
+// Wait half of an unsplit forward exchange: `st` waits for every source's rows (NCCL received them on `st` already).
+static int forward_wait_all(pgcn_plan* p, bool use_p2p, cudaStream_t st)
+{
+    int rc;
+    if (use_p2p)
+        for (int i = 1; i < p->k; ++i)
+            if ((rc = p2p_wait(p, step_src(p, i), st))) return rc;
+    return 0;
+}
+
 int pgcn_forward(pgcn_plan* p, const float* H_own, float* Z, int32_t f, void* stream)
 {
     int rc = check_f(p, f);
@@ -1744,35 +1797,12 @@ int pgcn_forward(pgcn_plan* p, const float* H_own, float* Z, int32_t f, void* st
     if (!use_p2p && !p->comm) return fail(p, PGCN_ERR_STATE, "k=%d: call pgcn_comm_init or pgcn_p2p_import first", p->k);
     const bool split = p->have_split && p->opt_overlap;
     const int k = p->k;
-    float* halo = p->d_halo_slab;
-    const float* halo_odd = nullptr;
-    if (use_p2p) {
-        if ((rc = advance_epoch(p, st))) return rc;
-        halo = arena_ptr(p->arena, p->off_fwd[0]);
-        halo_odd = arena_ptr(p->arena, p->off_fwd[1]);
-    }
-    cudaStream_t cs = split ? p->comm_stream : st;
-    if (split) {
-        CU(p, cudaEventRecord(p->ev_a, st));
-        CU(p, cudaStreamWaitEvent(cs, p->ev_a, 0));
-    }
-    // ---- send side (exchange stream): one peer after the other, in step order
-    if (use_p2p) {
-        for (int i = 1; i < k; ++i)
-            if ((rc = p2p_put(p, step_dst(p, i), H_own, f, false, cs))) return rc;
-        if (split) CU(p, cudaEventRecord(p->ev_b, cs));                   // H_own is free for the caller after this
-    } else {
-        if ((rc = launch_pack(p, H_own, p->d_send_slab, f, cs))) return rc;
-        for (int i = 1; i < k; ++i) {
-            if ((rc = nccl_step(p, p->d_send_slab, halo, f, 0, i, cs))) return rc;
-            if (split) CU(p, cudaEventRecord(p->ev_step[(size_t)i], cs));
-        }
-    }
+    float* halo = use_p2p ? arena_ptr(p->arena, p->off_fwd[0]) : p->d_halo_slab;
+    const float* halo_odd = use_p2p ? arena_ptr(p->arena, p->off_fwd[1]) : nullptr;
+    if ((rc = forward_send(p, H_own, f, use_p2p, split, st))) return rc;
     if (!split) {
         // no overlap requested (or nothing to split): wait for every block, then one pass over [own | halo]
-        if (use_p2p)
-            for (int i = 1; i < k; ++i)
-                if ((rc = p2p_wait(p, step_src(p, i), st))) return rc;
+        if ((rc = forward_wait_all(p, use_p2p, st))) return rc;
         return launch_spmm(p, p->fwd, H_own, p->h > 0 ? halo : nullptr, p->m, Z, nullptr, p->m, f, 0, st, relu, false,
                            p->h > 0 ? halo_odd : nullptr);
     }
@@ -1870,6 +1900,86 @@ int pgcn_sddmm(pgcn_plan* p, const float* gZ, const float* H_own, const float* H
     if (p->fwd.nnz > 0 && (!gZ || !H_own || !dvals)) return fail(p, PGCN_ERR_INVALID, "null gZ/H_own/dvals");
     if (p->h > 0 && !H_halo) return fail(p, PGCN_ERR_INVALID, "h=%d but H_halo is null", p->h);
     return launch_sddmm(p, gZ, H_own, p->h > 0 ? H_halo : nullptr, dvals, f, (cudaStream_t)stream);
+}
+
+// ---- sparse graph attention --------------------------------------------------------------------
+
+int pgcn_halo_rows(pgcn_plan* p, const float* X_own, float* X_halo_out, int32_t w, void* stream)
+{
+    int rc = check_f(p, w);
+    if (rc) return rc;
+    if (!p->bound) return fail(p, PGCN_ERR_STATE, "pgcn_halo_rows: call pgcn_plan_bind_values first");
+    if (p->k == 1) return 0;
+    if (p->m > 0 && !X_own) return fail(p, PGCN_ERR_INVALID, "null X_own");
+    if (p->h > 0 && !X_halo_out) return fail(p, PGCN_ERR_INVALID, "h=%d but X_halo_out is null", p->h);
+    const bool use_p2p = p->p2p && (w % 4 == 0);
+    if (!use_p2p && !p->comm) return fail(p, PGCN_ERR_STATE, "k=%d: call pgcn_comm_init or pgcn_p2p_import first", p->k);
+    cudaStream_t st = (cudaStream_t)stream;
+    if ((rc = forward_send(p, X_own, w, use_p2p, false, st))) return rc;
+    if ((rc = forward_wait_all(p, use_p2p, st))) return rc;
+    if (p->h == 0) return 0;
+    const float* src = use_p2p ? arena_ptr(p->arena, p->off_fwd[0]) : p->d_halo_slab;
+    const float* src_odd = use_p2p ? arena_ptr(p->arena, p->off_fwd[1]) : nullptr;
+    const long long n = (long long)p->h * w;
+    copy_halo_kernel<<<grid_for(n, p->num_sms), 256, 0, st>>>(src, src_odd, use_p2p ? p->d_epoch : nullptr, X_halo_out, n);
+    ++p->launches;
+    CU(p, cudaGetLastError());
+    return 0;
+}
+
+static int attn_check(pgcn_plan* p, const char* what, const float* el, const float* er_own, const float* er_halo)
+{
+    if (!p) return fail(nullptr, PGCN_ERR_INVALID, "null plan");
+    if (!p->bound) return fail(p, PGCN_ERR_STATE, "%s walks the forward rows: call pgcn_plan_bind_values first", what);
+    if (p->m > 0 && (!el || !er_own)) return fail(p, PGCN_ERR_INVALID, "%s: null el/er_own", what);
+    if (p->h > 0 && !er_halo) return fail(p, PGCN_ERR_INVALID, "%s: h=%d but er_halo is null", what, p->h);
+    return 0;
+}
+
+static int launch_attn(pgcn_plan* p, bool backward, const AttnArgs& a, cudaStream_t st)
+{
+    const unsigned grid = (unsigned)p->nlong_rows + (unsigned)((p->m + kAttnWarps - 1) / kAttnWarps);
+    if (backward) edge_softmax_backward_kernel<<<grid, kAttnThreads, 0, st>>>(a);
+    else edge_softmax_kernel<<<grid, kAttnThreads, 0, st>>>(a);
+    ++p->launches;
+    CU(p, cudaGetLastError());
+    return 0;
+}
+
+static AttnArgs attn_args(const pgcn_plan* p, const float* el, const float* er_own, const float* er_halo, float slope)
+{
+    AttnArgs a;
+    a.rowptr = p->d_rowptr; a.long_rows = p->d_long_rows; a.nlong = p->nlong_rows; a.m = p->m;
+    a.pieces = p->fwd.d_cw;
+    a.el = el; a.er_own = er_own; a.er_halo = p->h > 0 ? er_halo : nullptr; a.slope = slope;
+    a.alpha = a.dalpha = nullptr; a.out = a.d_el = nullptr;
+    return a;
+}
+
+int pgcn_edge_softmax(pgcn_plan* p, const float* el, const float* er_own, const float* er_halo, float negative_slope,
+                      float* alpha, void* stream)
+{
+    int rc = attn_check(p, "pgcn_edge_softmax", el, er_own, er_halo);
+    if (rc) return rc;
+    if (p->m == 0) return 0;
+    if (p->fwd.nnz > 0 && !alpha) return fail(p, PGCN_ERR_INVALID, "null alpha");
+    AttnArgs a = attn_args(p, el, er_own, er_halo, negative_slope);
+    a.out = alpha;
+    return launch_attn(p, false, a, (cudaStream_t)stream);
+}
+
+int pgcn_edge_softmax_backward(pgcn_plan* p, const float* el, const float* er_own, const float* er_halo,
+                               const float* alpha, const float* dalpha, float negative_slope, float* dpre, float* d_el,
+                               void* stream)
+{
+    int rc = attn_check(p, "pgcn_edge_softmax_backward", el, er_own, er_halo);
+    if (rc) return rc;
+    if (p->m == 0) return 0;
+    if (!d_el || (p->fwd.nnz > 0 && (!alpha || !dalpha || !dpre)))
+        return fail(p, PGCN_ERR_INVALID, "null alpha/dalpha/dpre/d_el");
+    AttnArgs a = attn_args(p, el, er_own, er_halo, negative_slope);
+    a.alpha = alpha; a.dalpha = dalpha; a.out = dpre; a.d_el = d_el;
+    return launch_attn(p, true, a, (cudaStream_t)stream);
 }
 
 static int host_slots(pgcn_plan* p, int64_t need)

@@ -198,6 +198,126 @@ class PSpMMWeighted(torch.autograd.Function):
         return None, dvals, dH
 
 
+def _check_scores(plan, x, rows, what):
+    if not x.is_cuda:
+        raise RuntimeError("%s must be a CUDA tensor: the PGCN H100 path has no CPU fallback" % what)
+    if x.dtype != torch.float32:
+        raise TypeError("%s must be float32, got %s" % (what, x.dtype))
+    if x.dim() != 1 or x.shape[0] != rows:
+        raise ValueError("%s must be [%d], got %s" % (what, rows, tuple(x.shape)))
+    x = x.detach()
+    return (x.index_select(0, plan.owned_index()) if plan.layout == "global" else x).contiguous()
+
+
+def _to_layout(plan, x_own, rows):
+    if plan.layout != "global":
+        return x_own
+    out = torch.zeros((rows,) + tuple(x_own.shape[1:]), dtype=torch.float32, device=x_own.device)
+    out.index_copy_(0, plan.owned_index(), x_own)
+    return out
+
+
+class PGATAttention(torch.autograd.Function):
+    """Single-head sparse graph attention over the plan's stored pattern (GPU/PGAT.py:139-148 without the dense n x n
+    score matrix):
+
+        PGATAttention.apply(A, Z, el, er, negative_slope)
+        s_e = LeakyReLU(el[row(e)] + er[col(e)]),  alpha = softmax of s over each row's stored entries,  out = A(alpha) Z
+
+    Z is [rows, f], el and er are [rows] fp32 CUDA tensors (rows = m in the "local" layout, n in the "global" one, whose
+    non-owned rows are ignored and come back zero), out is [rows, f]. er of the halo columns comes from their owners
+    (pgcn_halo_rows, padded to rows of 4 floats so that the peer transport carries it). Forward: the edge softmax kernel
+    writes alpha, which becomes the resident values of A for pgcn_forward_keep_halo(Z). Backward: dZ = A(alpha)^T gOut
+    with the exchange; dalpha = SDDMM(gOut, [Z_own; Z_halo]); the softmax backward kernel gives dpre and d_el; and
+    d_er = A(dpre)^T 1, the column sums of dpre with the halo partials summed at their owners (pgcn_backward on an
+    m x 4 matrix of ones). Everything is deterministic. Gradients to W and a flow through torch, since el and er are
+    computed outside. The plan must be bound (PgcnPlan.bind_values); a later PSpMM on it restores the creation values."""
+
+    @staticmethod
+    def forward(ctx, A, Z, el, er, negative_slope=0.2):
+        rows = A.n if A.layout == "global" else A.m
+        Z_own = _check_feat(A, Z, rows, "Z")
+        if A.layout == "global":
+            Z_own = Z_own.index_select(0, A.owned_index())
+        el_own = _check_scores(A, el, rows, "el")
+        er_own = _check_scores(A, er, rows, "er")
+        lp = A.lp
+        f = Z_own.shape[1]
+        dev = Z_own.device
+        slope = float(negative_slope)
+        lib = cabi.load()
+        with torch.cuda.device(dev):
+            if not A._bound:
+                raise RuntimeError("PGATAttention sets the plan's edge values: call PgcnPlan.bind_values() once (set-up, "
+                                   "before any CUDA-graph capture)")
+            er_halo = torch.empty((lp.h,), dtype=torch.float32, device=dev)
+            if lp.k > 1:
+                er4 = torch.zeros((lp.m, 4), dtype=torch.float32, device=dev)
+                er4[:, 0] = er_own
+                er_halo4 = torch.empty((lp.h, 4), dtype=torch.float32, device=dev)
+                cabi.check(lib.pgcn_halo_rows(A.handle, er4.data_ptr(), er_halo4.data_ptr(), 4, _stream_ptr()),
+                           A.handle)
+                A.count_exchange(backward=False)
+                er_halo = er_halo4[:, 0].contiguous()
+            alpha = torch.empty((lp.nnz(),), dtype=torch.float32, device=dev)
+            cabi.check(lib.pgcn_edge_softmax(A.handle, el_own.data_ptr(), er_own.data_ptr(), er_halo.data_ptr(), slope,
+                                             alpha.data_ptr(), _stream_ptr()), A.handle)
+            out = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+            Z_halo = torch.empty((lp.h, f), dtype=torch.float32, device=dev)
+            A.use_values(alpha)
+            if lp.k > 1 and lp.h > 0:
+                cabi.check(lib.pgcn_forward_keep_halo(A.handle, Z_own.data_ptr(), out.data_ptr(), Z_halo.data_ptr(), f,
+                                                      _stream_ptr()), A.handle)
+            else:
+                cabi.check(lib.pgcn_forward(A.handle, Z_own.data_ptr(), out.data_ptr(), f, _stream_ptr()), A.handle)
+            if lp.k > 1:
+                A.count_exchange(backward=False)
+        ctx.plan, ctx.rows, ctx.slope = A, rows, slope
+        ctx.save_for_backward(alpha, Z_own, Z_halo, el_own, er_own, er_halo)
+        return _to_layout(A, out, rows)
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        A, rows, slope = ctx.plan, ctx.rows, ctx.slope
+        alpha, Z_own, Z_halo, el_own, er_own, er_halo = ctx.saved_tensors
+        g = _check_feat(A, grad_output, rows, "grad_output")
+        if A.layout == "global":
+            g = g.index_select(0, A.owned_index())
+        lp = A.lp
+        f = g.shape[1]
+        dev = g.device
+        lib = cabi.load()
+        dZ = d_el = d_er = None
+        with torch.cuda.device(dev):
+            if ctx.needs_input_grad[1]:
+                A.use_values(alpha)
+                G = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+                cabi.check(lib.pgcn_backward(A.handle, g.data_ptr(), G.data_ptr(), f, _stream_ptr()), A.handle)
+                if lp.k > 1:
+                    A.count_exchange(backward=True)
+                dZ = _to_layout(A, G, rows)
+            if ctx.needs_input_grad[2] or ctx.needs_input_grad[3]:
+                dalpha = torch.empty_like(alpha)
+                cabi.check(lib.pgcn_sddmm(A.handle, g.data_ptr(), Z_own.data_ptr(), Z_halo.data_ptr(),
+                                          dalpha.data_ptr(), f, _stream_ptr()), A.handle)
+                dpre = torch.empty_like(alpha)
+                gel = torch.empty((lp.m,), dtype=torch.float32, device=dev)
+                cabi.check(lib.pgcn_edge_softmax_backward(A.handle, el_own.data_ptr(), er_own.data_ptr(),
+                                                          er_halo.data_ptr(), alpha.data_ptr(), dalpha.data_ptr(),
+                                                          slope, dpre.data_ptr(), gel.data_ptr(), _stream_ptr()),
+                           A.handle)
+                d_el = _to_layout(A, gel, rows) if ctx.needs_input_grad[2] else None
+                if ctx.needs_input_grad[3]:
+                    A.use_values(dpre)
+                    ones = torch.ones((lp.m, 4), dtype=torch.float32, device=dev)
+                    D = torch.empty((lp.m, 4), dtype=torch.float32, device=dev)
+                    cabi.check(lib.pgcn_backward(A.handle, ones.data_ptr(), D.data_ptr(), 4, _stream_ptr()), A.handle)
+                    if lp.k > 1:
+                        A.count_exchange(backward=True)
+                    d_er = _to_layout(A, D[:, 0].contiguous(), rows)
+        return None, dZ, d_el, d_er, None
+
+
 # ---- the pieces, individually callable (NCCL transport), mirroring communicate_fgm ----------------
 
 def spmm_local(plan, H_own, H_halo=None, transpose=False):

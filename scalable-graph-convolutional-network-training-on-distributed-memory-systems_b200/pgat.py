@@ -1,0 +1,158 @@
+"""PGAT trainer CLI — the reference's graph-attention surface (GPU/PGAT.py:124-286) over the H100 operator.
+
+    python PGAT.py -a A.mtx -p A.mtx.8.hp -b nccl -s 8 -l 2 -f 16 [--seed 0] [--negative-slope 1.0]
+
+Kept from the reference: flags -a -p -b -s -l -f; rank/size from SLURM_PROCID / SLURM_NPROCS with torchrun's RANK /
+WORLD_SIZE as a fallback (as pgcn.py); inputs H[i, :] = i (:186-188) and labels i % f (:192); L x PGAT layers with the
+reference's parameters and initialisation (:124-135: Linear(f, f, bias=False) and a (2f x 1) attention vector, both
+xavier_normal with the relu gain) averaged over ranks at start (:166-170); Adam lr 1e-3 (:200); 50 epochs (:204);
+gradients all-reduced / world_size (:158-162); stdout `Epoch {:05d} | Loss {:.4f}` and `Elapsed time {:.4f}`.
+
+Different by design (SURVEY.md §8a, the quirks G1-G6 of DESIGN.md §1): the softmax runs over each row's stored entries
+only (the reference gives non-edges score 0 and keeps them in the softmax); halo rows really are exchanged in every
+layer; the score goes through LeakyReLU(negative_slope), whose default here, 1.0, is the reference's raw score; the
+flags are honoured (the reference overwrites them); every tensor is [m_local, f], each rank's loss is
+sum_owned nll / n and the printed loss is its all-reduced sum, the global mean. `-b gloo` is refused: the H100 path has no
+CPU fallback (the fp64 oracle lives under oracle/ and is test infrastructure).
+"""
+import getopt
+import os
+import sys
+import time
+
+import torch
+import torch.distributed as dist
+import torch.nn as nn
+import torch.nn.functional as F
+
+from . import graphio, plan as planmod
+from .op import PGATAttention
+from .pgcn import average_gradients, initialize_parameters, init_process
+
+
+class PGAT(nn.Module):
+    """GPU/PGAT.py:124-148 with the plan handle in place of the dense matrix and a sparse edge softmax."""
+
+    def __init__(self, A, in_features, out_features, negative_slope=0.2):
+        super().__init__()
+        self.in_features = in_features
+        self.out_features = out_features
+        self.A = A
+        self.negative_slope = negative_slope
+        self.linear = nn.Linear(in_features, out_features, bias=False)
+        self.attention = nn.Parameter(torch.empty(size=(2 * out_features, 1)))
+        self.reset_parameters()
+
+    def reset_parameters(self):
+        gain = nn.init.calculate_gain("relu")
+        nn.init.xavier_normal_(self.linear.weight, gain=gain)
+        nn.init.xavier_normal_(self.attention, gain=gain)
+
+    def forward(self, H):
+        Z = self.linear(H)
+        f = self.out_features
+        el = torch.matmul(Z, self.attention[:f, :]).squeeze(1)
+        er = torch.matmul(Z, self.attention[f:, :]).squeeze(1)
+        return PGATAttention.apply(self.A, Z, el, er, self.negative_slope)
+
+
+def run(rank, size, nlayers, nfeatures, path_A, path_partvec, backend, transport="auto", out=sys.stdout, seed=None,
+        negative_slope=1.0, epochs=50):
+    if backend != "nccl":
+        raise RuntimeError("backend '%s': the H100 PGAT path runs on CUDA devices over NCCL/NVLink only "
+                           "(no CPU fallback); use -b nccl" % backend)
+    device = torch.device("cuda", rank % torch.cuda.device_count())
+    torch.cuda.set_device(device)
+    A = graphio.read_adjacency(path_A)
+    partvec = graphio.read_partvec(path_partvec, A.shape[0])
+    graphio.check_partvec(partvec, size)
+    lp_host = planmod.build_local_plan(A, partvec, rank, size)
+    n = lp_host.n
+    plan = planmod.PgcnPlan(lp_host, nfeatures, device=device)
+    used = plan.init_comm(transport=transport)
+    plan.bind_values()
+    lp = plan.lp
+
+    own = torch.from_numpy(lp.owned).to(device)
+    H = own.to(torch.float32).unsqueeze(1).repeat(1, nfeatures).contiguous().requires_grad_(True)
+    labels = own % nfeatures
+
+    if seed is not None:
+        torch.manual_seed(seed)
+    model = nn.Sequential(*[PGAT(plan, nfeatures, nfeatures, negative_slope) for _ in range(nlayers)]).to(device)
+    if size > 1:
+        initialize_parameters(model, size)
+    optimizer = torch.optim.Adam(model.parameters(), lr=1e-3)
+
+    torch.cuda.synchronize()
+    start = time.time()
+    losses = []
+    for ep in range(epochs):
+        logits = model(H)
+        loss = F.nll_loss(F.log_softmax(logits, 1), labels, reduction="sum") / n
+        optimizer.zero_grad()
+        loss.backward()
+        if size > 1:
+            average_gradients(model, size)
+        optimizer.step()
+        total = loss.detach().clone()
+        if size > 1:
+            dist.all_reduce(total, op=dist.ReduceOp.SUM)
+        losses.append(float(total))
+        if rank == 0:
+            print("Epoch {:05d} | Loss {:.4f}".format(ep, losses[-1]), file=out, flush=True)
+    torch.cuda.synchronize()
+    elapsed = torch.tensor([time.time() - start], device=device)
+    if size > 1:
+        dist.all_reduce(elapsed, op=dist.ReduceOp.MAX)
+    if rank == 0:
+        print("Elapsed time {:.4f}".format(elapsed.item()), file=out, flush=True)
+    result = {"losses": losses, "elapsed": float(elapsed.item()), "transport": used, "stats": dict(plan.stats)}
+    plan.close()
+    return result
+
+
+def main(argv):
+    size = int(os.environ.get("SLURM_NPROCS", os.environ.get("WORLD_SIZE", "1")))
+    rank = int(os.environ.get("SLURM_PROCID", os.environ.get("RANK", "0")))
+    os.environ["RANK"] = str(rank)
+    try:
+        opts, _ = getopt.getopt(argv, "a:p:b:s:l:f:", ["transport=", "seed=", "negative-slope="])
+    except getopt.GetoptError:
+        print("a:p:b:", flush=True)                                       # the reference's usage text
+        sys.exit(2)
+    path_A = path_partvec = None
+    backend = "nccl"
+    nlayers = nfeatures = None
+    kw = {}
+    for opt, arg in opts:
+        if opt == "-a":
+            path_A = arg
+        elif opt == "-p":
+            path_partvec = arg
+        elif opt == "-b":
+            backend = arg
+        elif opt == "-s":
+            size = int(arg)
+        elif opt == "-l":
+            nlayers = int(arg)
+        elif opt == "-f":
+            nfeatures = int(arg)
+        elif opt == "--transport":
+            kw["transport"] = arg
+        elif opt == "--seed":
+            kw["seed"] = int(arg)
+        elif opt == "--negative-slope":
+            kw["negative_slope"] = float(arg)
+    if path_A is None or path_partvec is None or nlayers is None or nfeatures is None:
+        print("usage: PGAT.py -a <A.mtx> -p <partvec> -b nccl -s <nparts> -l <nlayers> -f <nfeatures> "
+              "[--seed N] [--negative-slope S]", flush=True)
+        sys.exit(2)
+    os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
+    os.environ.setdefault("MASTER_PORT", "29500")
+    os.environ["WORLD_SIZE"] = str(size)
+    init_process(rank, size, run, nlayers, nfeatures, path_A, path_partvec, backend, **kw)
+
+
+if __name__ == "__main__":
+    main(sys.argv[1:])
