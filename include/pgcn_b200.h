@@ -99,7 +99,9 @@ int pgcn_plan_destroy(pgcn_plan* plan);
  *   "kernel"               0 = automatic (default): widths that are multiples of 128 floats with 16-byte aligned
  *                          operands take the shared-memory ring kernel fed by 2-D tensor-map TMA, everything else the
  *                          register-pipeline kernel; 4 = always the register kernel; 5 / 6 / 7 = ring kernel fed by
- *                          1-D cp.async.bulk / cp.async / 2-D tensor-map TMA (one row per copy)
+ *                          1-D cp.async.bulk / cp.async / 2-D tensor-map TMA (one row per copy). Under every setting
+ *                          an operand that is not 16-byte aligned takes the register kernel with scalar accesses:
+ *                          slower, same bits as the register kernel on aligned copies
  *   "ring_slots"           row slots per warp of the ring kernel: 16 (default), 32, 64; "ring_groups" 2 | 4 (64 slots)
  *   "ring_tile_floats"     floats of H one ring slot holds: 0 = tuned by pgcn_plan_autotune, else the full width
  *                          (256 when f % 256 == 0, else 128) (default); 64 = 256-byte slices, gathered one slice of
@@ -113,7 +115,7 @@ int pgcn_plan_destroy(pgcn_plan* plan);
  *   "edges_per_block", "long_row", "tile_floats"   the same for the register kernel (defaults 128, 4 * block, 0)
  *   "overlap"              1 = split A_local into own / per-peer halo blocks and pipeline the exchange with them
  *                          (Parallel-GCN/main.c:271 then :275-299)                         (default 1)
- *   "relu"                 1 = pgcn_forward writes max(0, A_local * H)                      (default 0)
+ *   "relu"                 1 = pgcn_forward writes relu(A_local * H); NaN stays NaN, as in torch.relu (default 0)
  *   "p2p"                  0 = never use the peer-memory transport (all ranks must agree)  (default 1)
  * pgcn_plan_autotune overrides block sizes / ring depth / ring tile width per matrix; setting a block size or the
  * ring depth explicitly clears the tuned values, a non-zero "ring_tile_floats" overrides the tuned width. "hot_mb" (L2-resident hot set of H rows) is fixed at plan creation: environment variable PGCN_HOT_MB.
@@ -199,6 +201,8 @@ int pgcn_p2p_import(pgcn_plan* plan, const void* handles_k);
  *   transpose = 2 : own-columns half of the overlapped forward, Z  = A_own  * H_own
  *   transpose = 3 : halo-columns half,                          Z += A_halo * H_halo
  *                   (Parallel-GCN/main.c:271 then :295; plans with k > 1 and h > 0 only)
+ * Operands need 4-byte alignment only. When one of them is not 16-byte aligned (or f % 4 != 0) the call takes the
+ * register kernel with scalar accesses, which is slower; the same holds for every entry point below.
  */
 int pgcn_spmm(pgcn_plan* plan, int transpose,
               const float* H_own, const float* H_halo,

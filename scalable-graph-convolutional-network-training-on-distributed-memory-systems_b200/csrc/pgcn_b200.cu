@@ -408,10 +408,12 @@ struct TileCfg { int lpe, vpl, vw, tiles; };
 
 int pow2ceil(int x) { int p = 1; while (p < x) p <<= 1; return p; }
 
-TileCfg choose_tile(const pgcn_plan* p, int f)
+// vw: floats per vector access, 4 or 1 (vec_width). Each output element sums the same products in the same order
+// at either width, so the width changes the launch shape but not a bit of the result.
+TileCfg choose_tile(const pgcn_plan* p, int f, int vw)
 {
     TileCfg t;
-    t.vw = (f % 4 == 0) ? 4 : 1;
+    t.vw = vw;
     const int nvec = f / t.vw;
     int tile_vecs = nvec;
     if (p->opt_tile > 0) tile_vecs = std::max<int>(1, (int)std::min<int64_t>(nvec, p->opt_tile / t.vw));
@@ -546,7 +548,7 @@ void preload_kernels()
     touch_kernel(spmm_fixup_kernel<4>); touch_kernel(spmm_fixup_kernel<1>);
     touch_kernel(pack_rows_kernel<4>); touch_kernel(pack_rows_kernel<1>);
     touch_kernel(unpack_add_kernel<4>); touch_kernel(unpack_add_kernel<1>);
-    touch_kernel(put_rows_kernel<4>); touch_kernel(p2p_wait_kernel); touch_kernel(epoch_advance_kernel);
+    touch_kernel(put_rows_kernel<4>); touch_kernel(put_rows_kernel<1>); touch_kernel(p2p_wait_kernel); touch_kernel(epoch_advance_kernel);
     touch_kernel(set_values_kernel); touch_kernel(copy_halo_kernel); touch_kernel(sddmm_plain_kernel);
     touch_kernel(sddmm_ring_kernel<1>); touch_kernel(sddmm_ring_kernel<2>);
     touch_kernel(sddmm_ring_kernel<3>); touch_kernel(sddmm_ring_kernel<4>);
@@ -554,6 +556,17 @@ void preload_kernels()
 }
 
 bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
+
+// Vector width of the element-wise kernels (register SpMM, zero-rows, fixup, pack, unpack, put): 16-byte accesses need
+// whole 4-float vectors AND every operand the launch accesses by vector 16-byte aligned (null operands do not count).
+// Any other operand takes the scalar instances, which are slower but compute the same bits.
+int vec_width(int f, std::initializer_list<const void*> ops)
+{
+    if (f % 4 != 0) return 1;
+    for (const void* q : ops)
+        if (!aligned16(q)) return 1;
+    return 4;
+}
 
 // Which SpMM kernel serves width f with these operands: the shared-memory ring (TMA bulk copies) needs whole
 // 128-float vectors and 16-byte aligned rows; everything else takes the register pipeline.
@@ -623,7 +636,7 @@ int launch_spmm(pgcn_plan* p, DevCsr& c, const float* H0, const float* H1, int s
     if (!sched_ready(c, ring ? 1 : 0, epb, long_row) && (rc = refuse_under_capture(p, st))) return rc;
     if ((rc = build_schedule(p, c, ring ? 1 : 0, epb, long_row))) return rc;
     const DevCsr::Sched& sc = c.sched[ring ? 1 : 0];
-    const TileCfg t = choose_tile(p, f);
+    const TileCfg t = choose_tile(p, f, vec_width(f, {H0, H1, H_odd, Z0, Z1}));
     if (c.nempty > 0 && !beta) {
         ZeroArgs za;
         za.rows = c.d_empty; za.nrows_empty = c.nempty; za.Z0 = Z0; za.Z1 = Z1; za.zsplit = zsplit; za.f = f;
@@ -733,7 +746,7 @@ int launch_pack(pgcn_plan* p, const float* H, float* slab, int f, cudaStream_t s
     if (p->S == 0) return 0;
     PackArgs a;
     a.send_idx = p->d_send_idx; a.S = p->S; a.H = H; a.slab = slab; a.f = f;
-    const int vw = (f % 4 == 0) ? 4 : 1;
+    const int vw = vec_width(f, {H, slab});
     const unsigned grid = grid_for(p->S * (f / vw), p->num_sms);
     if (vw == 4) pack_rows_kernel<4><<<grid, 256, 0, st>>>(a);
     else pack_rows_kernel<1><<<grid, 256, 0, st>>>(a);
@@ -750,7 +763,7 @@ int launch_unpack(pgcn_plan* p, const float* recv, float* G, int f, cudaStream_t
     a.brow = p->d_brow; a.bptr = p->d_bptr; a.bpos = p->d_bpos; a.nb = p->nb;
     a.recv = recv; a.G = G; a.f = f;
     a.recv_odd = recv_odd; a.epoch = recv_odd ? p->d_epoch : nullptr;
-    const int vw = (f % 4 == 0) ? 4 : 1;
+    const int vw = vec_width(f, {recv, recv_odd, G});
     const long long total = (long long)p->nb * (f / vw);
     const unsigned grid = (unsigned)((total + 255) / 256);
     if (vw == 4) unpack_add_kernel<4><<<grid, 256, 0, st>>>(a);
@@ -924,10 +937,13 @@ int p2p_put(pgcn_plan* p, int dst, const float* src, int f, bool reverse, cudaSt
     a.done = p->d_done + (reverse ? 32 : 0) + dst;     // kMaxPeers <= 16 destinations per direction
     a.flag = flag_slot(p->peer_arena[dst], pb.off_flags, p->rank);
     a.epoch = p->d_epoch;
+    // the peer slabs are 16-byte aligned (f % 4 == 0 on this transport); the caller's rows may not be
+    const int vw = vec_width(f, {src});
     // enough CTAs to keep the NVLink store queues full, few enough not to crowd out the SpMM running beside it
-    const long long items = a.nrows * (f / 4);
+    const long long items = a.nrows * (f / vw);
     const unsigned grid = (unsigned)std::max<long long>(1, std::min<long long>((items + 255) / 256, 4LL * p->num_sms));
-    put_rows_kernel<4><<<grid, 256, 0, st>>>(a);
+    if (vw == 4) put_rows_kernel<4><<<grid, 256, 0, st>>>(a);
+    else put_rows_kernel<1><<<grid, 256, 0, st>>>(a);
     ++p->launches;
     CU(p, cudaGetLastError());
     return 0;

@@ -22,7 +22,8 @@
 //   * rows longer than `long_row` are split into segments that write partial sums to a side
 //     buffer; a second tiny kernel adds the segments in a fixed order (deterministic, no atomics);
 //   * blockIdx.y walks feature tiles, so a wide H can be processed one L2-resident column slice
-//     at a time (tile_floats option) and any f is supported (scalar path when f % 4 != 0).
+//     at a time (tile_floats option) and any f is supported (scalar path when f % 4 != 0 or an operand is not
+//     16-byte aligned: .v4 accesses need natural alignment).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -83,8 +84,16 @@ __global__ void epoch_advance_kernel(unsigned long long* epoch) { ++*epoch; }
 
 __device__ __forceinline__ bool epoch_odd(const unsigned long long* epoch) { return epoch != nullptr && (*epoch & 1ull); }
 
-__device__ __forceinline__ float4 vrelu(const float4& a) { return make_float4(fmaxf(a.x, 0.f), fmaxf(a.y, 0.f), fmaxf(a.z, 0.f), fmaxf(a.w, 0.f)); }
-__device__ __forceinline__ float vrelu(const float& a) { return fmaxf(a, 0.f); }
+// relu that keeps NaN, as torch.relu does (fmaxf(NaN, 0) would return 0 and hide a diverging run). max.NaN (sm_80+) is
+// the same single min/max instruction as fmaxf, so the kernels keep their registers; finite results are fmaxf's.
+__device__ __forceinline__ float relu1(float x)
+{
+    float r;
+    asm("max.NaN.f32 %0, %1, 0f00000000;" : "=f"(r) : "f"(x));
+    return r;
+}
+__device__ __forceinline__ float4 vrelu(const float4& a) { return make_float4(relu1(a.x), relu1(a.y), relu1(a.z), relu1(a.w)); }
+__device__ __forceinline__ float vrelu(const float& a) { return relu1(a); }
 
 template <int VW> struct Vec;
 template <> struct Vec<4> { typedef float4 type; };
@@ -98,7 +107,7 @@ __device__ __forceinline__ void vfma(float4& a, float w, const float4& r) {
 __device__ __forceinline__ void vfma(float& a, float w, const float& r) { a = fmaf(w, r, a); }
 __device__ __forceinline__ void vfma(float2& a, float w, const float2& r) { a.x = fmaf(w, r.x, a.x); a.y = fmaf(w, r.y, a.y); }
 __device__ __forceinline__ void vadd(float2& a, const float2& r) { a.x += r.x; a.y += r.y; }
-__device__ __forceinline__ float2 vrelu(const float2& a) { return make_float2(fmaxf(a.x, 0.f), fmaxf(a.y, 0.f)); }
+__device__ __forceinline__ float2 vrelu(const float2& a) { return make_float2(relu1(a.x), relu1(a.y)); }
 __device__ __forceinline__ float2 vzero(float2*) { return make_float2(0.f, 0.f); }
 __device__ __forceinline__ void vadd(float4& a, const float4& r) { a.x += r.x; a.y += r.y; a.z += r.z; a.w += r.w; }
 __device__ __forceinline__ void vadd(float& a, const float& r) { a += r; }
