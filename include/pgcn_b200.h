@@ -304,6 +304,39 @@ int pgcn_edge_softmax_backward(pgcn_plan* plan, const float* el, const float* er
                                void* stream);
 int pgcn_halo_rows(pgcn_plan* plan, const float* X_own, float* X_halo_out, int32_t w, void* stream);
 
+/* ---- multi-head sparse graph attention: K = heads in {1, 2, 4, 8} heads of width d = f / K ------------------------ */
+/*
+ * Every array is row-major and head-minor: el, er_own and d_el are m x K, er_halo is h x K, alpha, dalpha and dpre are
+ * nnz x K in forward CSR order (the order of pgcn_plan_set_values). Head h of the output is
+ *   Z[:, h d:(h+1) d] = A(alpha[:, h]) [H_own ; H_halo][:, h d:(h+1) d]
+ * and the heads are concatenated. None of these calls reads or writes the plan's resident values (pgcn_plan_set_values
+ * is never needed): the aggregation takes its weights from alpha.
+ * pgcn_edge_softmax_heads / pgcn_edge_softmax_backward_heads: pgcn_edge_softmax / _backward for every head at once (one
+ *   gather of a column brings its K er values). heads == 1 launches the single-head kernels: the same bits.
+ * pgcn_forward_heads: the exchange of pgcn_forward without its per-source overlap (both transports), then one launch of
+ *   the register SpMM with the heads' weights over [H_own | halo rows]; with H_halo_out (h x f, may be NULL) the halo
+ *   rows received are copied out as in pgcn_forward_keep_halo. The device epoch advances as in every fused call.
+ * pgcn_backward_heads: G_own = A(alpha)^T gZ with the halo partials summed at their owners (pgcn_backward without its
+ *   per-peer pipelining). With alpha[:, h] equal to the plan's creation values for every head, both calls give the bits of
+ *   pgcn_forward / pgcn_backward with the plan option kernel = 4 (the same schedule and summation order).
+ * pgcn_sddmm_heads: dalpha[e, h] = < gZ[row(e), h d:(h+1) d], [H_own ; H_halo][col(e), h d:(h+1) d] >. f = 128, 256 or
+ *   512 with d % 4 == 0 and 16-byte aligned operands takes a ring kernel, every other case a plain kernel; heads == 1 is
+ *   pgcn_sddmm.
+ * All five need pgcn_plan_bind_values (PGCN_ERR_STATE before). heads outside {1, 2, 4, 8}, f % heads != 0 and null
+ * arguments return PGCN_ERR_INVALID. After pgcn_plan_prepare(plan, f) they are capturable.
+ */
+int pgcn_edge_softmax_heads(pgcn_plan* plan, int32_t heads, const float* el, const float* er_own, const float* er_halo,
+                            float negative_slope, float* alpha, void* stream);
+int pgcn_edge_softmax_backward_heads(pgcn_plan* plan, int32_t heads, const float* el, const float* er_own,
+                                     const float* er_halo, const float* alpha, const float* dalpha, float negative_slope,
+                                     float* dpre, float* d_el, void* stream);
+int pgcn_forward_heads(pgcn_plan* plan, int32_t heads, const float* alpha, const float* H_own, float* Z,
+                       float* H_halo_out, int32_t f, void* stream);
+int pgcn_backward_heads(pgcn_plan* plan, int32_t heads, const float* alpha, const float* gZ, float* G_own, int32_t f,
+                        void* stream);
+int pgcn_sddmm_heads(pgcn_plan* plan, int32_t heads, const float* gZ, const float* H_own, const float* H_halo,
+                     float* dalpha, int32_t f, void* stream);
+
 /* ---- host-buffer variant: what a non-torch host (the reference's C path) would bind -------- */
 /*
  * Same as pgcn_forward but H and Z are HOST pointers (pinned or pageable): copies H to the

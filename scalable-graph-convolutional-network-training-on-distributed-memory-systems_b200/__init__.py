@@ -19,7 +19,8 @@ def __getattr__(name):
     if name in ("op", "pgcn", "pgat", "minibatch"):
         import importlib
         return importlib.import_module("." + name, __name__)
-    if name in ("PSpMM", "PSpMMWeighted", "PGATAttention", "aggregate_forward", "aggregate_backward"):
+    if name in ("PSpMM", "PSpMMWeighted", "PGATAttention", "PGATMultiHeadAttention", "aggregate_forward",
+                "aggregate_backward"):
         from . import op
         return getattr(op, name)
     raise AttributeError(name)

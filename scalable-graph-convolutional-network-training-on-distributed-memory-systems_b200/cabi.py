@@ -22,6 +22,8 @@ SYMBOLS = [
     "pgcn_forward", "pgcn_backward", "pgcn_forward_host", "pgcn_forward_host_async", "pgcn_forward_host_wait",
     "pgcn_plan_bind_values", "pgcn_plan_set_values", "pgcn_sddmm", "pgcn_forward_keep_halo",
     "pgcn_edge_softmax", "pgcn_edge_softmax_backward", "pgcn_halo_rows",
+    "pgcn_edge_softmax_heads", "pgcn_edge_softmax_backward_heads", "pgcn_forward_heads", "pgcn_backward_heads",
+    "pgcn_sddmm_heads",
 ]
 
 
@@ -125,6 +127,16 @@ def load(build_if_missing=True):
     lib.pgcn_edge_softmax_backward.argtypes = [vp, vp, vp, vp, vp, vp, C.c_float, vp, vp, vp]
     lib.pgcn_halo_rows.restype = C.c_int
     lib.pgcn_halo_rows.argtypes = [vp, vp, vp, i32, vp]
+    lib.pgcn_edge_softmax_heads.restype = C.c_int
+    lib.pgcn_edge_softmax_heads.argtypes = [vp, i32, vp, vp, vp, C.c_float, vp, vp]
+    lib.pgcn_edge_softmax_backward_heads.restype = C.c_int
+    lib.pgcn_edge_softmax_backward_heads.argtypes = [vp, i32, vp, vp, vp, vp, vp, C.c_float, vp, vp, vp]
+    lib.pgcn_forward_heads.restype = C.c_int
+    lib.pgcn_forward_heads.argtypes = [vp, i32, vp, vp, vp, vp, i32, vp]
+    lib.pgcn_backward_heads.restype = C.c_int
+    lib.pgcn_backward_heads.argtypes = [vp, i32, vp, vp, vp, i32, vp]
+    lib.pgcn_sddmm_heads.restype = C.c_int
+    lib.pgcn_sddmm_heads.argtypes = [vp, i32, vp, vp, vp, vp, i32, vp]
     _lib = lib
     return lib
 

@@ -193,6 +193,8 @@ struct pgcn_plan {
     long long vtotal = 0;                  // entries over all sets
     bool sddmm_attr_set[5] = {false};      // per f / 128 of the SDDMM ring kernel
     int sddmm_ctas_per_sm[5] = {0};
+    bool sddmm_heads_attr_set[5][9] = {};  // per f / 128 and head count of the multi-head SDDMM ring kernel
+    int sddmm_heads_ctas_per_sm[5][9] = {};
     int* d_rowptr = nullptr;               // m + 1, the forward rowptr (edge softmax)
     int* d_long_rows = nullptr;            // rows of more than kAttnLongRow entries (one CTA each in the edge softmax)
     int nlong_rows = 0;
@@ -448,6 +450,51 @@ spmm_fn pick_lpe(int lpe, int vpl, bool halo)
     }
 }
 
+// Multi-head instances of the register kernel (spmm_heads_kernel): one vector per lane (the feature row is walked in
+// blockIdx.y tiles of LPE vectors), NH heads staged per chunk.
+typedef void (*spmm_heads_fn)(const SpmmArgs, const SpmmHeadArgs);
+
+template <int LPE, int VW, bool HALO>
+spmm_heads_fn pick_heads_nh(int nh)
+{
+    switch (nh) {
+        case 1: return spmm_heads_kernel<LPE, VW, HALO, 1>;
+        case 2: return spmm_heads_kernel<LPE, VW, HALO, 2>;
+        case 4: return spmm_heads_kernel<LPE, VW, HALO, 4>;
+        default: return spmm_heads_kernel<LPE, VW, HALO, 8>;
+    }
+}
+
+template <int VW, bool HALO>
+spmm_heads_fn pick_heads_lpe(int lpe, int nh)
+{
+    switch (lpe) {
+        case 4: return pick_heads_nh<4, VW, HALO>(nh);
+        case 8: return pick_heads_nh<8, VW, HALO>(nh);
+        case 16: return pick_heads_nh<16, VW, HALO>(nh);
+        default: return pick_heads_nh<32, VW, HALO>(nh);
+    }
+}
+
+spmm_heads_fn pick_heads(int lpe, int vw, bool halo, int nh)
+{
+    if (vw == 4) return halo ? pick_heads_lpe<4, true>(lpe, nh) : pick_heads_lpe<4, false>(lpe, nh);
+    return halo ? pick_heads_lpe<1, true>(lpe, nh) : pick_heads_lpe<1, false>(lpe, nh);
+}
+
+// Launch shape of the multi-head instances: one vector per lane, as many lanes as the row needs (4 .. 32), the rest
+// of the row in blockIdx.y tiles.
+TileCfg choose_tile_heads(int f, int vw)
+{
+    TileCfg t;
+    t.vw = vw;
+    const int nvec = f / vw;
+    t.lpe = std::max(4, std::min(32, pow2ceil(nvec)));
+    t.vpl = 1;
+    t.tiles = (nvec + t.lpe - 1) / t.lpe;
+    return t;
+}
+
 typedef void (*ring_fn)(const SpmmArgs, const RingArgs);
 typedef void (*ring_tm_fn)(const SpmmArgs, const RingArgs, const CUtensorMap, const CUtensorMap, const CUtensorMap);
 
@@ -523,6 +570,44 @@ ring_tm_fn pick_ring_tm(int tf, int shape, bool halo)
     return halo ? pick_ring_tm_t<128, true>(shape) : pick_ring_tm_t<128, false>(shape);
 }
 
+typedef void (*attn_fn)(const AttnArgs);
+
+// the edge softmax instance of K heads (VEC: vector loads of the K values of an entry or row)
+template <int K>
+attn_fn pick_softmax_k(bool vec, bool backward)
+{
+    if (vec) return backward ? edge_softmax_backward_kernel<K, true> : edge_softmax_kernel<K, true>;
+    return backward ? edge_softmax_backward_kernel<K, false> : edge_softmax_kernel<K, false>;
+}
+attn_fn pick_softmax(int k, bool vec, bool backward)
+{
+    switch (k) {
+        case 1: return backward ? edge_softmax_backward_kernel<1, false> : edge_softmax_kernel<1, false>;
+        case 2: return pick_softmax_k<2>(vec, backward);
+        case 4: return pick_softmax_k<4>(vec, backward);
+        default: return pick_softmax_k<8>(vec, backward);
+    }
+}
+
+typedef void (*sddmm_fn)(const SddmmArgs);
+
+template <int NV>
+sddmm_fn pick_sddmm_heads_nv(int k)
+{
+    switch (k) {
+        case 2: return sddmm_heads_ring_kernel<NV, 2>;
+        case 4: return sddmm_heads_ring_kernel<NV, 4>;
+        default: return sddmm_heads_ring_kernel<NV, 8>;
+    }
+}
+// the multi-head SDDMM ring instance of f = 128 nv (nv = 1, 2, 4) and k = 2, 4, 8 heads
+sddmm_fn pick_sddmm_heads(int nv, int k)
+{
+    if (nv == 1) return pick_sddmm_heads_nv<1>(k);
+    if (nv == 2) return pick_sddmm_heads_nv<2>(k);
+    return pick_sddmm_heads_nv<4>(k);
+}
+
 // CUDA loads kernels lazily, at their first launch, and that load synchronises with the device. A rank whose
 // stream already holds a spinning p2p_wait_kernel must therefore never launch a not-yet-loaded kernel behind it
 // when the ranks it waits for live in the SAME process (single-process multi-rank use: tests, smoke) — their put
@@ -552,7 +637,15 @@ void preload_kernels()
     touch_kernel(set_values_kernel); touch_kernel(copy_halo_kernel); touch_kernel(sddmm_plain_kernel);
     touch_kernel(sddmm_ring_kernel<1>); touch_kernel(sddmm_ring_kernel<2>);
     touch_kernel(sddmm_ring_kernel<3>); touch_kernel(sddmm_ring_kernel<4>);
-    touch_kernel(edge_softmax_kernel); touch_kernel(edge_softmax_backward_kernel);
+    touch_kernel(edge_softmax_kernel<1, false>); touch_kernel(edge_softmax_backward_kernel<1, false>);
+    for (int halo = 0; halo < 2; ++halo)
+        for (int lpe = 4; lpe <= 32; lpe *= 2)
+            for (int nh = 1; nh <= 8; nh *= 2) { touch_kernel(pick_heads(lpe, 4, halo != 0, nh)); touch_kernel(pick_heads(lpe, 1, halo != 0, nh)); }
+    for (int nh = 2; nh <= 8; nh *= 2)
+        for (int vec = 0; vec < 2; ++vec) { touch_kernel(pick_softmax(nh, vec != 0, false)); touch_kernel(pick_softmax(nh, vec != 0, true)); }
+    for (int nv = 1; nv <= 4; nv *= 2)
+        for (int nh = 2; nh <= 8; nh *= 2) touch_kernel(pick_sddmm_heads(nv, nh));
+    touch_kernel(sddmm_plain_heads_kernel);
 }
 
 bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
@@ -622,21 +715,33 @@ int ring_attr(pgcn_plan* p, int tf, int shape, int mode, bool halo, cudaStream_t
     return 0;
 }
 
+// Weights of a multi-head aggregation: nh heads of width f / nh; alpha is nnz x nh in forward CSR order, map (null for
+// the forward records) takes an entry of the launched matrix to its forward entry.
+struct HeadArgs {
+    const float* alpha;
+    const int* map;
+    int nh;
+};
+
 // H_odd: the halo slab of odd exchange epochs when the operand that holds the halo slab (H1, or H0 without H1) is the
 // peer transport's double-buffered slab; the kernels then pick the buffer from the plan's device epoch.
+// heads: multi-head weights instead of the records' values; the launch then takes the register kernel (schedule 0) and
+// its multi-head instance. Null: nothing changes.
 int launch_spmm(pgcn_plan* p, DevCsr& c, const float* H0, const float* H1, int split,
                 float* Z0, float* Z1, int zsplit, int f, int beta, cudaStream_t st, int relu = 0, bool use_final = false,
-                const float* H_odd = nullptr)
+                const float* H_odd = nullptr, const HeadArgs* heads = nullptr)
 {
     if (c.nrows == 0) return 0;
-    const bool ring = use_ring(p, H0, H1, f) && aligned16(Z0) && aligned16(Z1) && (!H_odd || aligned16(H_odd));
+    const bool ring = !heads && use_ring(p, H0, H1, f) && aligned16(Z0) && aligned16(Z1) && (!H_odd || aligned16(H_odd));
     int64_t epb, long_row;
     sched_params(p, c, ring, &epb, &long_row);
     int rc;
     if (!sched_ready(c, ring ? 1 : 0, epb, long_row) && (rc = refuse_under_capture(p, st))) return rc;
     if ((rc = build_schedule(p, c, ring ? 1 : 0, epb, long_row))) return rc;
     const DevCsr::Sched& sc = c.sched[ring ? 1 : 0];
-    const TileCfg t = choose_tile(p, f, vec_width(f, {H0, H1, H_odd, Z0, Z1}));
+    // multi-head: 4-float vectors also need whole vectors per head
+    const int vw = (heads && (f / heads->nh) % 4 != 0) ? 1 : vec_width(f, {H0, H1, H_odd, Z0, Z1});
+    const TileCfg t = heads ? choose_tile_heads(f, vw) : choose_tile(p, f, vw);
     if (c.nempty > 0 && !beta) {
         ZeroArgs za;
         za.rows = c.d_empty; za.nrows_empty = c.nempty; za.Z0 = Z0; za.Z1 = Z1; za.zsplit = zsplit; za.f = f;
@@ -709,8 +814,14 @@ int launch_spmm(pgcn_plan* p, DevCsr& c, const float* H0, const float* H1, int s
         const int groups_per_cta = kSpmmThreads / t.lpe;
         dim3 grid((unsigned)((sc.nblocks + groups_per_cta - 1) / groups_per_cta), (unsigned)t.tiles);
         const bool halo = (H1 != nullptr);
-        spmm_fn fn = (t.vw == 4) ? pick_lpe<4>(t.lpe, t.vpl, halo) : pick_lpe<1>(t.lpe, t.vpl, halo);
-        fn<<<grid, kSpmmThreads, 0, st>>>(a);
+        if (heads) {
+            SpmmHeadArgs ha;
+            ha.alpha = heads->alpha; ha.amap = heads->map; ha.hd = f / heads->nh;
+            pick_heads(t.lpe, t.vw, halo, heads->nh)<<<grid, kSpmmThreads, 0, st>>>(a, ha);
+        } else {
+            spmm_fn fn = (t.vw == 4) ? pick_lpe<4>(t.lpe, t.vpl, halo) : pick_lpe<1>(t.lpe, t.vpl, halo);
+            fn<<<grid, kSpmmThreads, 0, st>>>(a);
+        }
         ++p->launches;
     }
     if (sc.nlong > 0) {
@@ -775,8 +886,6 @@ int launch_unpack(pgcn_plan* p, const float* recv, float* G, int f, cudaStream_t
 
 // ---- edge values -----------------------------------------------------------------------------
 
-typedef void (*sddmm_fn)(const SddmmArgs);
-
 sddmm_fn pick_sddmm(int nv)
 {
     switch (nv) {
@@ -839,6 +948,67 @@ int launch_sddmm(pgcn_plan* p, const float* gZ, const float* H0, const float* H1
         pick_sddmm(f / 128)<<<grid, kSddmmWarps * 32, sddmm_smem_bytes(f / 128), st>>>(a);
     } else {
         sddmm_plain_kernel<<<(unsigned)((sc.nblocks + 7) / 8), 256, 0, st>>>(a);
+    }
+    ++p->launches;
+    CU(p, cudaGetLastError());
+    return 0;
+}
+
+// The multi-head SDDMM ring instance serves f = 128, 256 or 512 with 2, 4 or 8 heads of at least 4 floats and 16-byte
+// aligned operands (the single-head ring's rule); k == 1 is pgcn_sddmm itself.
+bool sddmm_heads_use_ring(const pgcn_plan* p, const float* gZ, const float* H0, const float* H1, int f, int k)
+{
+    return k > 1 && (f == 128 || f == 256 || f == 512) && (f / k) % 4 == 0 && sddmm_use_ring(p, gZ, H0, H1, f);
+}
+
+int sddmm_heads_attr(pgcn_plan* p, int f, int k, cudaStream_t st)
+{
+    const int nv = f / 128;
+    if (p->sddmm_heads_attr_set[nv][k]) return 0;
+    int rc = refuse_under_capture(p, st);
+    if (rc) return rc;
+    const void* fptr = (const void*)pick_sddmm_heads(nv, k);
+    const size_t smem = sddmm_smem_bytes(nv);
+    CU(p, cudaFuncSetAttribute(fptr, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int nb = 0;
+    CU(p, cudaOccupancyMaxActiveBlocksPerMultiprocessorWithFlags(&nb, fptr, kSddmmWarps * 32, smem, 0));
+    p->sddmm_heads_ctas_per_sm[nv][k] = std::max(nb, 1);
+    p->sddmm_heads_attr_set[nv][k] = true;
+    return 0;
+}
+
+// dalpha (nnz x k) = the SDDMM per head over the forward matrix; k == 1 is launch_sddmm
+int launch_sddmm_heads(pgcn_plan* p, int k, const float* gZ, const float* H0, const float* H1, float* dalpha, int f,
+                       cudaStream_t st)
+{
+    if (k == 1) return launch_sddmm(p, gZ, H0, H1, dalpha, f, st);
+    DevCsr& c = p->fwd;
+    if (c.nnz == 0 || c.nrows == 0) return 0;
+    const bool ring = sddmm_heads_use_ring(p, gZ, H0, H1, f, k);
+    int64_t epb, long_row;
+    sched_params(p, c, ring, &epb, &long_row);
+    int rc;
+    if (!sched_ready(c, ring ? 1 : 0, epb, long_row) && (rc = refuse_under_capture(p, st))) return rc;
+    if ((rc = build_schedule(p, c, ring ? 1 : 0, epb, long_row))) return rc;
+    const DevCsr::Sched& sc = c.sched[ring ? 1 : 0];
+    SddmmArgs a;
+    a.blocks = sc.d_blocks; a.nblocks = sc.nblocks;
+    a.pieces = c.d_cw;
+    a.gZ = gZ; a.H0 = H0; a.H1 = H1; a.split = p->m;
+    a.rowids = c.d_rowids;
+    a.dvals = dalpha; a.f = f;
+    a.counter = nullptr;
+    if (sc.nblocks == 0) return 0;
+    if (ring) {
+        const int nv = f / 128;
+        if ((rc = sddmm_heads_attr(p, f, k, st))) return rc;
+        CU(p, cudaMemsetAsync(p->d_counter, 0, sizeof(unsigned int), st));
+        a.counter = p->d_counter;
+        const unsigned ctas = (unsigned)((sc.nblocks + kSddmmWarps - 1) / kSddmmWarps);
+        const unsigned grid = std::min<unsigned>(ctas, (unsigned)(p->num_sms * p->sddmm_heads_ctas_per_sm[nv][k]));
+        pick_sddmm_heads(nv, k)<<<grid, kSddmmWarps * 32, sddmm_smem_bytes(nv), st>>>(a);
+    } else {
+        sddmm_plain_heads_kernel<<<(unsigned)((sc.nblocks + 7) / 8), 256, 0, st>>>(a, k);
     }
     ++p->launches;
     CU(p, cudaGetLastError());
@@ -1449,6 +1619,10 @@ int pgcn_plan_prepare(pgcn_plan* p, int32_t f)
             }
     // pgcn_sddmm walks the forward matrix's schedules (built above); its ring instance of width f needs its attribute
     if (ring && f <= 512 && (rc = sddmm_attr(p, f, p->host_stream))) return rc;
+    // the multi-head calls: the register schedules (built above) and the multi-head SDDMM ring instances of width f
+    if (ring && (f == 128 || f == 256 || f == 512))
+        for (int k = 2; k <= 8; k *= 2)
+            if ((f / k) % 4 == 0 && (rc = sddmm_heads_attr(p, f, k, p->host_stream))) return rc;
     p->prepared = true;
     return 0;
 }
@@ -1952,11 +2126,11 @@ static int attn_check(pgcn_plan* p, const char* what, const float* el, const flo
     return 0;
 }
 
-static int launch_attn(pgcn_plan* p, bool backward, const AttnArgs& a, cudaStream_t st)
+// k heads; vec: every [., k] operand is aligned to the vector loads of its k values (attn_vec)
+static int launch_attn(pgcn_plan* p, bool backward, const AttnArgs& a, cudaStream_t st, int k = 1, bool vec = false)
 {
     const unsigned grid = (unsigned)p->nlong_rows + (unsigned)((p->m + kAttnWarps - 1) / kAttnWarps);
-    if (backward) edge_softmax_backward_kernel<<<grid, kAttnThreads, 0, st>>>(a);
-    else edge_softmax_kernel<<<grid, kAttnThreads, 0, st>>>(a);
+    pick_softmax(k, vec, backward)<<<grid, kAttnThreads, 0, st>>>(a);
     ++p->launches;
     CU(p, cudaGetLastError());
     return 0;
@@ -1996,6 +2170,136 @@ int pgcn_edge_softmax_backward(pgcn_plan* p, const float* el, const float* er_ow
     AttnArgs a = attn_args(p, el, er_own, er_halo, negative_slope);
     a.alpha = alpha; a.dalpha = dalpha; a.out = dpre; a.d_el = d_el;
     return launch_attn(p, true, a, (cudaStream_t)stream);
+}
+
+// ---- multi-head sparse graph attention ------------------------------------------------------------------------------
+
+static int heads_check(pgcn_plan* p, const char* what, int heads)
+{
+    if (!p) return fail(nullptr, PGCN_ERR_INVALID, "null plan");
+    if (heads != 1 && heads != 2 && heads != 4 && heads != 8)
+        return fail(p, PGCN_ERR_INVALID, "%s: heads=%d, not 1, 2, 4 or 8", what, heads);
+    if (!p->bound) return fail(p, PGCN_ERR_STATE, "%s reads the value maps: call pgcn_plan_bind_values first", what);
+    return 0;
+}
+
+static int heads_check_f(pgcn_plan* p, const char* what, int heads, int f)
+{
+    int rc = heads_check(p, what, heads);
+    if (rc) return rc;
+    if ((rc = check_f(p, f))) return rc;
+    if (f % heads != 0) return fail(p, PGCN_ERR_INVALID, "%s: f=%d is not a multiple of heads=%d", what, f, heads);
+    return 0;
+}
+
+// Vector loads of the k values of a row or entry: k floats (4 .. 32 bytes) need alignment to min(4 k, 16) bytes
+static bool attn_vec(int k, std::initializer_list<const void*> ops)
+{
+    const uintptr_t mask = (uintptr_t)std::min(4 * k, 16) - 1;
+    for (const void* q : ops)
+        if (q && (reinterpret_cast<uintptr_t>(q) & mask)) return false;
+    return k > 1;
+}
+
+int pgcn_edge_softmax_heads(pgcn_plan* p, int32_t heads, const float* el, const float* er_own, const float* er_halo,
+                            float negative_slope, float* alpha, void* stream)
+{
+    int rc = heads_check(p, "pgcn_edge_softmax_heads", heads);
+    if (rc || (rc = attn_check(p, "pgcn_edge_softmax_heads", el, er_own, er_halo))) return rc;
+    if (p->m == 0) return 0;
+    if (p->fwd.nnz > 0 && !alpha) return fail(p, PGCN_ERR_INVALID, "null alpha");
+    AttnArgs a = attn_args(p, el, er_own, er_halo, negative_slope);
+    a.out = alpha;
+    return launch_attn(p, false, a, (cudaStream_t)stream, heads, attn_vec(heads, {el, er_own, a.er_halo, alpha}));
+}
+
+int pgcn_edge_softmax_backward_heads(pgcn_plan* p, int32_t heads, const float* el, const float* er_own,
+                                     const float* er_halo, const float* alpha, const float* dalpha, float negative_slope,
+                                     float* dpre, float* d_el, void* stream)
+{
+    int rc = heads_check(p, "pgcn_edge_softmax_backward_heads", heads);
+    if (rc || (rc = attn_check(p, "pgcn_edge_softmax_backward_heads", el, er_own, er_halo))) return rc;
+    if (p->m == 0) return 0;
+    if (!d_el || (p->fwd.nnz > 0 && (!alpha || !dalpha || !dpre)))
+        return fail(p, PGCN_ERR_INVALID, "null alpha/dalpha/dpre/d_el");
+    AttnArgs a = attn_args(p, el, er_own, er_halo, negative_slope);
+    a.alpha = alpha; a.dalpha = dalpha; a.out = dpre; a.d_el = d_el;
+    return launch_attn(p, true, a, (cudaStream_t)stream, heads,
+                       attn_vec(heads, {el, er_own, a.er_halo, alpha, dalpha, dpre, d_el}));
+}
+
+// The unsplit forward exchange of pgcn_forward (both transports), then one multi-head launch over [H_own | halo slab of
+// the call's parity], then the halo copy. The plan's resident values are not read.
+int pgcn_forward_heads(pgcn_plan* p, int32_t heads, const float* alpha, const float* H_own, float* Z, float* H_halo_out,
+                       int32_t f, void* stream)
+{
+    int rc = heads_check_f(p, "pgcn_forward_heads", heads, f);
+    if (rc) return rc;
+    if (p->m > 0 && (!H_own || !Z)) return fail(p, PGCN_ERR_INVALID, "null H_own/Z");
+    if (p->fwd.nnz > 0 && !alpha) return fail(p, PGCN_ERR_INVALID, "null alpha");
+    cudaStream_t st = (cudaStream_t)stream;
+    const HeadArgs ha = {alpha, nullptr, heads};
+    if (p->k == 1)
+        return launch_spmm(p, p->fwd, H_own, p->h > 0 ? p->d_halo_slab : nullptr, p->m, Z, nullptr, p->m, f, 0, st, 0,
+                           false, nullptr, &ha);
+    const bool use_p2p = p->p2p && (f % 4 == 0);
+    if (!use_p2p && !p->comm) return fail(p, PGCN_ERR_STATE, "k=%d: call pgcn_comm_init or pgcn_p2p_import first", p->k);
+    float* halo = use_p2p ? arena_ptr(p->arena, p->off_fwd[0]) : p->d_halo_slab;
+    const float* halo_odd = use_p2p ? arena_ptr(p->arena, p->off_fwd[1]) : nullptr;
+    if ((rc = forward_send(p, H_own, f, use_p2p, false, st))) return rc;
+    if ((rc = forward_wait_all(p, use_p2p, st))) return rc;
+    if ((rc = launch_spmm(p, p->fwd, H_own, p->h > 0 ? halo : nullptr, p->m, Z, nullptr, p->m, f, 0, st, 0, false,
+                          p->h > 0 ? halo_odd : nullptr, &ha)))
+        return rc;
+    if (!H_halo_out || p->h == 0) return 0;
+    const long long n = (long long)p->h * f;
+    copy_halo_kernel<<<grid_for(n, p->num_sms), 256, 0, st>>>(halo, halo_odd, use_p2p ? p->d_epoch : nullptr, H_halo_out, n);
+    ++p->launches;
+    CU(p, cudaGetLastError());
+    return 0;
+}
+
+// The unsplit backward of pgcn_backward with multi-head weights on the transposed records (through their value map).
+int pgcn_backward_heads(pgcn_plan* p, int32_t heads, const float* alpha, const float* gZ, float* G_own, int32_t f,
+                        void* stream)
+{
+    int rc = heads_check_f(p, "pgcn_backward_heads", heads, f);
+    if (rc) return rc;
+    if (p->m > 0 && (!gZ || !G_own)) return fail(p, PGCN_ERR_INVALID, "null gZ/G_own");
+    if (p->fwd.nnz > 0 && !alpha) return fail(p, PGCN_ERR_INVALID, "null alpha");
+    cudaStream_t st = (cudaStream_t)stream;
+    const HeadArgs ha = {alpha, p->tr.d_vmap, heads};
+    if (p->k == 1)
+        return launch_spmm(p, p->tr, gZ, nullptr, p->m, G_own, p->d_hsend_slab, p->m, f, 0, st, 0, false, nullptr, &ha);
+    const bool use_p2p = p->p2p && (f % 4 == 0);
+    if (!use_p2p && !p->comm) return fail(p, PGCN_ERR_STATE, "k=%d: call pgcn_comm_init or pgcn_p2p_import first", p->k);
+    float* rrecv = p->d_rrecv_slab;
+    const float* rrecv_odd = nullptr;
+    if (use_p2p) {
+        if ((rc = advance_epoch(p, st))) return rc;
+        rrecv = arena_ptr(p->arena, p->off_bwd[0]);
+        rrecv_odd = arena_ptr(p->arena, p->off_bwd[1]);
+    }
+    if ((rc = launch_spmm(p, p->tr, gZ, nullptr, p->m, G_own, p->d_hsend_slab, p->m, f, 0, st, 0, false, nullptr, &ha)))
+        return rc;
+    for (int i = 1; i < p->k; ++i) {
+        if (use_p2p) { if ((rc = p2p_put(p, step_dst(p, i), p->d_hsend_slab, f, true, st))) return rc; }
+        else if ((rc = nccl_step(p, p->d_hsend_slab, rrecv, f, 1, i, st))) return rc;
+    }
+    if (use_p2p)
+        for (int i = 1; i < p->k; ++i)
+            if ((rc = p2p_wait(p, step_src(p, i), st))) return rc;
+    return launch_unpack(p, rrecv, G_own, f, st, rrecv_odd);
+}
+
+int pgcn_sddmm_heads(pgcn_plan* p, int32_t heads, const float* gZ, const float* H_own, const float* H_halo,
+                     float* dalpha, int32_t f, void* stream)
+{
+    int rc = heads_check_f(p, "pgcn_sddmm_heads", heads, f);
+    if (rc) return rc;
+    if (p->fwd.nnz > 0 && (!gZ || !H_own || !dalpha)) return fail(p, PGCN_ERR_INVALID, "null gZ/H_own/dalpha");
+    if (p->h > 0 && !H_halo) return fail(p, PGCN_ERR_INVALID, "h=%d but H_halo is null", p->h);
+    return launch_sddmm_heads(p, heads, gZ, H_own, p->h > 0 ? H_halo : nullptr, dalpha, f, (cudaStream_t)stream);
 }
 
 static int host_slots(pgcn_plan* p, int64_t need)

@@ -347,6 +347,206 @@ spmm_rowblock_kernel(const SpmmArgs a)
     }
 }
 
+// Weights of the multi-head aggregation (spmm_heads_kernel): alpha is nnz x NH in forward CSR order; amap takes an
+// entry of the launched records to its forward entry (null: the identity, the forward records themselves); hd = f / NH.
+struct SpmmHeadArgs {
+    const float* alpha;
+    const int* amap;
+    int hd;
+};
+
+// The staged head weights of the NH-head instances: two chunks of NH floats per thread, next to s_cw.
+template <int NH>
+__device__ __forceinline__ float* spmm_head_smem()
+{
+    __shared__ float s_al[2 * kSpmmThreads * NH];
+    return s_al;
+}
+
+// Multi-head aggregation: spmm_rowblock_kernel with one vector per lane (VPL = 1: the rest of a wide row is walked in
+// blockIdx.y tiles) and another weight. Vector v of a lane is weighted by alpha[map(e) * NH + head], head = (its first
+// float) / hd, instead of the entry's value: the same rows, segments, flushes and summation order. The NH weights of a
+// chunk's entries are staged in shared memory next to s_cw, and the next chunk's are in flight in registers.
+// Registers: 4 CTAs of 256 threads per SM instead of 6 (the NH staged weights in flight).
+//
+// Per chunk of LPE edges a lane group stages its (column|flags, value) pairs in shared memory, so
+// the inner loop costs one broadcast LDS.64 per edge instead of two divergence-guarded shuffles;
+// the H row address is one IMAD.WIDE.U32 (32-bit column x row pitch in bytes + 64-bit base); the
+// own/halo base is a select, not a branch; full chunks run a predicate-free loop. Two gathers are in
+// flight per lane group (register double buffer A/B); the next chunk's index pairs are already in
+// flight in registers while the current chunk is processed.
+template <int LPE, int VW, bool HALO, int NH>
+__global__ void __launch_bounds__(kSpmmThreads, 4)
+spmm_heads_kernel(const SpmmArgs a, const SpmmHeadArgs ha)
+{
+    constexpr int VPL = 1;
+    typedef typename Vec<VW>::type vec_t;
+    __shared__ int2 s_cw[2][kSpmmThreads];
+
+    const int lane_w = threadIdx.x & 31;
+    const int gl = threadIdx.x & (LPE - 1);
+    const int gbase = threadIdx.x & ~(LPE - 1);
+    const unsigned gmask = (LPE == 32) ? 0xffffffffu
+                                       : (((1u << (LPE & 31)) - 1u) << (lane_w & ~(LPE - 1)));
+    const int group = (int)((blockIdx.x * (unsigned)kSpmmThreads + threadIdx.x) / LPE);
+    if (group >= a.nblocks) return;           // whole lane groups leave together
+
+    const int4 b = a.blocks[group];
+    const bool seg = b.y < 0;                 // a segment of one split row: row marks are ignored
+    const int lastmask = seg ? 0 : kLastFlag;
+    const int e_end = b.w;
+    int e = b.z;
+    int row = b.x;
+
+    // this lane's slice of a feature row: byte offset of its first vector inside the row
+    const unsigned pitch = (unsigned)a.f * 4u;                       // row pitch in bytes
+    const int f0 = blockIdx.y * (LPE * VPL * VW) + gl * VW;          // first float of vector 0
+    bool fok[VPL];
+#pragma unroll
+    for (int v = 0; v < VPL; ++v) fok[v] = f0 + v * LPE * VW < a.f;  // f % VW == 0 (launcher)
+    const bool odd = epoch_odd(a.epoch);
+    const float* H0 = (!HALO && odd) ? a.H_odd : a.H0;
+    const float* H1 = (HALO && odd) ? a.H_odd : a.H1;
+    const char* hb0 = reinterpret_cast<const char*>(H0) + (size_t)f0 * 4;
+    const char* hb1 = HALO ? reinterpret_cast<const char*>(H1) + (size_t)f0 * 4 - (size_t)a.split * pitch
+                           : hb0;
+    // the head of each vector (a vector never straddles two heads: hd % VW == 0, launcher)
+    float* s_al = spmm_head_smem<NH>();
+    int hv[VPL];
+    float al_next[NH];
+#pragma unroll
+    for (int v = 0; v < VPL; ++v) hv[v] = fok[v] ? (f0 + v * LPE * VW) / ha.hd : 0;
+    // the NH weights of entry ee (zero past the block's end)
+    auto ld_alpha = [&](float (&al)[NH], int ee) {
+        const bool ok = ee < e_end;
+        const int me = !ok ? 0 : (ha.amap ? __ldg(ha.amap + ee) : ee);
+#pragma unroll
+        for (int h = 0; h < NH; ++h) al[h] = ok ? __ldg(ha.alpha + (size_t)me * NH + h) : 0.f;
+    };
+    auto st_alpha = [&](int bf, const float (&al)[NH]) {
+#pragma unroll
+        for (int h = 0; h < NH; ++h) s_al[((size_t)bf * kSpmmThreads + threadIdx.x) * NH + h] = al[h];
+    };
+
+#if PGCN_LDMODE >= 2
+    const unsigned long long pol_hot = l2_policy_evict_last();
+    const unsigned long long pol_cold = l2_policy_evict_first();
+#endif
+
+    vec_t acc[VPL];
+#pragma unroll
+    for (int v = 0; v < VPL; ++v) acc[v] = vzero((vec_t*)nullptr);
+
+    auto flush_row = [&]() {
+        // write the finished row, clear the accumulator, advance to the next row of the block
+        const int orow = (a.rowids != nullptr) ? __ldg(a.rowids + row) : row;
+        const bool relu_row = a.relu && (a.final == nullptr || __ldg(a.final + row) != 0);
+        char* zb = (orow < a.zsplit)
+                       ? reinterpret_cast<char*>(a.Z0) + (size_t)(unsigned)orow * pitch
+                       : reinterpret_cast<char*>(a.Z1) + (size_t)(unsigned)(orow - a.zsplit) * pitch;
+        zb += (size_t)f0 * 4;
+#pragma unroll
+        for (int v = 0; v < VPL; ++v) {
+            if (fok[v]) {
+                vec_t* zp = reinterpret_cast<vec_t*>(zb + v * LPE * VW * 4);
+                if (a.beta) vadd(acc[v], *zp);
+                if (relu_row) acc[v] = vrelu(acc[v]);
+                st_out(zp, acc[v]);
+            }
+            acc[v] = vzero((vec_t*)nullptr);
+        }
+        ++row;
+    };
+
+    auto gather = [&](vec_t (&r)[VPL], int craw) {
+        const unsigned cj = (unsigned)(craw & kColMask);
+        const char* hb = (HALO && cj >= (unsigned)a.split) ? hb1 : hb0;
+        const char* hp = hb + (size_t)cj * pitch;
+#if PGCN_LDMODE >= 2
+        const unsigned long long pol = (craw & kColdFlag) ? pol_cold : pol_hot;
+#pragma unroll
+        for (int v = 0; v < VPL; ++v)
+            if (fok[v]) r[v] = ld_feat_hint(reinterpret_cast<const vec_t*>(hp + v * LPE * VW * 4), pol);
+#else
+#pragma unroll
+        for (int v = 0; v < VPL; ++v)
+            if (fok[v]) r[v] = ld_feat(reinterpret_cast<const vec_t*>(hp + v * LPE * VW * 4));
+#endif
+    };
+    auto consume = [&](const vec_t (&r)[VPL], int2 cw, int j, int bf) {
+#pragma unroll
+        for (int v = 0; v < VPL; ++v)
+            if (fok[v]) vfma(acc[v], s_al[((size_t)bf * kSpmmThreads + gbase + j) * NH + hv[v]], r[v]);
+        if (cw.x & lastmask) flush_row();
+    };
+
+    // chunk 0 -> shared; chunk 1 -> registers (in flight)
+    int buf = 0;
+    {
+        int2 cw = make_int2(0, 0);
+        if (e + gl < e_end) cw = ld_entry(a.pieces, e + gl);
+        s_cw[0][threadIdx.x] = cw;
+        float al[NH];
+        ld_alpha(al, e + gl);
+        st_alpha(0, al);
+    }
+    int2 cw_next = make_int2(0, 0);
+    if (e + LPE + gl < e_end) cw_next = ld_entry(a.pieces, e + LPE + gl);
+    ld_alpha(al_next, e + LPE + gl);
+    __syncwarp(gmask);
+
+    while (e < e_end) {
+        const int n = min(LPE, e_end - e);
+        const int2* cwp = &s_cw[buf][gbase];
+        // two register buffers: edge j+1 is gathered before edge j is consumed. (A ring of 4 buffers
+        // was measured 27 % SLOWER on C2: 1.31 vs 1.03 ms — deeper per-warp pipelines lose to occupancy.)
+        vec_t rA[VPL], rB[VPL];
+        int2 cwA = cwp[0], cwB;
+        gather(rA, cwA.x);
+        if (n == LPE) {
+            // full chunk: no bounds predicates inside
+#pragma unroll 1
+            for (int j = 0; j < LPE - 2; j += 2) {
+                cwB = cwp[j + 1];
+                gather(rB, cwB.x);
+                consume(rA, cwA, j, buf);
+                cwA = cwp[j + 2];
+                gather(rA, cwA.x);
+                consume(rB, cwB, j + 1, buf);
+            }
+            cwB = cwp[LPE - 1];
+            gather(rB, cwB.x);
+            consume(rA, cwA, LPE - 2, buf);
+            consume(rB, cwB, LPE - 1, buf);
+        } else {
+#pragma unroll 1
+            for (int j = 0; j < n; j += 2) {
+                const bool hasB = j + 1 < n;
+                if (hasB) { cwB = cwp[j + 1]; gather(rB, cwB.x); }
+                consume(rA, cwA, j, buf);
+                if (j + 2 < n) { cwA = cwp[j + 2]; gather(rA, cwA.x); }
+                if (hasB) consume(rB, cwB, j + 1, buf);
+            }
+        }
+        e += n;
+        // publish the next chunk (it has been in flight since the previous iteration), fetch the one after
+        buf ^= 1;
+        s_cw[buf][threadIdx.x] = cw_next;
+        cw_next = make_int2(0, 0);
+        if (e + LPE + gl < e_end) cw_next = ld_entry(a.pieces, e + LPE + gl);
+        st_alpha(buf, al_next);
+        ld_alpha(al_next, e + LPE + gl);
+        __syncwarp(gmask);
+    }
+
+    if (seg) {
+        char* pb = reinterpret_cast<char*>(a.partial) + (size_t)(unsigned)(-b.y - 1) * pitch + (size_t)f0 * 4;
+#pragma unroll
+        for (int v = 0; v < VPL; ++v)
+            if (fok[v]) *reinterpret_cast<vec_t*>(pb + v * LPE * VW * 4) = acc[v];
+    }
+}
+
 // Rows without any stored entry are squeezed out of the schedule; they are zero-filled here.
 struct ZeroArgs {
     const int* rows; int nrows_empty;

@@ -318,6 +318,130 @@ class PGATAttention(torch.autograd.Function):
         return None, dZ, d_el, d_er, None
 
 
+HEADS = (1, 2, 4, 8)
+
+
+def _check_head_scores(plan, x, rows, heads, what):
+    if not x.is_cuda:
+        raise RuntimeError("%s must be a CUDA tensor: the PGCN H100 path has no CPU fallback" % what)
+    if x.dtype != torch.float32:
+        raise TypeError("%s must be float32, got %s" % (what, x.dtype))
+    if x.dim() != 2 or x.shape[0] != rows or x.shape[1] != heads:
+        raise ValueError("%s must be [%d, %d], got %s" % (what, rows, heads, tuple(x.shape)))
+    x = x.detach()
+    return (x.index_select(0, plan.owned_index()) if plan.layout == "global" else x).contiguous()
+
+
+class PGATMultiHeadAttention(torch.autograd.Function):
+    """Multi-head sparse graph attention over the plan's stored pattern: K = el.shape[1] heads (1, 2, 4 or 8) of width
+    d = f / K, concatenated.
+
+        PGATMultiHeadAttention.apply(A, Z, el, er, negative_slope)
+        s_eh = LeakyReLU(el[row(e), h] + er[col(e), h]),  alpha_.h = softmax of s_.h over each row's stored entries,
+        out[:, h d:(h+1) d] = A(alpha[:, h]) Z[:, h d:(h+1) d]
+
+    Z is [rows, f], el and er are [rows, K] fp32 CUDA tensors, out is [rows, f] (rows = m in the "local" layout, n in the
+    "global" one, as PGATAttention). One exchange per layer carries the f-wide Z for every head, and er of the halo
+    columns travels once for all heads (pgcn_halo_rows, rows padded to a multiple of 4 floats). The kernels take alpha
+    ([nnz, K]) as an argument, so the plan's resident values are never rewritten: a PSpMM on the same plan needs no
+    restore. Backward: dZ = A(alpha)^T gOut per head (pgcn_backward_heads), dalpha from pgcn_sddmm_heads, dpre and d_el
+    from the softmax backward, d_er[:, h] = A(dpre[:, h])^T 1 (pgcn_backward_heads on an m x 4K matrix of ones, column
+    4h), so the plan's f_max must be at least max(f, 4K). Deterministic. The exchange is the unsplit one (no per-source
+    overlap). The plan must be bound (PgcnPlan.bind_values)."""
+
+    @staticmethod
+    def forward(ctx, A, Z, el, er, negative_slope=0.2):
+        rows = A.n if A.layout == "global" else A.m
+        if el.dim() != 2:
+            raise ValueError("el must be [%d, heads], got %s" % (rows, tuple(el.shape)))
+        K = el.shape[1]
+        if K not in HEADS:
+            raise ValueError("heads=%d: the multi-head kernels take 1, 2, 4 or 8 heads" % K)
+        Z_own = _check_feat(A, Z, rows, "Z")
+        f = Z_own.shape[1]
+        if f % K:
+            raise ValueError("f=%d is not a multiple of heads=%d" % (f, K))
+        if A.f_max < 4 * K:
+            raise ValueError("heads=%d: the backward aggregates rows of 4 x heads = %d floats, the plan's f_max is %d"
+                             % (K, 4 * K, A.f_max))
+        if A.layout == "global":
+            Z_own = Z_own.index_select(0, A.owned_index())
+        el_own = _check_head_scores(A, el, rows, K, "el")
+        er_own = _check_head_scores(A, er, rows, K, "er")
+        lp = A.lp
+        dev = Z_own.device
+        slope = float(negative_slope)
+        lib = cabi.load()
+        with torch.cuda.device(dev):
+            if not A._bound:
+                raise RuntimeError("PGATMultiHeadAttention reads the plan's value maps: call PgcnPlan.bind_values() once "
+                                   "(set-up, before any CUDA-graph capture)")
+            er_halo = torch.empty((lp.h, K), dtype=torch.float32, device=dev)
+            if lp.k > 1:
+                w = (K + 3) // 4 * 4
+                erw = torch.zeros((lp.m, w), dtype=torch.float32, device=dev)
+                erw[:, :K] = er_own
+                er_halo_w = torch.empty((lp.h, w), dtype=torch.float32, device=dev)
+                cabi.check(lib.pgcn_halo_rows(A.handle, erw.data_ptr(), er_halo_w.data_ptr(), w, _stream_ptr()),
+                           A.handle)
+                A.count_exchange(backward=False)
+                er_halo = er_halo_w[:, :K].contiguous()
+            alpha = torch.empty((lp.nnz(), K), dtype=torch.float32, device=dev)
+            cabi.check(lib.pgcn_edge_softmax_heads(A.handle, K, el_own.data_ptr(), er_own.data_ptr(), er_halo.data_ptr(),
+                                                   slope, alpha.data_ptr(), _stream_ptr()), A.handle)
+            out = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+            Z_halo = torch.empty((lp.h, f), dtype=torch.float32, device=dev)
+            keep = lp.k > 1 and lp.h > 0
+            cabi.check(lib.pgcn_forward_heads(A.handle, K, alpha.data_ptr(), Z_own.data_ptr(), out.data_ptr(),
+                                              Z_halo.data_ptr() if keep else None, f, _stream_ptr()), A.handle)
+            if lp.k > 1:
+                A.count_exchange(backward=False)
+        ctx.plan, ctx.rows, ctx.slope, ctx.heads = A, rows, slope, K
+        ctx.save_for_backward(alpha, Z_own, Z_halo, el_own, er_own, er_halo)
+        return _to_layout(A, out, rows)
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        A, rows, slope, K = ctx.plan, ctx.rows, ctx.slope, ctx.heads
+        alpha, Z_own, Z_halo, el_own, er_own, er_halo = ctx.saved_tensors
+        g = _check_feat(A, grad_output, rows, "grad_output")
+        if A.layout == "global":
+            g = g.index_select(0, A.owned_index())
+        lp = A.lp
+        f = g.shape[1]
+        dev = g.device
+        lib = cabi.load()
+        dZ = d_el = d_er = None
+        with torch.cuda.device(dev):
+            if ctx.needs_input_grad[1]:
+                G = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+                cabi.check(lib.pgcn_backward_heads(A.handle, K, alpha.data_ptr(), g.data_ptr(), G.data_ptr(), f,
+                                                   _stream_ptr()), A.handle)
+                if lp.k > 1:
+                    A.count_exchange(backward=True)
+                dZ = _to_layout(A, G, rows)
+            if ctx.needs_input_grad[2] or ctx.needs_input_grad[3]:
+                dalpha = torch.empty_like(alpha)
+                cabi.check(lib.pgcn_sddmm_heads(A.handle, K, g.data_ptr(), Z_own.data_ptr(), Z_halo.data_ptr(),
+                                                dalpha.data_ptr(), f, _stream_ptr()), A.handle)
+                dpre = torch.empty_like(alpha)
+                gel = torch.empty((lp.m, K), dtype=torch.float32, device=dev)
+                cabi.check(lib.pgcn_edge_softmax_backward_heads(A.handle, K, el_own.data_ptr(), er_own.data_ptr(),
+                                                                er_halo.data_ptr(), alpha.data_ptr(), dalpha.data_ptr(),
+                                                                slope, dpre.data_ptr(), gel.data_ptr(), _stream_ptr()),
+                           A.handle)
+                d_el = _to_layout(A, gel, rows) if ctx.needs_input_grad[2] else None
+                if ctx.needs_input_grad[3]:
+                    ones = torch.ones((lp.m, 4 * K), dtype=torch.float32, device=dev)
+                    D = torch.empty((lp.m, 4 * K), dtype=torch.float32, device=dev)
+                    cabi.check(lib.pgcn_backward_heads(A.handle, K, dpre.data_ptr(), ones.data_ptr(), D.data_ptr(),
+                                                       4 * K, _stream_ptr()), A.handle)
+                    if lp.k > 1:
+                        A.count_exchange(backward=True)
+                    d_er = _to_layout(A, D[:, 0::4].contiguous(), rows)
+        return None, dZ, d_el, d_er, None
+
+
 # ---- the pieces, individually callable (NCCL transport), mirroring communicate_fgm ----------------
 
 def spmm_local(plan, H_own, H_halo=None, transpose=False):

@@ -1,6 +1,6 @@
 """PGAT trainer CLI — the reference's graph-attention surface (GPU/PGAT.py:124-286) over the H100 operator.
 
-    python PGAT.py -a A.mtx -p A.mtx.8.hp -b nccl -s 8 -l 2 -f 16 [--seed 0] [--negative-slope 1.0]
+    python PGAT.py -a A.mtx -p A.mtx.8.hp -b nccl -s 8 -l 2 -f 16 [--seed 0] [--negative-slope 1.0] [--heads K]
 
 Kept from the reference: flags -a -p -b -s -l -f; rank/size from SLURM_PROCID / SLURM_NPROCS with torchrun's RANK /
 WORLD_SIZE as a fallback (as pgcn.py); inputs H[i, :] = i (:186-188) and labels i % f (:192); L x PGAT layers with the
@@ -14,6 +14,11 @@ layer; the score goes through LeakyReLU(negative_slope), whose default here, 1.0
 flags are honoured (the reference overwrites them); every tensor is [m_local, f], each rank's loss is
 sum_owned nll / n and the printed loss is its all-reduced sum, the global mean. `-b gloo` is refused: the H100 path has no
 CPU fallback (the fp64 oracle lives under oracle/ and is test infrastructure).
+
+--heads K (1, 2, 4 or 8, dividing f; default 1): K attention heads of width d = f / K per layer, concatenated, so every
+layer stays f -> f. K = 1 is the single-head layer above, with the same parameter draws. K > 1: Linear(f, f, bias=False)
+and a (2d x K) attention matrix, both xavier_normal with the relu gain in that order; el[:, h] = Z_h a[:d, h] and
+er[:, h] = Z_h a[d:, h] for head h's slice Z_h of Z (op.PGATMultiHeadAttention).
 """
 import getopt
 import os
@@ -26,21 +31,23 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import graphio, plan as planmod
-from .op import PGATAttention
+from .op import HEADS, PGATAttention, PGATMultiHeadAttention
 from .pgcn import average_gradients, initialize_parameters, init_process
 
 
 class PGAT(nn.Module):
     """GPU/PGAT.py:124-148 with the plan handle in place of the dense matrix and a sparse edge softmax."""
 
-    def __init__(self, A, in_features, out_features, negative_slope=0.2):
+    def __init__(self, A, in_features, out_features, negative_slope=0.2, heads=1):
         super().__init__()
         self.in_features = in_features
         self.out_features = out_features
         self.A = A
         self.negative_slope = negative_slope
+        self.heads = heads
         self.linear = nn.Linear(in_features, out_features, bias=False)
-        self.attention = nn.Parameter(torch.empty(size=(2 * out_features, 1)))
+        d = out_features // heads
+        self.attention = nn.Parameter(torch.empty(size=(2 * out_features, 1) if heads == 1 else (2 * d, heads)))
         self.reset_parameters()
 
     def reset_parameters(self):
@@ -51,13 +58,19 @@ class PGAT(nn.Module):
     def forward(self, H):
         Z = self.linear(H)
         f = self.out_features
+        if self.heads > 1:
+            d = f // self.heads
+            Zh = Z.view(Z.shape[0], self.heads, d)
+            el = torch.einsum("nhd,dh->nh", Zh, self.attention[:d])
+            er = torch.einsum("nhd,dh->nh", Zh, self.attention[d:])
+            return PGATMultiHeadAttention.apply(self.A, Z, el, er, self.negative_slope)
         el = torch.matmul(Z, self.attention[:f, :]).squeeze(1)
         er = torch.matmul(Z, self.attention[f:, :]).squeeze(1)
         return PGATAttention.apply(self.A, Z, el, er, self.negative_slope)
 
 
 def run(rank, size, nlayers, nfeatures, path_A, path_partvec, backend, transport="auto", out=sys.stdout, seed=None,
-        negative_slope=1.0, epochs=50):
+        negative_slope=1.0, epochs=50, heads=1):
     if backend != "nccl":
         raise RuntimeError("backend '%s': the H100 PGAT path runs on CUDA devices over NCCL/NVLink only "
                            "(no CPU fallback); use -b nccl" % backend)
@@ -68,7 +81,8 @@ def run(rank, size, nlayers, nfeatures, path_A, path_partvec, backend, transport
     graphio.check_partvec(partvec, size)
     lp_host = planmod.build_local_plan(A, partvec, rank, size)
     n = lp_host.n
-    plan = planmod.PgcnPlan(lp_host, nfeatures, device=device)
+    # the multi-head backward gets d_er from an aggregation of width 4 K (PGATMultiHeadAttention)
+    plan = planmod.PgcnPlan(lp_host, nfeatures if heads == 1 else max(nfeatures, 4 * heads), device=device)
     used = plan.init_comm(transport=transport)
     plan.bind_values()
     lp = plan.lp
@@ -79,7 +93,7 @@ def run(rank, size, nlayers, nfeatures, path_A, path_partvec, backend, transport
 
     if seed is not None:
         torch.manual_seed(seed)
-    model = nn.Sequential(*[PGAT(plan, nfeatures, nfeatures, negative_slope) for _ in range(nlayers)]).to(device)
+    model = nn.Sequential(*[PGAT(plan, nfeatures, nfeatures, negative_slope, heads) for _ in range(nlayers)]).to(device)
     if size > 1:
         initialize_parameters(model, size)
     optimizer = torch.optim.Adam(model.parameters(), lr=1e-3)
@@ -117,7 +131,7 @@ def main(argv):
     rank = int(os.environ.get("SLURM_PROCID", os.environ.get("RANK", "0")))
     os.environ["RANK"] = str(rank)
     try:
-        opts, _ = getopt.getopt(argv, "a:p:b:s:l:f:", ["transport=", "seed=", "negative-slope="])
+        opts, _ = getopt.getopt(argv, "a:p:b:s:l:f:", ["transport=", "seed=", "negative-slope=", "heads="])
     except getopt.GetoptError:
         print("a:p:b:", flush=True)                                       # the reference's usage text
         sys.exit(2)
@@ -144,9 +158,16 @@ def main(argv):
             kw["seed"] = int(arg)
         elif opt == "--negative-slope":
             kw["negative_slope"] = float(arg)
-    if path_A is None or path_partvec is None or nlayers is None or nfeatures is None:
+        elif opt == "--heads":
+            try:
+                kw["heads"] = int(arg)
+            except ValueError:
+                kw["heads"] = -1
+    heads = kw.get("heads", 1)
+    if (path_A is None or path_partvec is None or nlayers is None or nfeatures is None or heads not in HEADS
+            or nfeatures % heads):
         print("usage: PGAT.py -a <A.mtx> -p <partvec> -b nccl -s <nparts> -l <nlayers> -f <nfeatures> "
-              "[--seed N] [--negative-slope S]", flush=True)
+              "[--seed N] [--negative-slope S] [--heads 1|2|4|8, dividing nfeatures]", flush=True)
         sys.exit(2)
     os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
     os.environ.setdefault("MASTER_PORT", "29500")
