@@ -60,14 +60,25 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
         ::"r"(dst), "l"(src), "r"(bytes), "r"(bar), "l"(pol) : "memory");
 }
 // 2-D tensor-map TMA in tile mode: one row tile of H (row r, column offset x; the map's box is {tile, 1 row}) lands
-// in one row slot (UTMALDG.2D). The map carries the row pitch, so the issuing lane computes no address.
-__device__ __forceinline__ void tma_row(uint32_t dst, const CUtensorMap* tm, int x, int r, uint32_t bar,
-                                       unsigned long long pol)
+// in one row slot (UTMALDG.2D). The map carries the row pitch, so no address is computed.
+// The copy is issued ONCE for the whole warp, by the lane elect.sync picks. Every lane calls it, converged, with
+// warp-uniform operands; ptxas then emits a bare UTMALDG fed from uniform registers. A per-lane form (each lane its
+// own row) costs a waterfall loop per copy instead: ELECT, six R2UR, two PLOP3 and a branch around each UTMALDG.
+__device__ __forceinline__ void tma_row_warp(uint32_t dst, const CUtensorMap* tm, int x, int r, uint32_t bar,
+                                            unsigned long long pol)
 {
     asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.L2::cache_hint"
-        " [%0], [%1, {%2, %3}], [%4], %5;"
+        "{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\t"
+        "@p cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.L2::cache_hint"
+        " [%0], [%1, {%2, %3}], [%4], %5;\n\t}"
         ::"r"(dst), "l"(tm), "r"(x), "r"(r), "r"(bar), "l"(pol) : "memory");
+}
+// A value every lane of the warp holds, moved into a uniform register (REDUX writes one), so that ptxas can treat
+// what is computed from it as warp-uniform.
+__device__ __forceinline__ uint32_t warp_uniform(uint32_t v) { return __reduce_or_sync(0xffffffffu, v); }
+__device__ __forceinline__ unsigned long long warp_uniform64(unsigned long long v)
+{
+    return ((unsigned long long)warp_uniform((uint32_t)(v >> 32)) << 32) | warp_uniform((uint32_t)v);
 }
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, unsigned long long pol)
 {
@@ -99,6 +110,14 @@ __device__ __noinline__ void ring_store_row(V a0, V a1, const int* rowids, int r
         st_out(zq, a1);
     }
 }
+
+// Cost probe, for variant builds only (PGCN_B200_VARIANT + PGCN_B200_DEFS=-DPGCN_RING_DIAG=n, timed by
+// tools/tune_spmm.py --gather-sweep --all-hit): bit 0 drops the consumer's slot reads and FFMA, bit 1 makes the
+// tensor-map ring issue no row copy and wait on none. Such a build computes wrong results; the library is built with 0.
+#ifndef PGCN_RING_DIAG
+#define PGCN_RING_DIAG 0
+#endif
+constexpr bool kDiagNoFma = (PGCN_RING_DIAG & 1) != 0, kDiagNoCopy = (PGCN_RING_DIAG & 2) != 0;
 
 constexpr int kRingPieces = 4;       // index pieces (32 entries, kPieceBytes each) resident per warp
 
@@ -165,8 +184,9 @@ __device__ __forceinline__ void reg_set(uint32_t (&a)[N], int i, uint32_t v)
 // one bulk copy: 32 plain column indices, 32 values, a row-end bit mask and a cold-column bit mask), a group =
 // entries [G g, G g + G) (one completion unit of the row ring, slot group g % NG). A row block [e0, e1) starts and
 // ends anywhere; entries of its first / last group outside the block are masked. The steady state per group is:
-//   issue   : one broadcast LDS.64 (masks), lanes 0..G-1 read their column index and fire one TMA copy each;
-//             lane 0 arms the group's mbarrier with G x row bytes;
+//   issue   : one broadcast LDS.64 (masks); lane 0 arms the group's mbarrier with G x row bytes. MODE 2: the warp reads
+//             the G column indices 4 at a time (broadcast LDS.128), moves each into a uniform register and one
+//             elected lane fires the copy (tma_row_warp). MODES 0 / 1: lanes 0..G-1 each copy the row of their column;
 //   consume : mbarrier wait, 8 x LDS.128 rows + 2 x LDS.128 values (straight from the resident piece), 32 FFMA per
 //             8 edges; a row-end test per edge only in groups whose row-end mask is non-zero.
 // Pieces stay resident until their last group has been CONSUMED (the values are read at consumption time), so
@@ -199,7 +219,8 @@ __device__ __forceinline__ void ring_body(const SpmmArgs& a, const RingArgs& ra,
 
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     unsigned char* wbase = ring_smem + (size_t)warp * ring_warp_bytes(TF, NS, NG);
-    const uint32_t s_data = smem_u32(wbase);                             // NS slots of RB bytes
+    // MODE 2 issues each row copy once per warp from uniform registers (tma_row_warp)
+    const uint32_t s_data = MODE == 2 ? warp_uniform(smem_u32(wbase)) : smem_u32(wbase);   // NS slots of RB bytes
     const uint32_t s_idx = s_data + NS * RB;                             // NP pieces
     const uint32_t s_gbar = s_idx + NP * kPieceBytes;                    // NG group barriers
     const uint32_t s_pbar = s_gbar + NG * 8;                             // NP piece barriers
@@ -214,8 +235,8 @@ __device__ __forceinline__ void ring_body(const SpmmArgs& a, const RingArgs& ra,
     }
     __syncwarp();
 
-    const unsigned long long pol_hot = l2_policy_evict_last();
-    const unsigned long long pol_cold = l2_policy_evict_first();
+    const unsigned long long pol_hot = MODE == 2 ? warp_uniform64(l2_policy_evict_last()) : l2_policy_evict_last();
+    const unsigned long long pol_cold = MODE == 2 ? warp_uniform64(l2_policy_evict_first()) : l2_policy_evict_first();
     // row pitch f * 4; tile t covers floats [t TF, t TF + TF)
     const size_t pitch = (size_t)a.f * 4;
     const unsigned usplit = HALO ? (unsigned)a.split : 0xffffffffu;
@@ -237,14 +258,22 @@ __device__ __forceinline__ void ring_body(const SpmmArgs& a, const RingArgs& ra,
         if (lane == 0) w = (int)atomicAdd(counter, 1u);
         w = __shfl_sync(0xffffffffu, w, 0);
     }
+    if (MODE == 2) w = (int)warp_uniform((uint32_t)w);
 
     while (w < nitems) {
         const int tile = w / a.nblocks, blk = w - tile * a.nblocks;
         const size_t toff = (size_t)tile * RB;
+        const int tx = MODE == 2 ? (int)warp_uniform((uint32_t)(tile * TF)) : 0;   // the tile's first column in H
         const bool odd = MODE != 2 && epoch_odd(a.epoch);
         const char* hb0 = reinterpret_cast<const char*>((!HALO && odd) ? a.H_odd : a.H0) + toff;
         const char* hb1 = HALO ? reinterpret_cast<const char*>(odd ? a.H_odd : a.H1) + toff - (size_t)a.split * pitch : hb0;
-        const int4 b = __ldg(a.blocks + blk);
+        int4 b = __ldg(a.blocks + blk);
+        if (MODE == 2) {
+            // uniform block bounds make every loop and branch around the warp-level copies warp-uniform, so ptxas keeps
+            // their operands in uniform registers (else it moves them back, and wraps each copy in an ELECT loop)
+            b = make_int4((int)warp_uniform((uint32_t)b.x), (int)warp_uniform((uint32_t)b.y),
+                          (int)warp_uniform((uint32_t)b.z), (int)warp_uniform((uint32_t)b.w));
+        }
         const bool seg = b.y < 0;
         const int e0 = b.z, e1 = b.w;
         int row = b.x;
@@ -286,8 +315,9 @@ __device__ __forceinline__ void ring_body(const SpmmArgs& a, const RingArgs& ra,
             for (int v = 0; v < NV; ++v) acc[v] = vzero((V*)nullptr);
             ++row;
         };
-        // issue the group at sub-position qs of piece `pi` into slot group sg; vm = valid entries (FULL inside the block)
-        auto issue = [&](int qs, int sg, uint32_t vm) {
+        // issue the group at sub-position qs of piece `pi` into slot group sg; vm = valid entries (FULL inside the block:
+        // `whole`, a compile-time constant at every call)
+        auto issue = [&](int qs, int sg, uint32_t vm, bool whole) {
             // {row-end mask, cold mask} of the piece; 64-float slices use the cold mask of their own (larger) hot set
             uint2 m;
             if (TF == 64) { const uint4 q = *reinterpret_cast<const uint4*>(pi + 64); m = make_uint2(q.x, q.z); }
@@ -312,16 +342,34 @@ __device__ __forceinline__ void ring_body(const SpmmArgs& a, const RingArgs& ra,
                 cp_async_commit();
                 return;
             }
+            if (kDiagNoCopy && MODE == 2) return;
             if (lane == 0) mbar_expect_tx(s_gbar + sg * 8, (uint32_t)__popc(vm) * RB);
+            if (MODE == 2) {
+                // the whole warp walks the group's columns 4 at a time (broadcast LDS.128); one elected lane copies
+                const uint32_t vu = whole ? FULL : warp_uniform(vm), cu = warp_uniform(cm);
+                const uint32_t dst = s_data + sg * G * RB, bar = s_gbar + sg * 8;
+#pragma unroll 1
+                for (int j = 0; j < G; j += 4) {
+                    const int4 c4 = *reinterpret_cast<const int4*>(cols + j);
+                    const int cc[4] = {c4.x, c4.y, c4.z, c4.w};
+                    const uint32_t vj = vu >> j, cmj = cu >> j;
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) {
+                        if (whole || (vj >> k & 1)) {
+                            const unsigned cj = warp_uniform((unsigned)cc[k]);
+                            const bool halo = HALO && cj >= usplit;
+                            tma_row_warp(dst + (j + k) * RB, halo ? tm1 : tm0, tx, (int)(halo ? cj - usplit : cj), bar,
+                                         (cmj >> k & 1) ? pol_cold : pol_hot);
+                        }
+                    }
+                }
+                return;
+            }
             if (lane < G && (vm >> lane & 1)) {
                 const unsigned cj = (unsigned)cols[lane];
                 const bool halo = cj >= usplit;
                 const unsigned long long pol = (cm >> lane & 1) ? pol_cold : pol_hot;
-                if (MODE == 2)
-                    tma_row(s_data + (sg * G + lane) * RB, halo ? tm1 : tm0, tile * TF,
-                            (int)(halo ? cj - usplit : cj), s_gbar + sg * 8, pol);
-                else
-                    bulk_g2s(s_data + (sg * G + lane) * RB, (halo ? hb1 : hb0) + (size_t)cj * pitch, RB, s_gbar + sg * 8, pol);
+                bulk_g2s(s_data + (sg * G + lane) * RB, (halo ? hb1 : hb0) + (size_t)cj * pitch, RB, s_gbar + sg * 8, pol);
             }
         };
         // consume slot group sg = the group at sub-position qs of piece `pc`
@@ -331,8 +379,8 @@ __device__ __forceinline__ void ring_body(const SpmmArgs& a, const RingArgs& ra,
                 if (MODE == 1) cp_async_wait<NG - 1>();
                 return;
             }
-            if (MODE != 1) { mbar_wait(s_gbar + sg * 8, (gpar >> sg) & 1); gpar ^= 1u << sg; }
-            else cp_async_wait<NG - 1>();
+            if (MODE == 1) cp_async_wait<NG - 1>();
+            else if (!(kDiagNoCopy && MODE == 2)) { mbar_wait(s_gbar + sg * 8, (gpar >> sg) & 1); gpar ^= 1u << sg; }
             const uint32_t em = reg_get(emask, sg);
             const V* slot = data_gen + (size_t)(sg * G) * RV;
             const float* wv = reinterpret_cast<const float*>(pc) + 32 + qs * G;
@@ -351,12 +399,12 @@ __device__ __forceinline__ void ring_body(const SpmmArgs& a, const RingArgs& ra,
 #pragma unroll
                         for (int j = 0; j < 8; ++j)
 #pragma unroll
-                            for (int v = 0; v < NV; ++v) vfma(acc[v], w[j], r[j][v]);
+                            for (int v = 0; v < NV; ++v) if (!kDiagNoFma) vfma(acc[v], w[j], r[j][v]);
                     } else {
 #pragma unroll
                         for (int j = 0; j < 8; ++j) {
 #pragma unroll
-                            for (int v = 0; v < NV; ++v) vfma(acc[v], w[j], r[j][v]);
+                            for (int v = 0; v < NV; ++v) if (!kDiagNoFma) vfma(acc[v], w[j], r[j][v]);
                             if (em >> (c + j) & 1) flush_row();
                         }
                     }
@@ -367,7 +415,7 @@ __device__ __forceinline__ void ring_body(const SpmmArgs& a, const RingArgs& ra,
                     if (vm >> j & 1) {
                         const float wj = wv[j];
 #pragma unroll
-                        for (int v = 0; v < NV; ++v) vfma(acc[v], wj, slot[j * RV + v * 32]);
+                        for (int v = 0; v < NV; ++v) if (!kDiagNoFma) vfma(acc[v], wj, slot[j * RV + v * 32]);
                         if (em >> j & 1) flush_row();
                     }
                 }
@@ -385,7 +433,7 @@ __device__ __forceinline__ void ring_body(const SpmmArgs& a, const RingArgs& ra,
         auto issue_checked = [&](int gi, int qs, int sg) {
             const uint32_t vm = group_mask(gi);
             if (vm == 0) { reg_set(vmask, sg, 0u); if (MODE == 1) cp_async_commit(); return; }
-            issue(qs, sg, vm);
+            issue(qs, sg, vm, false);
         };
 
         // prologue: index pieces in flight, first piece landed, the first NG groups issued
@@ -415,7 +463,7 @@ __device__ __forceinline__ void ring_body(const SpmmArgs& a, const RingArgs& ra,
                 const int Pi = P + (idx + NG) / PG;                      // its piece
                 if (interior) {
                     if (qi == 0) wait_piece();
-                    issue(qi, sg, FULL);
+                    issue(qi, sg, FULL, true);
                 } else {
                     if (qi == 0 && Pi <= P1) wait_piece();               // first group of a new piece
                     if (Pi <= P1) issue_checked(PG * Pi + qi, qi, sg);
@@ -438,6 +486,7 @@ __device__ __forceinline__ void ring_body(const SpmmArgs& a, const RingArgs& ra,
         if (!counter) break;
         if (lane == 0) w = (int)atomicAdd(counter, 1u);
         w = __shfl_sync(0xffffffffu, w, 0);
+        if (MODE == 2) w = (int)warp_uniform((uint32_t)w);
     }
     if (MODE == 1) cp_async_wait<0>();
 }
@@ -456,8 +505,11 @@ __global__ void __launch_bounds__(ring_cta_warps(TF, G * NG, NG) * 32)
 spmm_ring_tm_kernel(const SpmmArgs a, const RingArgs ra, const __grid_constant__ CUtensorMap tm0,
                     const __grid_constant__ CUtensorMap tm1, const __grid_constant__ CUtensorMap tm_odd)
 {
+    // the map pointers feed the warp-level copies: uniform values, computed once
     const bool odd = epoch_odd(a.epoch);
-    ring_body<TF, G, NG, 2, HALO>(a, ra, (!HALO && odd) ? &tm_odd : &tm0, (HALO && odd) ? &tm_odd : &tm1);
+    const CUtensorMap* m0 = reinterpret_cast<const CUtensorMap*>(warp_uniform64((unsigned long long)((!HALO && odd) ? &tm_odd : &tm0)));
+    const CUtensorMap* m1 = reinterpret_cast<const CUtensorMap*>(warp_uniform64((unsigned long long)((HALO && odd) ? &tm_odd : &tm1)));
+    ring_body<TF, G, NG, 2, HALO>(a, ra, m0, m1);
 }
 
 }  // namespace pgcn

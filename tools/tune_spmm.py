@@ -6,6 +6,7 @@
     python tools/tune_spmm.py --config C2 --single edges_per_block=256,tile_floats=0 --iters 5   (for ncu)
     python tools/tune_spmm.py --gather-sweep        (L2 capacity / bandwidth probe with windowed columns)
     python tools/tune_spmm.py --gather-sweep --mixed   (0-40 % of the columns from a 512 MB window, the rest from 16 MB)
+    python tools/tune_spmm.py --gather-sweep --all-hit --iters 20   (the ring's own cost per copy; see the option's help)
     python tools/tune_spmm.py --config C2 --sweep slices   (ring row tile: full width vs 64-float slices)
 """
 import argparse
@@ -44,6 +45,8 @@ def main():
     ap.add_argument("--baselines", action="store_true")
     ap.add_argument("--gather-sweep", action="store_true")
     ap.add_argument("--mixed", action="store_true", help="with --gather-sweep: mix a 512 MB and a 16 MB window of columns")
+    ap.add_argument("--all-hit", action="store_true", help="with --gather-sweep: only the 16 MB window, full width and 64-float "
+                    "slices at 16 and 32 slots")
     ap.add_argument("--transpose", action="store_true")
     ap.add_argument("--cache", default="/tmp/pgcn_b200_cache")
     ap.add_argument("--out", default="")
@@ -89,6 +92,29 @@ def main():
                 emit({"probe": "gather-mixed", "wide_frac": frac, "ring_tile_floats": tile, "ring_slots": slots, "ms": med,
                       "gather_GBs": p.lp.nnz() * f * 4 / med / 1e6})
             p.close()
+        return
+
+    if args.gather_sweep and args.all_hit:
+        # every gathered row hits L2 (16 MB window), so the time is what the ring itself pays per copied byte. Run it
+        # on the probe builds as well (PGCN_B200_VARIANT=<name> PGCN_B200_DEFS=-DPGCN_RING_DIAG=1 / 2 / 3: no slot
+        # reads or FFMA / no row copies or waits / neither) to split copy rate, shared-memory reads and bookkeeping.
+        n, d, f, W = 1_000_000, 16, 128, 32_000
+        rng = np.random.default_rng(0)
+        col = rng.integers(0, W, size=n * d, dtype=np.int64)
+        row = np.repeat(np.arange(n, dtype=np.int64), d)
+        A = sp.coo_matrix((np.ones(n * d, dtype=np.float32), (row, col)), shape=(n, n))
+        p = planmod.build_plan(A, np.zeros(n, dtype=np.int64), 0, 1, f, device=dev)
+        H = torch.rand((n, f), device=dev); Z = torch.empty((n, f), device=dev)
+        nnz = p.lp.nnz()
+        for tile, slots in itertools.product((128, 64), (16, 32)):
+            p.set_option("ring_tile_floats", tile)
+            p.set_option("ring_slots", slots)
+            med, mn = timed(lambda: cabi.check(lib.pgcn_spmm(p.handle, 0, H.data_ptr(), None, Z.data_ptr(), None, f, stream), p.handle),
+                            args.iters, warm=20)
+            emit({"probe": "gather-all-hit", "lib": os.path.basename(cabi.lib_path()), "window_MB": W * f * 4 / 1e6,
+                  "ring_tile_floats": tile, "ring_slots": slots, "ms": med, "gather_GBs": nnz * f * 4 / med / 1e6,
+                  "copies_per_us": nnz * (f // tile) / med / 1e3})
+        p.close()
         return
 
     if args.gather_sweep:
