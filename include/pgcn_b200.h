@@ -337,6 +337,29 @@ int pgcn_backward_heads(pgcn_plan* plan, int32_t heads, const float* alpha, cons
 int pgcn_sddmm_heads(pgcn_plan* plan, int32_t heads, const float* gZ, const float* H_own, const float* H_halo,
                      float* dalpha, int32_t f, void* stream);
 
+/* ---- max aggregation: the element-wise maximum over each row's neighbours (GraphSAGE "pool", PyG aggr="max") ------- */
+/*
+ * For every owned row i and feature c, with X = [H_own ; H_halo]:
+ *   Z[i, c] = X[col(e*), c],  arg[i, c] = e*
+ * e* is the FIRST stored entry of row i in forward CSR order whose value is >= every other entry's, NaN counting as
+ * larger than any number (numpy.argmax over the row's entries); Z is copied from the winner bit for bit (its sign of
+ * zero, its NaN payload). arg indexes the colidx / vals arrays given to pgcn_plan_create (colidx[arg] is the local
+ * column). Rows without an entry give Z = 0 and arg = -1. The values of A are not read, only its pattern: of duplicated
+ * (row, column) entries the first copy wins. A max is exact, so Z does not depend on the block size, width, alignment or
+ * long-row split. On several ranks Z is the same on every partition; where values tie, the winner follows the local
+ * column order [own | halo by peer], so arg may name another (equal-valued) global column than on one rank.
+ * Z and gZ are m x f fp32, arg is m x f int32, all row-major with row stride f.
+ * pgcn_forward_max: the exchange of pgcn_forward without its per-source overlap (both transports), then one launch of
+ *   the max kernel over [H_own | halo rows]. The device epoch advances as in every fused call.
+ * pgcn_backward_max: G_own[j, c] = sum of gZ[i, c] over every row i, on every rank, whose arg[i, c] is an entry of
+ *   column j: one launch over the transposed records, then the exchange of pgcn_backward without its per-peer
+ *   pipelining, the halo partials summed at their owners in a fixed order. Run-to-run identical, like the forward.
+ * Both need pgcn_plan_bind_values (PGCN_ERR_STATE before). f outside [1, f_max] and null arguments return
+ * PGCN_ERR_INVALID. After pgcn_plan_prepare(plan, f) they are capturable.
+ */
+int pgcn_forward_max(pgcn_plan* plan, const float* H_own, float* Z, int32_t* arg, int32_t f, void* stream);
+int pgcn_backward_max(pgcn_plan* plan, const int32_t* arg, const float* gZ, float* G_own, int32_t f, void* stream);
+
 /* ---- host-buffer variant: what a non-torch host (the reference's C path) would bind -------- */
 /*
  * Same as pgcn_forward but H and Z are HOST pointers (pinned or pageable): copies H to the

@@ -10,6 +10,7 @@
 #include "spmm_ring.cuh"
 #include "sddmm.cuh"
 #include "attention.cuh"
+#include "spmm_max.cuh"
 
 #include <dlfcn.h>
 #include <unistd.h>
@@ -101,6 +102,8 @@ struct DevCsr {
         int nlong = 0;
         int nslots = 0;
         float* d_partial = nullptr;
+        int* d_apart = nullptr;     // entries of the max aggregation's split-row partials (forward register schedule,
+                                    // bound plans only: allocated by the first max call or pgcn_plan_prepare)
         int64_t epb = -1, long_row = -1;
     } sched[2];
 };
@@ -323,7 +326,7 @@ void csr_free(DevCsr& c)
 {
     if (!c.view) { cudaFree(c.d_cw); cudaFree(c.d_rowids); cudaFree(c.d_empty); cudaFree(c.d_vmap); }
     cudaFree(c.d_final);
-    for (auto& sc : c.sched) { cudaFree(sc.d_blocks); cudaFree(sc.d_long); cudaFree(sc.d_partial); }
+    for (auto& sc : c.sched) { cudaFree(sc.d_blocks); cudaFree(sc.d_long); cudaFree(sc.d_partial); cudaFree(sc.d_apart); }
     c = DevCsr();
 }
 
@@ -386,12 +389,12 @@ int build_schedule(pgcn_plan* p, DevCsr& c, int which, int64_t epb, int64_t long
 
     if (p->prepared && sc.epb >= 0) {
         // a graph captured after pgcn_plan_prepare may still launch the old schedule: keep it until pgcn_plan_destroy
-        p->retired.insert(p->retired.end(), {(void*)sc.d_blocks, (void*)sc.d_long, (void*)sc.d_partial});
+        p->retired.insert(p->retired.end(), {(void*)sc.d_blocks, (void*)sc.d_long, (void*)sc.d_partial, (void*)sc.d_apart});
         ++p->nretired;
     } else {
-        cudaFree(sc.d_blocks); cudaFree(sc.d_long); cudaFree(sc.d_partial);
+        cudaFree(sc.d_blocks); cudaFree(sc.d_long); cudaFree(sc.d_partial); cudaFree(sc.d_apart);
     }
-    sc.d_blocks = nullptr; sc.d_long = nullptr; sc.d_partial = nullptr;
+    sc.d_blocks = nullptr; sc.d_long = nullptr; sc.d_partial = nullptr; sc.d_apart = nullptr;
     int rc;
     if ((rc = upload(p, &sc.d_blocks, blocks.data(), blocks.size()))) return rc;
     if ((rc = upload(p, &sc.d_long, longs.data(), longs.size()))) return rc;
@@ -494,6 +497,40 @@ TileCfg choose_tile_heads(int f, int vw)
     t.tiles = (nvec + t.lpe - 1) / t.lpe;
     return t;
 }
+
+// Max aggregation instances (spmm_max.cuh): one vector per lane, the launch shape of the multi-head instances.
+typedef void (*spmm_max_fn)(const SpmmArgs, int*, int*);
+typedef void (*spmm_max_bwd_fn)(const SpmmArgs, const int*, const int*);
+
+template <int VW, bool HALO>
+spmm_max_fn pick_max_lpe(int lpe)
+{
+    switch (lpe) {
+        case 4: return spmm_max_kernel<4, VW, HALO>;
+        case 8: return spmm_max_kernel<8, VW, HALO>;
+        case 16: return spmm_max_kernel<16, VW, HALO>;
+        default: return spmm_max_kernel<32, VW, HALO>;
+    }
+}
+
+spmm_max_fn pick_max(int lpe, int vw, bool halo)
+{
+    if (vw == 4) return halo ? pick_max_lpe<4, true>(lpe) : pick_max_lpe<4, false>(lpe);
+    return halo ? pick_max_lpe<1, true>(lpe) : pick_max_lpe<1, false>(lpe);
+}
+
+template <int VW>
+spmm_max_bwd_fn pick_max_bwd_lpe(int lpe)
+{
+    switch (lpe) {
+        case 4: return spmm_max_backward_kernel<4, VW>;
+        case 8: return spmm_max_backward_kernel<8, VW>;
+        case 16: return spmm_max_backward_kernel<16, VW>;
+        default: return spmm_max_backward_kernel<32, VW>;
+    }
+}
+
+spmm_max_bwd_fn pick_max_bwd(int lpe, int vw) { return vw == 4 ? pick_max_bwd_lpe<4>(lpe) : pick_max_bwd_lpe<1>(lpe); }
 
 typedef void (*ring_fn)(const SpmmArgs, const RingArgs);
 typedef void (*ring_tm_fn)(const SpmmArgs, const RingArgs, const CUtensorMap, const CUtensorMap, const CUtensorMap);
@@ -646,6 +683,12 @@ void preload_kernels()
     for (int nv = 1; nv <= 4; nv *= 2)
         for (int nh = 2; nh <= 8; nh *= 2) touch_kernel(pick_sddmm_heads(nv, nh));
     touch_kernel(sddmm_plain_heads_kernel);
+    for (int lpe = 4; lpe <= 32; lpe *= 2)
+        for (int vw = 1; vw <= 4; vw += 3) {
+            touch_kernel(pick_max(lpe, vw, false)); touch_kernel(pick_max(lpe, vw, true)); touch_kernel(pick_max_bwd(lpe, vw));
+        }
+    touch_kernel(spmm_max_fixup_kernel<4>); touch_kernel(spmm_max_fixup_kernel<1>);
+    touch_kernel(max_empty_rows_kernel<4>); touch_kernel(max_empty_rows_kernel<1>);
 }
 
 bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
@@ -880,6 +923,121 @@ int launch_unpack(pgcn_plan* p, const float* recv, float* G, int f, cudaStream_t
     if (vw == 4) unpack_add_kernel<4><<<grid, 256, 0, st>>>(a);
     else unpack_add_kernel<1><<<grid, 256, 0, st>>>(a);
     ++p->launches;
+    CU(p, cudaGetLastError());
+    return 0;
+}
+
+// ---- max aggregation -------------------------------------------------------------------------
+
+// The entries of the (value, entry) partials of a schedule's split rows: allocated once per schedule, the first time a
+// max call or pgcn_plan_prepare of a bound plan needs them (never under capture), and retired with the schedule.
+int max_partial(pgcn_plan* p, DevCsr::Sched& sc, cudaStream_t st)
+{
+    if (sc.nslots == 0 || sc.d_apart) return 0;
+    int rc = refuse_under_capture(p, st);
+    if (rc) return rc;
+    CU(p, cudaMalloc((void**)&sc.d_apart, (size_t)sc.nslots * p->f_max * sizeof(int)));
+    return 0;
+}
+
+// Z, arg = the max over each forward row's entries of [H0 | H1] (H1: the halo slab, H_odd its odd-epoch twin or null),
+// on the register schedule of the forward records.
+int launch_max(pgcn_plan* p, const float* H0, const float* H1, const float* H_odd, float* Z, int* arg, int f,
+               cudaStream_t st)
+{
+    DevCsr& c = p->fwd;
+    if (c.nrows == 0) return 0;
+    int64_t epb, long_row;
+    sched_params(p, c, false, &epb, &long_row);
+    int rc;
+    if (!sched_ready(c, 0, epb, long_row) && (rc = refuse_under_capture(p, st))) return rc;
+    if ((rc = build_schedule(p, c, 0, epb, long_row))) return rc;
+    DevCsr::Sched& sc = c.sched[0];
+    if ((rc = max_partial(p, sc, st))) return rc;
+    const int vw = vec_width(f, {H0, H1, H_odd, Z, arg});
+    const TileCfg t = choose_tile_heads(f, vw);
+    if (c.nempty > 0) {
+        MaxEmptyArgs za;
+        za.rows = c.d_empty; za.nrows_empty = c.nempty; za.Z = Z; za.arg = arg; za.f = f;
+        const unsigned grid = (unsigned)(((long long)c.nempty * (f / vw) + 255) / 256);
+        if (vw == 4) max_empty_rows_kernel<4><<<grid, 256, 0, st>>>(za);
+        else max_empty_rows_kernel<1><<<grid, 256, 0, st>>>(za);
+        ++p->launches;
+    }
+    if (sc.nblocks > 0) {
+        SpmmArgs a;
+        a.blocks = sc.d_blocks; a.nblocks = sc.nblocks;
+        a.pieces = c.d_cw;
+        a.H0 = H0; a.H1 = H1; a.split = p->m;
+        a.Z0 = Z; a.Z1 = nullptr; a.zsplit = p->m;
+        a.rowids = c.d_rowids;
+        a.partial = sc.d_partial; a.f = f; a.beta = 0;
+        a.relu = 0; a.final = nullptr;
+        a.H_odd = H_odd; a.epoch = H_odd ? p->d_epoch : nullptr;
+        const int groups_per_cta = kSpmmThreads / t.lpe;
+        dim3 grid((unsigned)((sc.nblocks + groups_per_cta - 1) / groups_per_cta), (unsigned)t.tiles);
+        pick_max(t.lpe, vw, H1 != nullptr)<<<grid, kSpmmThreads, 0, st>>>(a, arg, sc.d_apart);
+        ++p->launches;
+    }
+    if (sc.nlong > 0) {
+        MaxFixupArgs fa;
+        fa.long_rows = sc.d_long; fa.partial = sc.d_partial; fa.apart = sc.d_apart;
+        fa.Z = Z; fa.arg = arg; fa.rowids = c.d_rowids; fa.f = f;
+        const unsigned grid = (unsigned)sc.nlong * (unsigned)((f / vw + 31) / 32);
+        if (vw == 4) spmm_max_fixup_kernel<4><<<grid, 32 * kFixupGroups, 0, st>>>(fa);
+        else spmm_max_fixup_kernel<1><<<grid, 32 * kFixupGroups, 0, st>>>(fa);
+        ++p->launches;
+    }
+    CU(p, cudaGetLastError());
+    return 0;
+}
+
+// G_own (rows [0, m)) and G_halo (rows [m, m + h)) = gZ routed by arg, on the register schedule of the transposed records.
+int launch_max_backward(pgcn_plan* p, const int* arg, const float* gZ, float* G_own, float* G_halo, int f, cudaStream_t st)
+{
+    DevCsr& c = p->tr;
+    if (c.nrows == 0) return 0;
+    int64_t epb, long_row;
+    sched_params(p, c, false, &epb, &long_row);
+    int rc;
+    if (!sched_ready(c, 0, epb, long_row) && (rc = refuse_under_capture(p, st))) return rc;
+    if ((rc = build_schedule(p, c, 0, epb, long_row))) return rc;
+    const DevCsr::Sched& sc = c.sched[0];
+    const int vw = vec_width(f, {gZ, arg, G_own, G_halo});
+    const TileCfg t = choose_tile_heads(f, vw);
+    if (c.nempty > 0) {
+        ZeroArgs za;
+        za.rows = c.d_empty; za.nrows_empty = c.nempty; za.Z0 = G_own; za.Z1 = G_halo; za.zsplit = p->m; za.f = f;
+        const unsigned grid = (unsigned)(((long long)c.nempty * (f / vw) + 255) / 256);
+        if (vw == 4) zero_rows_kernel<4><<<grid, 256, 0, st>>>(za);
+        else zero_rows_kernel<1><<<grid, 256, 0, st>>>(za);
+        ++p->launches;
+    }
+    if (sc.nblocks > 0) {
+        SpmmArgs a;
+        a.blocks = sc.d_blocks; a.nblocks = sc.nblocks;
+        a.pieces = c.d_cw;
+        a.H0 = gZ; a.H1 = nullptr; a.split = p->m;
+        a.Z0 = G_own; a.Z1 = G_halo; a.zsplit = p->m;
+        a.rowids = c.d_rowids;
+        a.partial = sc.d_partial; a.f = f; a.beta = 0;
+        a.relu = 0; a.final = nullptr;
+        a.H_odd = nullptr; a.epoch = nullptr;
+        const int groups_per_cta = kSpmmThreads / t.lpe;
+        dim3 grid((unsigned)((sc.nblocks + groups_per_cta - 1) / groups_per_cta), (unsigned)t.tiles);
+        pick_max_bwd(t.lpe, vw)<<<grid, kSpmmThreads, 0, st>>>(a, arg, c.d_vmap);
+        ++p->launches;
+    }
+    if (sc.nlong > 0) {
+        FixupArgs fa;
+        fa.long_rows = sc.d_long; fa.nlong = sc.nlong; fa.partial = sc.d_partial;
+        fa.Z0 = G_own; fa.Z1 = G_halo; fa.zsplit = p->m; fa.rowids = c.d_rowids; fa.f = f; fa.beta = 0;
+        fa.relu = 0; fa.final = nullptr;
+        const unsigned grid = (unsigned)sc.nlong * (unsigned)((f / vw + 31) / 32);
+        if (vw == 4) spmm_fixup_kernel<4><<<grid, 32 * kFixupGroups, 0, st>>>(fa);
+        else spmm_fixup_kernel<1><<<grid, 32 * kFixupGroups, 0, st>>>(fa);
+        ++p->launches;
+    }
     CU(p, cudaGetLastError());
     return 0;
 }
@@ -1623,6 +1781,8 @@ int pgcn_plan_prepare(pgcn_plan* p, int32_t f)
     if (ring && (f == 128 || f == 256 || f == 512))
         for (int k = 2; k <= 8; k *= 2)
             if ((f / k) % 4 == 0 && (rc = sddmm_heads_attr(p, f, k, p->host_stream))) return rc;
+    // the max calls of a bound plan: the register schedules (built above) and the entries of the forward's split rows
+    if (p->bound && (rc = max_partial(p, p->fwd.sched[0], p->host_stream))) return rc;
     p->prepared = true;
     return 0;
 }
@@ -2228,51 +2388,35 @@ int pgcn_edge_softmax_backward_heads(pgcn_plan* p, int32_t heads, const float* e
                        attn_vec(heads, {el, er_own, a.er_halo, alpha, dalpha, dpre, d_el}));
 }
 
-// The unsplit forward exchange of pgcn_forward (both transports), then one multi-head launch over [H_own | halo slab of
-// the call's parity], then the halo copy. The plan's resident values are not read.
-int pgcn_forward_heads(pgcn_plan* p, int32_t heads, const float* alpha, const float* H_own, float* Z, float* H_halo_out,
-                       int32_t f, void* stream)
+extern "C++" {
+
+// The unsplit forward exchange of the multi-head and max calls (pgcn_forward without its per-source overlap, both
+// transports): every source's rows have landed before launch(halo, halo_odd) runs on `st`. halo is the slab the rows
+// land in, halo_odd its odd-epoch twin on the peer transport (else null); on one rank there is no exchange.
+template <class Launch>
+static int unsplit_forward(pgcn_plan* p, const float* H_own, int f, cudaStream_t st, Launch launch)
 {
-    int rc = heads_check_f(p, "pgcn_forward_heads", heads, f);
-    if (rc) return rc;
-    if (p->m > 0 && (!H_own || !Z)) return fail(p, PGCN_ERR_INVALID, "null H_own/Z");
-    if (p->fwd.nnz > 0 && !alpha) return fail(p, PGCN_ERR_INVALID, "null alpha");
-    cudaStream_t st = (cudaStream_t)stream;
-    const HeadArgs ha = {alpha, nullptr, heads};
-    if (p->k == 1)
-        return launch_spmm(p, p->fwd, H_own, p->h > 0 ? p->d_halo_slab : nullptr, p->m, Z, nullptr, p->m, f, 0, st, 0,
-                           false, nullptr, &ha);
+    if (p->k == 1) return launch(p->d_halo_slab, (const float*)nullptr);
     const bool use_p2p = p->p2p && (f % 4 == 0);
     if (!use_p2p && !p->comm) return fail(p, PGCN_ERR_STATE, "k=%d: call pgcn_comm_init or pgcn_p2p_import first", p->k);
     float* halo = use_p2p ? arena_ptr(p->arena, p->off_fwd[0]) : p->d_halo_slab;
     const float* halo_odd = use_p2p ? arena_ptr(p->arena, p->off_fwd[1]) : nullptr;
+    int rc;
     if ((rc = forward_send(p, H_own, f, use_p2p, false, st))) return rc;
     if ((rc = forward_wait_all(p, use_p2p, st))) return rc;
-    if ((rc = launch_spmm(p, p->fwd, H_own, p->h > 0 ? halo : nullptr, p->m, Z, nullptr, p->m, f, 0, st, 0, false,
-                          p->h > 0 ? halo_odd : nullptr, &ha)))
-        return rc;
-    if (!H_halo_out || p->h == 0) return 0;
-    const long long n = (long long)p->h * f;
-    copy_halo_kernel<<<grid_for(n, p->num_sms), 256, 0, st>>>(halo, halo_odd, use_p2p ? p->d_epoch : nullptr, H_halo_out, n);
-    ++p->launches;
-    CU(p, cudaGetLastError());
-    return 0;
+    return launch(halo, halo_odd);
 }
 
-// The unsplit backward of pgcn_backward with multi-head weights on the transposed records (through their value map).
-int pgcn_backward_heads(pgcn_plan* p, int32_t heads, const float* alpha, const float* gZ, float* G_own, int32_t f,
-                        void* stream)
+// The unsplit backward exchange of the multi-head and max calls (pgcn_backward without its per-peer pipelining):
+// launch() writes the rows of A^T gZ, [0, m) into G_own and the halo partials into the reverse send slab; they go back
+// to their owners and every rank adds what it receives into G_own in a fixed order.
+template <class Launch>
+static int unsplit_backward(pgcn_plan* p, float* G_own, int f, cudaStream_t st, Launch launch)
 {
-    int rc = heads_check_f(p, "pgcn_backward_heads", heads, f);
-    if (rc) return rc;
-    if (p->m > 0 && (!gZ || !G_own)) return fail(p, PGCN_ERR_INVALID, "null gZ/G_own");
-    if (p->fwd.nnz > 0 && !alpha) return fail(p, PGCN_ERR_INVALID, "null alpha");
-    cudaStream_t st = (cudaStream_t)stream;
-    const HeadArgs ha = {alpha, p->tr.d_vmap, heads};
-    if (p->k == 1)
-        return launch_spmm(p, p->tr, gZ, nullptr, p->m, G_own, p->d_hsend_slab, p->m, f, 0, st, 0, false, nullptr, &ha);
+    if (p->k == 1) return launch();
     const bool use_p2p = p->p2p && (f % 4 == 0);
     if (!use_p2p && !p->comm) return fail(p, PGCN_ERR_STATE, "k=%d: call pgcn_comm_init or pgcn_p2p_import first", p->k);
+    int rc;
     float* rrecv = p->d_rrecv_slab;
     const float* rrecv_odd = nullptr;
     if (use_p2p) {
@@ -2280,8 +2424,7 @@ int pgcn_backward_heads(pgcn_plan* p, int32_t heads, const float* alpha, const f
         rrecv = arena_ptr(p->arena, p->off_bwd[0]);
         rrecv_odd = arena_ptr(p->arena, p->off_bwd[1]);
     }
-    if ((rc = launch_spmm(p, p->tr, gZ, nullptr, p->m, G_own, p->d_hsend_slab, p->m, f, 0, st, 0, false, nullptr, &ha)))
-        return rc;
+    if ((rc = launch())) return rc;
     for (int i = 1; i < p->k; ++i) {
         if (use_p2p) { if ((rc = p2p_put(p, step_dst(p, i), p->d_hsend_slab, f, true, st))) return rc; }
         else if ((rc = nccl_step(p, p->d_hsend_slab, rrecv, f, 1, i, st))) return rc;
@@ -2292,6 +2435,47 @@ int pgcn_backward_heads(pgcn_plan* p, int32_t heads, const float* alpha, const f
     return launch_unpack(p, rrecv, G_own, f, st, rrecv_odd);
 }
 
+}  // extern "C++"
+
+// The unsplit forward exchange, then one multi-head launch over [H_own | halo slab of the call's parity], then the halo
+// copy. The plan's resident values are not read.
+int pgcn_forward_heads(pgcn_plan* p, int32_t heads, const float* alpha, const float* H_own, float* Z, float* H_halo_out,
+                       int32_t f, void* stream)
+{
+    int rc = heads_check_f(p, "pgcn_forward_heads", heads, f);
+    if (rc) return rc;
+    if (p->m > 0 && (!H_own || !Z)) return fail(p, PGCN_ERR_INVALID, "null H_own/Z");
+    if (p->fwd.nnz > 0 && !alpha) return fail(p, PGCN_ERR_INVALID, "null alpha");
+    cudaStream_t st = (cudaStream_t)stream;
+    const HeadArgs ha = {alpha, nullptr, heads};
+    return unsplit_forward(p, H_own, f, st, [&](float* halo, const float* halo_odd) -> int {
+        int rc2 = launch_spmm(p, p->fwd, H_own, p->h > 0 ? halo : nullptr, p->m, Z, nullptr, p->m, f, 0, st, 0, false,
+                              p->h > 0 ? halo_odd : nullptr, &ha);
+        if (rc2 || p->k == 1 || !H_halo_out || p->h == 0) return rc2;
+        const long long n = (long long)p->h * f;
+        copy_halo_kernel<<<grid_for(n, p->num_sms), 256, 0, st>>>(halo, halo_odd, halo_odd ? p->d_epoch : nullptr,
+                                                                  H_halo_out, n);
+        ++p->launches;
+        CU(p, cudaGetLastError());
+        return 0;
+    });
+}
+
+// The unsplit backward with multi-head weights on the transposed records (through their value map).
+int pgcn_backward_heads(pgcn_plan* p, int32_t heads, const float* alpha, const float* gZ, float* G_own, int32_t f,
+                        void* stream)
+{
+    int rc = heads_check_f(p, "pgcn_backward_heads", heads, f);
+    if (rc) return rc;
+    if (p->m > 0 && (!gZ || !G_own)) return fail(p, PGCN_ERR_INVALID, "null gZ/G_own");
+    if (p->fwd.nnz > 0 && !alpha) return fail(p, PGCN_ERR_INVALID, "null alpha");
+    cudaStream_t st = (cudaStream_t)stream;
+    const HeadArgs ha = {alpha, p->tr.d_vmap, heads};
+    return unsplit_backward(p, G_own, f, st, [&]() {
+        return launch_spmm(p, p->tr, gZ, nullptr, p->m, G_own, p->d_hsend_slab, p->m, f, 0, st, 0, false, nullptr, &ha);
+    });
+}
+
 int pgcn_sddmm_heads(pgcn_plan* p, int32_t heads, const float* gZ, const float* H_own, const float* H_halo,
                      float* dalpha, int32_t f, void* stream)
 {
@@ -2300,6 +2484,39 @@ int pgcn_sddmm_heads(pgcn_plan* p, int32_t heads, const float* gZ, const float* 
     if (p->fwd.nnz > 0 && (!gZ || !H_own || !dalpha)) return fail(p, PGCN_ERR_INVALID, "null gZ/H_own/dalpha");
     if (p->h > 0 && !H_halo) return fail(p, PGCN_ERR_INVALID, "h=%d but H_halo is null", p->h);
     return launch_sddmm_heads(p, heads, gZ, H_own, p->h > 0 ? H_halo : nullptr, dalpha, f, (cudaStream_t)stream);
+}
+
+// ---- max aggregation ------------------------------------------------------------------------------------------------
+
+static int max_check(pgcn_plan* p, const char* what, int f)
+{
+    if (!p) return fail(nullptr, PGCN_ERR_INVALID, "null plan");
+    if (!p->bound) return fail(p, PGCN_ERR_STATE, "%s reads the value maps: call pgcn_plan_bind_values first", what);
+    return check_f(p, f);
+}
+
+// The unsplit forward exchange, then one max launch over [H_own | halo slab of the call's parity].
+int pgcn_forward_max(pgcn_plan* p, const float* H_own, float* Z, int32_t* arg, int32_t f, void* stream)
+{
+    int rc = max_check(p, "pgcn_forward_max", f);
+    if (rc) return rc;
+    if (p->m > 0 && (!H_own || !Z || !arg)) return fail(p, PGCN_ERR_INVALID, "pgcn_forward_max: null H_own/Z/arg");
+    cudaStream_t st = (cudaStream_t)stream;
+    return unsplit_forward(p, H_own, f, st, [&](float* halo, const float* halo_odd) {
+        return launch_max(p, H_own, p->h > 0 ? halo : nullptr, p->h > 0 ? halo_odd : nullptr, Z, arg, f, st);
+    });
+}
+
+// The transposed max launch (gZ routed by arg through the value map), then the unsplit backward exchange.
+int pgcn_backward_max(pgcn_plan* p, const int32_t* arg, const float* gZ, float* G_own, int32_t f, void* stream)
+{
+    int rc = max_check(p, "pgcn_backward_max", f);
+    if (rc) return rc;
+    if (p->m > 0 && (!arg || !gZ || !G_own)) return fail(p, PGCN_ERR_INVALID, "pgcn_backward_max: null arg/gZ/G_own");
+    cudaStream_t st = (cudaStream_t)stream;
+    return unsplit_backward(p, G_own, f, st, [&]() {
+        return launch_max_backward(p, arg, gZ, G_own, p->d_hsend_slab, f, st);
+    });
 }
 
 static int host_slots(pgcn_plan* p, int64_t need)

@@ -442,6 +442,78 @@ class PGATMultiHeadAttention(torch.autograd.Function):
         return None, dZ, d_el, d_er, None
 
 
+# ---- max aggregation -------------------------------------------------------------------------------------------------
+
+def _check_max_plan(plan, what):
+    if not plan._bound:
+        raise RuntimeError("%s walks the transposed records through the plan's value maps: call PgcnPlan.bind_values() "
+                           "once (set-up, before any CUDA-graph capture)" % what)
+
+
+def aggregate_max(plan, H_own):
+    """(Z_own, arg): the element-wise maximum over each owned row's stored entries of [H_own ; H_halo] (pgcn_forward_max).
+    Z_own is [m, f] fp32, arg [m, f] int32: the winning entry, the first in forward CSR order (lp.colidx's order) with
+    the largest value, NaN above every number; lp.colidx[arg] is its local column. Rows without an entry give 0 / -1."""
+    H_own = _check_feat(plan, H_own, plan.m, "H")
+    _check_max_plan(plan, "aggregate_max")
+    f = H_own.shape[1]
+    Z = torch.empty((plan.m, f), dtype=torch.float32, device=H_own.device)
+    arg = torch.empty((plan.m, f), dtype=torch.int32, device=H_own.device)
+    with torch.cuda.device(H_own.device):
+        cabi.check(cabi.load().pgcn_forward_max(plan.handle, H_own.data_ptr(), Z.data_ptr(), arg.data_ptr(), f,
+                                                _stream_ptr()), plan.handle)
+    if plan.lp.k > 1:
+        plan.count_exchange(backward=False)
+    return Z, arg
+
+
+def aggregate_max_backward(plan, arg, gZ_own):
+    """G_own [m, f]: gZ routed to the winning entries named by `arg` (aggregate_max's), summed per column on its owner
+    (pgcn_backward_max)."""
+    gZ_own = _check_feat(plan, gZ_own, plan.m, "grad_output")
+    _check_max_plan(plan, "aggregate_max_backward")
+    f = gZ_own.shape[1]
+    if arg.dtype != torch.int32 or arg.device != gZ_own.device or tuple(arg.shape) != (plan.m, f):
+        raise ValueError("arg must be int32 [%d, %d] on %s, got %s %s on %s"
+                         % (plan.m, f, gZ_own.device, arg.dtype, tuple(arg.shape), arg.device))
+    arg = arg.contiguous()
+    G = torch.empty((plan.m, f), dtype=torch.float32, device=gZ_own.device)
+    with torch.cuda.device(gZ_own.device):
+        cabi.check(cabi.load().pgcn_backward_max(plan.handle, arg.data_ptr(), gZ_own.data_ptr(), G.data_ptr(), f,
+                                                 _stream_ptr()), plan.handle)
+    if plan.lp.k > 1:
+        plan.count_exchange(backward=True)
+    return G
+
+
+class PSpMMMax(torch.autograd.Function):
+    """Z = max over each row's neighbours, element-wise (the GraphSAGE "pool" aggregator, PyG aggr="max"), with the call
+    shape of PSpMM: PSpMMMax.apply(A, H). The pattern of A is used, not its values. The gradient goes to the winning
+    entry of every (row, feature), the first one on ties (aggregate_max), including winners in other ranks' rows.
+    Layouts as PSpMM. The plan must be bound (PgcnPlan.bind_values)."""
+
+    @staticmethod
+    def forward(ctx, A, H):
+        ctx.plan = A
+        _check_max_plan(A, "PSpMMMax")
+        if A.layout == "global":
+            _check_feat(A, H, A.n, "H")
+            Z_own, arg = aggregate_max(A, H.index_select(0, A.owned_index()))
+        else:
+            Z_own, arg = aggregate_max(A, H)
+        ctx.save_for_backward(arg)
+        return _to_layout(A, Z_own, A.n)
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        A = ctx.plan
+        (arg,) = ctx.saved_tensors
+        if A.layout == "global":
+            g = _check_feat(A, grad_output, A.n, "grad_output").index_select(0, A.owned_index())
+            return None, _to_layout(A, aggregate_max_backward(A, arg, g), A.n)
+        return None, aggregate_max_backward(A, arg, grad_output)
+
+
 # ---- the pieces, individually callable (NCCL transport), mirroring communicate_fgm ----------------
 
 def spmm_local(plan, H_own, H_halo=None, transpose=False):
