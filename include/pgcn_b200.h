@@ -360,6 +360,40 @@ int pgcn_sddmm_heads(pgcn_plan* plan, int32_t heads, const float* gZ, const floa
 int pgcn_forward_max(pgcn_plan* plan, const float* H_own, float* Z, int32_t* arg, int32_t f, void* stream);
 int pgcn_backward_max(pgcn_plan* plan, const int32_t* arg, const float* gZ, float* G_own, int32_t f, void* stream);
 
+/* ---- GATv2 attention: dynamic attention (Brody et al.) over the stored pattern, K = heads in {1, 2, 4, 8} ---------- */
+/*
+ * Inputs: xl (source side, m x f; the halo rows come from their owners), xr (destination side, m x f; only owned rows
+ * are read, so only xl is exchanged), att (K x d, d = f / K, row-major: att[h, c] is float h d + c) and negative_slope.
+ * For every stored entry e = (i, j) of the local matrix (j a local column in [own | halo by peer]) and head h:
+ *   s_eh      = sum_{c < d} att[h, c] * LeakyReLU(xl[j, h d + c] + xr[i, h d + c])
+ *   alpha_.h  = the softmax of s_.h over the stored entries of each row, row maximum subtracted, full-precision expf
+ *   Z[i, h d:(h+1) d] = sum_e alpha_eh xl[j, h d:(h+1) d]                 (heads concatenated)
+ * This is PyG GATv2Conv(share_weights=False, concat=True, bias=False, add_self_loops=False, dropout=0) over the stored
+ * pattern; share_weights=True is xl == xr. Rows without entries give Z = 0 and write no alpha. alpha and work are
+ * nnz x K in forward CSR order (the order pgcn_plan_set_values takes). Every sum is added in a fixed order: two runs
+ * give the same bits, and so do the ring and plain score kernels and the 4-wide and scalar backward kernels.
+ * Backward, with dalpha = pgcn_sddmm_heads(gZ, xl), dscore_eh = alpha_eh (dalpha_eh - sum_row alpha_.h dalpha_.h),
+ * t = xl[j] + xr[i] and g_ec = dscore_e,h(c) * att_c * LeakyReLU'(t_c):
+ *   dxr[i]    = sum_{e in row i} g_e
+ *   dxl[j]    = sum_{e in column j} alpha_e,h(c) gZ[i, c] + g_ec     (halo columns summed at their owners)
+ *   datt[h, c] = sum_e dscore_eh * LeakyReLU(t_c)                    (no atomics: per-chunk partials, fixed order)
+ * pgcn_forward_gatv2: the exchange of xl as in pgcn_forward_heads (once), then the score kernel writes the scores into
+ *   alpha, the edge softmax turns them into alpha in place, the multi-head aggregation writes Z, and with xl_halo_out
+ *   (h x f, may be NULL) the received halo rows of xl are copied out for the backward. The device epoch advances as in
+ *   every fused call.
+ * pgcn_backward_gatv2: work (nnz x K, caller-owned) receives dalpha and then dscore in place; dxr (m x f) and datt (K x d)
+ *   from the forward records; dxl (m x f) from the transposed records, with the exchange of pgcn_backward_heads.
+ *   xl_halo: the rows pgcn_forward_gatv2 returned in xl_halo_out (h x f; unused when h == 0).
+ * Both need pgcn_plan_bind_values (PGCN_ERR_STATE before) and never read or write the plan's resident values. heads
+ * outside {1, 2, 4, 8}, f % heads != 0 and null arguments return PGCN_ERR_INVALID. After pgcn_plan_prepare(plan, f)
+ * both are capturable. The plan keeps f_max floats per 8 row blocks of its forward schedule for the datt partials.
+ */
+int pgcn_forward_gatv2(pgcn_plan* plan, int32_t heads, const float* xl_own, const float* xr, const float* att,
+                       float negative_slope, float* alpha, float* Z, float* xl_halo_out, int32_t f, void* stream);
+int pgcn_backward_gatv2(pgcn_plan* plan, int32_t heads, const float* alpha, const float* gZ, const float* xl_own,
+                        const float* xl_halo, const float* xr, const float* att, float negative_slope, float* work,
+                        float* dxl, float* dxr, float* datt, int32_t f, void* stream);
+
 /* ---- host-buffer variant: what a non-torch host (the reference's C path) would bind -------- */
 /*
  * Same as pgcn_forward but H and Z are HOST pointers (pinned or pageable): copies H to the

@@ -1,6 +1,6 @@
 """Build the native pieces in-tree (so the .so files travel to the GPU box with the snapshot).
 
-  lib/libpgcn_b200.so   csrc/pgcn_b200.cu (+ spmm_kernels.cuh, spmm_ring.cuh, sddmm.cuh, attention.cuh, spmm_max.cuh)   nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo
+  lib/libpgcn_b200.so   csrc/pgcn_b200.cu (+ spmm_kernels.cuh, spmm_ring.cuh, sddmm.cuh, attention.cuh, spmm_max.cuh, gatv2.cuh)   nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo
   (the CPU oracle under oracle/ is built by oracle/build_oracle.py — test infrastructure only)
 
 nvcc cross-compiles without a GPU; `python -m <pkg>.build` or `__graft_entry__.build()` runs this.
@@ -22,6 +22,7 @@ SOURCES = [os.path.join(CSRC, "pgcn_b200.cu")]
 # this file too: a library built with other compiler flags (another GPU architecture) is stale
 DEPS = SOURCES + [os.path.join(CSRC, "spmm_kernels.cuh"), os.path.join(CSRC, "spmm_ring.cuh"),
                   os.path.join(CSRC, "sddmm.cuh"), os.path.join(CSRC, "attention.cuh"), os.path.join(CSRC, "spmm_max.cuh"),
+                  os.path.join(CSRC, "gatv2.cuh"),
                   os.path.join(ROOT, "include", "pgcn_b200.h"), os.path.abspath(__file__)]
 
 NVCC_FLAGS = [

@@ -23,7 +23,7 @@ SYMBOLS = [
     "pgcn_plan_bind_values", "pgcn_plan_set_values", "pgcn_sddmm", "pgcn_forward_keep_halo",
     "pgcn_edge_softmax", "pgcn_edge_softmax_backward", "pgcn_halo_rows",
     "pgcn_edge_softmax_heads", "pgcn_edge_softmax_backward_heads", "pgcn_forward_heads", "pgcn_backward_heads",
-    "pgcn_sddmm_heads", "pgcn_forward_max", "pgcn_backward_max",
+    "pgcn_sddmm_heads", "pgcn_forward_max", "pgcn_backward_max", "pgcn_forward_gatv2", "pgcn_backward_gatv2",
 ]
 
 
@@ -141,6 +141,10 @@ def load(build_if_missing=True):
     lib.pgcn_forward_max.argtypes = [vp, vp, vp, vp, i32, vp]
     lib.pgcn_backward_max.restype = C.c_int
     lib.pgcn_backward_max.argtypes = [vp, vp, vp, vp, i32, vp]
+    lib.pgcn_forward_gatv2.restype = C.c_int
+    lib.pgcn_forward_gatv2.argtypes = [vp, i32, vp, vp, vp, C.c_float, vp, vp, vp, i32, vp]
+    lib.pgcn_backward_gatv2.restype = C.c_int
+    lib.pgcn_backward_gatv2.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, C.c_float, vp, vp, vp, vp, i32, vp]
     _lib = lib
     return lib
 

@@ -14,6 +14,8 @@
 // rows from the device rowptr pgcn_plan_bind_values keeps. K = 1 is the single-head layer.
 //
 //   edge_softmax_kernel<K, VEC>   / edge_softmax_backward_kernel<K, VEC>
+//   edge_softmax_raw_kernel<K, VEC> / edge_softmax_raw_backward_kernel<K, VEC>   the same rows over scores already stored
+//                                 in `out` (GATv2), in place; the backward has no slope factor and no d_el
 // One launch serves every row. Blocks [0, nlong) take one long row each (more than kAttnLongRow entries: the hub rows
 // of R-MAT graphs, which would set the launch time if one warp walked them); every later block gives one warp to each
 // of 8 consecutive rows and skips the long ones. Lanes stride over their row's entries; one gather of a column brings
@@ -128,14 +130,14 @@ __device__ __forceinline__ void sum_row(float (&x)[K], float (&sm)[kAttnWarps][K
 }
 
 // One row, walked by NT threads (t = this thread's index among them). Long rows (NT = a CTA) combine the warps'
-// results through shared memory in warp order.
-template <int NT, int K, bool VEC>
+// results through shared memory in warp order. RAW: `out` already holds the scores (GATv2), el / er are not read.
+template <int NT, int K, bool VEC, bool RAW = false>
 __device__ __forceinline__ void softmax_row(const AttnArgs& a, int i, int t)
 {
     __shared__ float sm_m[kAttnWarps][K], sm_s[kAttnWarps][K];
     const int b = __ldg(a.rowptr + i), end = __ldg(a.rowptr + i + 1);
     float eli[K];
-    ld_heads<K, VEC, true>(eli, a.el + (size_t)i * K);
+    if constexpr (!RAW) ld_heads<K, VEC, true>(eli, a.el + (size_t)i * K);
     float* __restrict__ out = a.out;
     // pass 1: the scores (kept in `out`, read back by this thread) and the row maxima. No exponential here, so the
     // gathers of consecutive entries do not wait for each other.
@@ -145,8 +147,12 @@ __device__ __forceinline__ void softmax_row(const AttnArgs& a, int i, int t)
 #pragma unroll 4
     for (int e = b + t; e < end; e += NT) {
         float x[K];
-        attn_score<K, VEC>(a, eli, e, x);
-        st_heads<K, VEC>(out + (size_t)e * K, x);
+        if constexpr (RAW) {
+            ld_heads<K, VEC, false>(x, out + (size_t)e * K);
+        } else {
+            attn_score<K, VEC>(a, eli, e, x);
+            st_heads<K, VEC>(out + (size_t)e * K, x);
+        }
 #pragma unroll
         for (int h = 0; h < K; ++h) m[h] = fmaxf(m[h], x[h]);
     }
@@ -187,7 +193,9 @@ __device__ __forceinline__ void softmax_row(const AttnArgs& a, int i, int t)
     }
 }
 
-template <int NT, int K, bool VEC>
+// RAW: dscore = alpha (dalpha - c) without the slope factor and d_el, written over dalpha (out == dalpha is allowed:
+// each entry is read and rewritten by one thread, so dalpha takes the coherent path).
+template <int NT, int K, bool VEC, bool RAW = false>
 __device__ __forceinline__ void softmax_backward_row(const AttnArgs& a, int i, int t)
 {
     __shared__ float sm_x[kAttnWarps][K];
@@ -198,11 +206,22 @@ __device__ __forceinline__ void softmax_backward_row(const AttnArgs& a, int i, i
     for (int e = b + t; e < end; e += NT) {
         float al[K], da[K];
         ld_heads<K, VEC, true>(al, a.alpha + (size_t)e * K);
-        ld_heads<K, VEC, true>(da, a.dalpha + (size_t)e * K);
+        ld_heads<K, VEC, !RAW>(da, a.dalpha + (size_t)e * K);
 #pragma unroll
         for (int h = 0; h < K; ++h) c[h] = fmaf(al[h], da[h], c[h]);
     }
     sum_row<NT, K>(c, sm_x, t);
+    if constexpr (RAW) {
+        for (int e = b + t; e < end; e += NT) {
+            float al[K], da[K];
+            ld_heads<K, VEC, true>(al, a.alpha + (size_t)e * K);
+            ld_heads<K, VEC, false>(da, a.dalpha + (size_t)e * K);
+#pragma unroll
+            for (int h = 0; h < K; ++h) da[h] = al[h] * (da[h] - c[h]);
+            st_heads<K, VEC>(a.out + (size_t)e * K, da);
+        }
+        return;
+    }
     if (NT > 32) __syncthreads();                           // sm_x is reused below
     float eli[K];
     ld_heads<K, VEC, true>(eli, a.el + (size_t)i * K);
@@ -250,6 +269,27 @@ edge_softmax_backward_kernel(const AttnArgs a)
     int i;
     if ((int)blockIdx.x < a.nlong) softmax_backward_row<kAttnThreads, K, VEC>(a, __ldg(a.long_rows + blockIdx.x), threadIdx.x);
     else if (attn_short_row(a, i)) softmax_backward_row<32, K, VEC>(a, i, threadIdx.x & 31);
+}
+
+// The edge softmax of stored scores (GATv2: the score kernel wrote them into `out`), in place: the same rows, passes,
+// orders and bits as edge_softmax_kernel once the scores are there.
+template <int K, bool VEC>
+__global__ void __launch_bounds__(kAttnThreads)
+edge_softmax_raw_kernel(const AttnArgs a)
+{
+    int i;
+    if ((int)blockIdx.x < a.nlong) softmax_row<kAttnThreads, K, VEC, true>(a, __ldg(a.long_rows + blockIdx.x), threadIdx.x);
+    else if (attn_short_row(a, i)) softmax_row<32, K, VEC, true>(a, i, threadIdx.x & 31);
+}
+
+// dscore = alpha (dalpha - sum_row alpha dalpha) per head, in place over dalpha (out == dalpha).
+template <int K, bool VEC>
+__global__ void __launch_bounds__(kAttnThreads)
+edge_softmax_raw_backward_kernel(const AttnArgs a)
+{
+    int i;
+    if ((int)blockIdx.x < a.nlong) softmax_backward_row<kAttnThreads, K, VEC, true>(a, __ldg(a.long_rows + blockIdx.x), threadIdx.x);
+    else if (attn_short_row(a, i)) softmax_backward_row<32, K, VEC, true>(a, i, threadIdx.x & 31);
 }
 
 }  // namespace pgcn

@@ -11,6 +11,7 @@
 #include "sddmm.cuh"
 #include "attention.cuh"
 #include "spmm_max.cuh"
+#include "gatv2.cuh"
 
 #include <dlfcn.h>
 #include <unistd.h>
@@ -104,6 +105,8 @@ struct DevCsr {
         float* d_partial = nullptr;
         int* d_apart = nullptr;     // entries of the max aggregation's split-row partials (forward register schedule,
                                     // bound plans only: allocated by the first max call or pgcn_plan_prepare)
+        float* d_datt = nullptr;    // GATv2 datt partials, f_max floats per chunk of kGatv2Chunk row blocks (forward
+                                    // register schedule, bound plans only: first GATv2 backward or pgcn_plan_prepare)
         int64_t epb = -1, long_row = -1;
     } sched[2];
 };
@@ -198,6 +201,8 @@ struct pgcn_plan {
     int sddmm_ctas_per_sm[5] = {0};
     bool sddmm_heads_attr_set[5][9] = {};  // per f / 128 and head count of the multi-head SDDMM ring kernel
     int sddmm_heads_ctas_per_sm[5][9] = {};
+    bool gatv2_attr_set[3][9] = {};        // per f / 128 and head count of the GATv2 score ring kernel
+    int gatv2_ctas_per_sm[3][9] = {};
     int* d_rowptr = nullptr;               // m + 1, the forward rowptr (edge softmax)
     int* d_long_rows = nullptr;            // rows of more than kAttnLongRow entries (one CTA each in the edge softmax)
     int nlong_rows = 0;
@@ -326,7 +331,7 @@ void csr_free(DevCsr& c)
 {
     if (!c.view) { cudaFree(c.d_cw); cudaFree(c.d_rowids); cudaFree(c.d_empty); cudaFree(c.d_vmap); }
     cudaFree(c.d_final);
-    for (auto& sc : c.sched) { cudaFree(sc.d_blocks); cudaFree(sc.d_long); cudaFree(sc.d_partial); cudaFree(sc.d_apart); }
+    for (auto& sc : c.sched) { cudaFree(sc.d_blocks); cudaFree(sc.d_long); cudaFree(sc.d_partial); cudaFree(sc.d_apart); cudaFree(sc.d_datt); }
     c = DevCsr();
 }
 
@@ -389,12 +394,13 @@ int build_schedule(pgcn_plan* p, DevCsr& c, int which, int64_t epb, int64_t long
 
     if (p->prepared && sc.epb >= 0) {
         // a graph captured after pgcn_plan_prepare may still launch the old schedule: keep it until pgcn_plan_destroy
-        p->retired.insert(p->retired.end(), {(void*)sc.d_blocks, (void*)sc.d_long, (void*)sc.d_partial, (void*)sc.d_apart});
+        p->retired.insert(p->retired.end(), {(void*)sc.d_blocks, (void*)sc.d_long, (void*)sc.d_partial, (void*)sc.d_apart,
+                                             (void*)sc.d_datt});
         ++p->nretired;
     } else {
-        cudaFree(sc.d_blocks); cudaFree(sc.d_long); cudaFree(sc.d_partial); cudaFree(sc.d_apart);
+        cudaFree(sc.d_blocks); cudaFree(sc.d_long); cudaFree(sc.d_partial); cudaFree(sc.d_apart); cudaFree(sc.d_datt);
     }
-    sc.d_blocks = nullptr; sc.d_long = nullptr; sc.d_partial = nullptr; sc.d_apart = nullptr;
+    sc.d_blocks = nullptr; sc.d_long = nullptr; sc.d_partial = nullptr; sc.d_apart = nullptr; sc.d_datt = nullptr;
     int rc;
     if ((rc = upload(p, &sc.d_blocks, blocks.data(), blocks.size()))) return rc;
     if ((rc = upload(p, &sc.d_long, longs.data(), longs.size()))) return rc;
@@ -645,6 +651,69 @@ sddmm_fn pick_sddmm_heads(int nv, int k)
     return pick_sddmm_heads_nv<4>(k);
 }
 
+// GATv2 instances (gatv2.cuh): the score ring kernel of f = 128 nv (nv = 1, 2) and k heads, the raw-score softmax,
+// and the two backward walks with the multi-head launch shape
+typedef void (*gatv2_score_fn)(SddmmArgs, const Gatv2Halo, const float*, float);
+template <int NV>
+gatv2_score_fn pick_gatv2_ring_nv(int k)
+{
+    switch (k) {
+        case 1: return gatv2_score_ring_kernel<NV, 1>;
+        case 2: return gatv2_score_ring_kernel<NV, 2>;
+        case 4: return gatv2_score_ring_kernel<NV, 4>;
+        default: return gatv2_score_ring_kernel<NV, 8>;
+    }
+}
+gatv2_score_fn pick_gatv2_ring(int nv, int k) { return nv == 1 ? pick_gatv2_ring_nv<1>(k) : pick_gatv2_ring_nv<2>(k); }
+
+template <int K>
+attn_fn pick_softmax_raw_k(bool vec, bool backward)
+{
+    if (vec) return backward ? edge_softmax_raw_backward_kernel<K, true> : edge_softmax_raw_kernel<K, true>;
+    return backward ? edge_softmax_raw_backward_kernel<K, false> : edge_softmax_raw_kernel<K, false>;
+}
+attn_fn pick_softmax_raw(int k, bool vec, bool backward)
+{
+    switch (k) {
+        case 1: return pick_softmax_raw_k<1>(false, backward);
+        case 2: return pick_softmax_raw_k<2>(vec, backward);
+        case 4: return pick_softmax_raw_k<4>(vec, backward);
+        default: return pick_softmax_raw_k<8>(vec, backward);
+    }
+}
+
+typedef void (*gatv2_bwd_fn)(const SpmmArgs, const Gatv2BwdArgs);
+
+template <int LPE, int VW>
+gatv2_bwd_fn pick_gatv2_bwd_nh(int nh, bool col, bool halo)
+{
+    switch (nh) {
+        case 1: return col ? gatv2_col_backward_kernel<LPE, VW, 1>
+                           : (halo ? gatv2_row_backward_kernel<LPE, VW, true, 1> : gatv2_row_backward_kernel<LPE, VW, false, 1>);
+        case 2: return col ? gatv2_col_backward_kernel<LPE, VW, 2>
+                           : (halo ? gatv2_row_backward_kernel<LPE, VW, true, 2> : gatv2_row_backward_kernel<LPE, VW, false, 2>);
+        case 4: return col ? gatv2_col_backward_kernel<LPE, VW, 4>
+                           : (halo ? gatv2_row_backward_kernel<LPE, VW, true, 4> : gatv2_row_backward_kernel<LPE, VW, false, 4>);
+        default: return col ? gatv2_col_backward_kernel<LPE, VW, 8>
+                            : (halo ? gatv2_row_backward_kernel<LPE, VW, true, 8> : gatv2_row_backward_kernel<LPE, VW, false, 8>);
+    }
+}
+template <int VW>
+gatv2_bwd_fn pick_gatv2_bwd_lpe(int lpe, int nh, bool col, bool halo)
+{
+    switch (lpe) {
+        case 4: return pick_gatv2_bwd_nh<4, VW>(nh, col, halo);
+        case 8: return pick_gatv2_bwd_nh<8, VW>(nh, col, halo);
+        case 16: return pick_gatv2_bwd_nh<16, VW>(nh, col, halo);
+        default: return pick_gatv2_bwd_nh<32, VW>(nh, col, halo);
+    }
+}
+// col: the transposed (dxl) walk, else the row (dxr, datt) walk with or without a halo operand
+gatv2_bwd_fn pick_gatv2_bwd(int lpe, int vw, int nh, bool col, bool halo)
+{
+    return vw == 4 ? pick_gatv2_bwd_lpe<4>(lpe, nh, col, halo) : pick_gatv2_bwd_lpe<1>(lpe, nh, col, halo);
+}
+
 // CUDA loads kernels lazily, at their first launch, and that load synchronises with the device. A rank whose
 // stream already holds a spinning p2p_wait_kernel must therefore never launch a not-yet-loaded kernel behind it
 // when the ranks it waits for live in the SAME process (single-process multi-rank use: tests, smoke) — their put
@@ -689,6 +758,14 @@ void preload_kernels()
         }
     touch_kernel(spmm_max_fixup_kernel<4>); touch_kernel(spmm_max_fixup_kernel<1>);
     touch_kernel(max_empty_rows_kernel<4>); touch_kernel(max_empty_rows_kernel<1>);
+    for (int nh = 1; nh <= 8; nh *= 2) {
+        for (int nv = 1; nv <= 2; ++nv) touch_kernel(pick_gatv2_ring(nv, nh));
+        for (int vec = 0; vec < 2; ++vec) { touch_kernel(pick_softmax_raw(nh, vec != 0, false)); touch_kernel(pick_softmax_raw(nh, vec != 0, true)); }
+        for (int lpe = 4; lpe <= 32; lpe *= 2)
+            for (int vw = 1; vw <= 4; vw += 3)
+                for (int kind = 0; kind < 3; ++kind) touch_kernel(pick_gatv2_bwd(lpe, vw, nh, kind == 2, kind == 1));
+    }
+    touch_kernel(gatv2_score_plain_kernel); touch_kernel(gatv2_datt_kernel);
 }
 
 bool aligned16(const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
@@ -1171,6 +1248,176 @@ int launch_sddmm_heads(pgcn_plan* p, int k, const float* gZ, const float* H0, co
     ++p->launches;
     CU(p, cudaGetLastError());
     return 0;
+}
+
+// ---- GATv2 ----------------------------------------------------------------------------------
+
+// The datt partials of the forward register schedule (f_max floats per chunk of kGatv2Chunk row blocks): allocated once
+// per schedule, the first time a GATv2 backward or pgcn_plan_prepare of a bound plan needs them (never under capture),
+// and retired with the schedule.
+int gatv2_partial(pgcn_plan* p, DevCsr::Sched& sc, cudaStream_t st)
+{
+    if (sc.nblocks == 0 || sc.d_datt) return 0;
+    int rc = refuse_under_capture(p, st);
+    if (rc) return rc;
+    const size_t nchunks = (size_t)(sc.nblocks + kGatv2Chunk - 1) / kGatv2Chunk;
+    CU(p, cudaMalloc((void**)&sc.d_datt, nchunks * p->f_max * sizeof(float)));
+    return 0;
+}
+
+// The GATv2 score ring instance serves f = 128 and 256 with 16-byte aligned operands (the multi-head SDDMM's rule)
+bool gatv2_use_ring(const pgcn_plan* p, const float* xr, const float* xl, const float* H1, const float* H1_odd,
+                    const float* att, int f)
+{
+    return (f == 128 || f == 256) && sddmm_use_ring(p, xr, xl, H1, f) && aligned16(H1_odd) && aligned16(att);
+}
+
+int gatv2_attr(pgcn_plan* p, int f, int k, cudaStream_t st)
+{
+    const int nv = f / 128;
+    if (p->gatv2_attr_set[nv][k]) return 0;
+    int rc = refuse_under_capture(p, st);
+    if (rc) return rc;
+    const void* fptr = (const void*)pick_gatv2_ring(nv, k);
+    const size_t smem = sddmm_smem_bytes(nv);
+    CU(p, cudaFuncSetAttribute(fptr, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int nb = 0;
+    CU(p, cudaOccupancyMaxActiveBlocksPerMultiprocessorWithFlags(&nb, fptr, kSddmmWarps * 32, smem, 0));
+    p->gatv2_ctas_per_sm[nv][k] = std::max(nb, 1);
+    p->gatv2_attr_set[nv][k] = true;
+    return 0;
+}
+
+// scores (nnz x k, forward CSR order) of the forward records, written into `out`; H1 / H1_odd: the halo slab of the
+// call and its odd-epoch twin on the peer transport (or null)
+int launch_gatv2_score(pgcn_plan* p, int k, const float* xr, const float* xl, const float* H1, const float* H1_odd,
+                       const float* att, float slope, float* out, int f, cudaStream_t st)
+{
+    DevCsr& c = p->fwd;
+    if (c.nnz == 0 || c.nrows == 0) return 0;
+    const bool ring = gatv2_use_ring(p, xr, xl, H1, H1_odd, att, f);
+    int64_t epb, long_row;
+    sched_params(p, c, ring, &epb, &long_row);
+    int rc;
+    if (!sched_ready(c, ring ? 1 : 0, epb, long_row) && (rc = refuse_under_capture(p, st))) return rc;
+    if ((rc = build_schedule(p, c, ring ? 1 : 0, epb, long_row))) return rc;
+    const DevCsr::Sched& sc = c.sched[ring ? 1 : 0];
+    if (sc.nblocks == 0) return 0;
+    SddmmArgs a;
+    a.blocks = sc.d_blocks; a.nblocks = sc.nblocks;
+    a.pieces = c.d_cw;
+    a.gZ = xr; a.H0 = xl; a.H1 = H1; a.split = p->m;
+    a.rowids = c.d_rowids;
+    a.dvals = out; a.f = f;
+    a.counter = nullptr;
+    const Gatv2Halo hl = {H1_odd, H1_odd ? p->d_epoch : nullptr};
+    if (ring) {
+        const int nv = f / 128;
+        if ((rc = gatv2_attr(p, f, k, st))) return rc;
+        CU(p, cudaMemsetAsync(p->d_counter, 0, sizeof(unsigned int), st));
+        a.counter = p->d_counter;
+        const unsigned ctas = (unsigned)((sc.nblocks + kSddmmWarps - 1) / kSddmmWarps);
+        const unsigned grid = std::min<unsigned>(ctas, (unsigned)(p->num_sms * p->gatv2_ctas_per_sm[nv][k]));
+        pick_gatv2_ring(nv, k)<<<grid, kSddmmWarps * 32, sddmm_smem_bytes(nv), st>>>(a, hl, att, slope);
+    } else {
+        gatv2_score_plain_kernel<<<(unsigned)((sc.nblocks + 7) / 8), 256, 0, st>>>(a, hl, att, slope, k);
+    }
+    ++p->launches;
+    CU(p, cudaGetLastError());
+    return 0;
+}
+
+// One of the two backward walks on the register schedule of c (the forward records: dxr and the datt partials; the
+// transposed ones: dxl and the halo partials), its empty rows and its split rows. vw: as the multi-head aggregation.
+int launch_gatv2_walk(pgcn_plan* p, DevCsr& c, bool col, int k, const SpmmArgs& a0, Gatv2BwdArgs g,
+                      std::initializer_list<const void*> ops, cudaStream_t st)
+{
+    const int f = a0.f;
+    int64_t epb, long_row;
+    sched_params(p, c, false, &epb, &long_row);
+    int rc;
+    if (!sched_ready(c, 0, epb, long_row) && (rc = refuse_under_capture(p, st))) return rc;
+    if ((rc = build_schedule(p, c, 0, epb, long_row))) return rc;
+    DevCsr::Sched& sc = c.sched[0];
+    if (!col && (rc = gatv2_partial(p, sc, st))) return rc;
+    const int vw = (f / k) % 4 != 0 ? 1 : vec_width(f, ops);
+    const TileCfg t = choose_tile_heads(f, vw);
+    if (c.nempty > 0) {
+        ZeroArgs za;
+        za.rows = c.d_empty; za.nrows_empty = c.nempty; za.Z0 = a0.Z0; za.Z1 = a0.Z1; za.zsplit = a0.zsplit; za.f = f;
+        const unsigned grid = (unsigned)(((long long)c.nempty * (f / vw) + 255) / 256);
+        if (vw == 4) zero_rows_kernel<4><<<grid, 256, 0, st>>>(za);
+        else zero_rows_kernel<1><<<grid, 256, 0, st>>>(za);
+        ++p->launches;
+    }
+    if (sc.nblocks > 0) {
+        SpmmArgs a = a0;
+        a.blocks = sc.d_blocks; a.nblocks = sc.nblocks;
+        a.pieces = c.d_cw;
+        a.rowids = c.d_rowids;
+        a.partial = sc.d_partial;
+        g.datt_part = sc.d_datt;
+        const int groups_per_cta = kSpmmThreads / t.lpe;
+        dim3 grid((unsigned)((sc.nblocks + groups_per_cta - 1) / groups_per_cta), (unsigned)t.tiles);
+        pick_gatv2_bwd(t.lpe, vw, k, col, a.H1 != nullptr)<<<grid, kSpmmThreads, 0, st>>>(a, g);
+        ++p->launches;
+    }
+    if (sc.nlong > 0) {
+        FixupArgs fa;
+        fa.long_rows = sc.d_long; fa.nlong = sc.nlong; fa.partial = sc.d_partial;
+        fa.Z0 = a0.Z0; fa.Z1 = a0.Z1; fa.zsplit = a0.zsplit; fa.rowids = c.d_rowids; fa.f = f; fa.beta = 0;
+        fa.relu = 0; fa.final = nullptr;
+        const unsigned grid = (unsigned)sc.nlong * (unsigned)((f / vw + 31) / 32);
+        if (vw == 4) spmm_fixup_kernel<4><<<grid, 32 * kFixupGroups, 0, st>>>(fa);
+        else spmm_fixup_kernel<1><<<grid, 32 * kFixupGroups, 0, st>>>(fa);
+        ++p->launches;
+    }
+    CU(p, cudaGetLastError());
+    return 0;
+}
+
+// dxr (m x f) and datt (f) from dscore (nnz x k) on the forward records
+int launch_gatv2_rows(pgcn_plan* p, int k, const float* dscore, const float* xl, const float* xl_halo, const float* xr,
+                      const float* att, float slope, float* dxr, float* datt, int f, cudaStream_t st)
+{
+    DevCsr& c = p->fwd;
+    if (c.nrows > 0) {
+        SpmmArgs a = {};
+        a.H0 = xl; a.H1 = xl_halo; a.split = p->m;
+        a.Z0 = dxr; a.Z1 = nullptr; a.zsplit = p->m;
+        a.f = f;
+        Gatv2BwdArgs g = {};
+        g.dscore = dscore; g.att = att; g.slope = slope; g.hd = f / k; g.xv = xr;
+        int rc = launch_gatv2_walk(p, c, false, k, a, g, {xl, xl_halo, xr, att, dxr}, st);
+        if (rc) return rc;
+    }
+    const int nblocks = c.nrows > 0 ? c.sched[0].nblocks : 0;
+    if (nblocks == 0) {
+        CU(p, cudaMemsetAsync(datt, 0, (size_t)f * sizeof(float), st));
+        return 0;
+    }
+    const int nchunks = (nblocks + kGatv2Chunk - 1) / kGatv2Chunk;
+    gatv2_datt_kernel<<<(unsigned)((f + 31) / 32), 32 * kGatv2RedWarps, 0, st>>>(c.sched[0].d_datt, nchunks, f, datt);
+    ++p->launches;
+    CU(p, cudaGetLastError());
+    return 0;
+}
+
+// dxl (rows < m) and the halo partials (rows m .., into G_halo) on the transposed records
+int launch_gatv2_cols(pgcn_plan* p, int k, const float* alpha, const float* dscore, const float* gZ, const float* xl,
+                      const float* xl_halo, const float* xr, const float* att, float slope, float* dxl, float* G_halo,
+                      int f, cudaStream_t st)
+{
+    DevCsr& c = p->tr;
+    if (c.nrows == 0) return 0;
+    SpmmArgs a = {};
+    a.H0 = gZ; a.H1 = xr; a.split = p->m;
+    a.Z0 = dxl; a.Z1 = G_halo; a.zsplit = p->m;
+    a.f = f;
+    Gatv2BwdArgs g = {};
+    g.alpha = alpha; g.dscore = dscore; g.att = att; g.slope = slope; g.hd = f / k; g.amap = c.d_vmap;
+    g.xv = xl; g.xv_halo = xl_halo;
+    return launch_gatv2_walk(p, c, true, k, a, g, {gZ, xr, xl, xl_halo, att, dxl, G_halo}, st);
 }
 
 // Set-up copies of pgcn_plan_bind_values. They run on the plan's own non-blocking stream and wait for that stream only:
@@ -1783,6 +2030,11 @@ int pgcn_plan_prepare(pgcn_plan* p, int32_t f)
             if ((f / k) % 4 == 0 && (rc = sddmm_heads_attr(p, f, k, p->host_stream))) return rc;
     // the max calls of a bound plan: the register schedules (built above) and the entries of the forward's split rows
     if (p->bound && (rc = max_partial(p, p->fwd.sched[0], p->host_stream))) return rc;
+    // the GATv2 calls: the score ring instances of width f and the datt partials of a bound plan
+    if (ring && (f == 128 || f == 256))
+        for (int k = 1; k <= 8; k *= 2)
+            if ((rc = gatv2_attr(p, f, k, p->host_stream))) return rc;
+    if (p->bound && (rc = gatv2_partial(p, p->fwd.sched[0], p->host_stream))) return rc;
     p->prepared = true;
     return 0;
 }
@@ -2516,6 +2768,74 @@ int pgcn_backward_max(pgcn_plan* p, const int32_t* arg, const float* gZ, float* 
     cudaStream_t st = (cudaStream_t)stream;
     return unsplit_backward(p, G_own, f, st, [&]() {
         return launch_max_backward(p, arg, gZ, G_own, p->d_hsend_slab, f, st);
+    });
+}
+
+// ---- GATv2 attention ------------------------------------------------------------------------------------------------
+
+static int launch_softmax_raw(pgcn_plan* p, bool backward, int k, const float* alpha, float* io, cudaStream_t st)
+{
+    if (p->m == 0 || p->fwd.nnz == 0) return 0;
+    AttnArgs a = attn_args(p, nullptr, nullptr, nullptr, 0.f);
+    a.alpha = backward ? alpha : nullptr;
+    a.dalpha = backward ? io : nullptr;
+    a.out = io;
+    const unsigned grid = (unsigned)p->nlong_rows + (unsigned)((p->m + kAttnWarps - 1) / kAttnWarps);
+    pick_softmax_raw(k, attn_vec(k, {alpha, io}), backward)<<<grid, kAttnThreads, 0, st>>>(a);
+    ++p->launches;
+    CU(p, cudaGetLastError());
+    return 0;
+}
+
+// The unsplit forward exchange of xl, then in one launch sequence: the scores into alpha, their softmax in place, the
+// multi-head aggregation of xl with alpha over [xl_own | halo slab of the call's parity], and the halo copy.
+int pgcn_forward_gatv2(pgcn_plan* p, int32_t heads, const float* xl_own, const float* xr, const float* att,
+                       float negative_slope, float* alpha, float* Z, float* xl_halo_out, int32_t f, void* stream)
+{
+    int rc = heads_check_f(p, "pgcn_forward_gatv2", heads, f);
+    if (rc) return rc;
+    if (!att || (p->m > 0 && (!xl_own || !xr || !Z)))
+        return fail(p, PGCN_ERR_INVALID, "pgcn_forward_gatv2: null xl_own/xr/att/Z");
+    if (p->fwd.nnz > 0 && !alpha) return fail(p, PGCN_ERR_INVALID, "pgcn_forward_gatv2: null alpha");
+    cudaStream_t st = (cudaStream_t)stream;
+    const HeadArgs ha = {alpha, nullptr, heads};
+    return unsplit_forward(p, xl_own, f, st, [&](float* halo, const float* halo_odd) -> int {
+        const float* H1 = p->h > 0 ? halo : nullptr;
+        const float* H1_odd = p->h > 0 ? halo_odd : nullptr;
+        int rc2 = launch_gatv2_score(p, heads, xr, xl_own, H1, H1_odd, att, negative_slope, alpha, f, st);
+        if (rc2 || (rc2 = launch_softmax_raw(p, false, heads, nullptr, alpha, st))) return rc2;
+        if ((rc2 = launch_spmm(p, p->fwd, xl_own, H1, p->m, Z, nullptr, p->m, f, 0, st, 0, false, H1_odd, &ha)))
+            return rc2;
+        if (p->k == 1 || !xl_halo_out || p->h == 0) return 0;
+        const long long n = (long long)p->h * f;
+        copy_halo_kernel<<<grid_for(n, p->num_sms), 256, 0, st>>>(halo, halo_odd, halo_odd ? p->d_epoch : nullptr,
+                                                                  xl_halo_out, n);
+        ++p->launches;
+        CU(p, cudaGetLastError());
+        return 0;
+    });
+}
+
+// dalpha = SDDMM(gZ, xl) into work, dscore over it in place, dxr and datt on the forward records, then dxl on the
+// transposed records inside the unsplit backward exchange.
+int pgcn_backward_gatv2(pgcn_plan* p, int32_t heads, const float* alpha, const float* gZ, const float* xl_own,
+                        const float* xl_halo, const float* xr, const float* att, float negative_slope, float* work,
+                        float* dxl, float* dxr, float* datt, int32_t f, void* stream)
+{
+    int rc = heads_check_f(p, "pgcn_backward_gatv2", heads, f);
+    if (rc) return rc;
+    if (!att || !datt || (p->m > 0 && (!gZ || !xl_own || !xr || !dxl || !dxr)))
+        return fail(p, PGCN_ERR_INVALID, "pgcn_backward_gatv2: null gZ/xl_own/xr/att/dxl/dxr/datt");
+    if (p->fwd.nnz > 0 && (!alpha || !work)) return fail(p, PGCN_ERR_INVALID, "pgcn_backward_gatv2: null alpha/work");
+    if (p->h > 0 && !xl_halo) return fail(p, PGCN_ERR_INVALID, "pgcn_backward_gatv2: h=%d but xl_halo is null", p->h);
+    cudaStream_t st = (cudaStream_t)stream;
+    const float* xh = p->h > 0 ? xl_halo : nullptr;
+    if ((rc = launch_sddmm_heads(p, heads, gZ, xl_own, xh, work, f, st))) return rc;
+    if ((rc = launch_softmax_raw(p, true, heads, alpha, work, st))) return rc;
+    if ((rc = launch_gatv2_rows(p, heads, work, xl_own, xh, xr, att, negative_slope, dxr, datt, f, st))) return rc;
+    return unsplit_backward(p, dxl, f, st, [&]() {
+        return launch_gatv2_cols(p, heads, alpha, work, gZ, xl_own, xh, xr, att, negative_slope, dxl, p->d_hsend_slab,
+                                 f, st);
     });
 }
 

@@ -293,9 +293,19 @@ __device__ __forceinline__ void sddmm_reduce_heads(float (&p)[N], int lane)
     for (int t = S; t < LB; ++t) p[0] += __shfl_xor_sync(0xffffffffu, p[0], L >> (t + 1));
 }
 
-template <int NV, int K>
-__global__ void __maxnreg__(232)         // launched with kSddmmWarps * 32 threads; without a limit ptxas caps some at 128 and spills
-sddmm_heads_ring_kernel(const SddmmArgs a)
+// The per-element term of the multi-head SDDMM: s += gZ_c * H_c (g: the row held in registers, r: the gathered row).
+struct SddmmDot {
+    __device__ __forceinline__ void operator()(float& s, const float4& g, const float4& r, int) const
+    {
+        s = fmaf(g.x, r.x, s); s = fmaf(g.y, r.y, s);
+        s = fmaf(g.z, r.z, s); s = fmaf(g.w, r.w, s);
+    }
+};
+
+// The ring walk of sddmm_heads_ring_kernel with the per-element term C (called with the chain sum, the register row's
+// float4 v, the gathered row's float4 v and v): the SDDMM's dot product, or GATv2's score (gatv2.cuh).
+template <int NV, int K, class C>
+__device__ __forceinline__ void sddmm_heads_ring_walk(const SddmmArgs& a, const C& comb)
 {
     typedef SddmmHeadShape<NV, K> S;
     constexpr int G = kSddmmG, NG = kSddmmNG, NS = G * NG;
@@ -399,8 +409,7 @@ sddmm_heads_ring_kernel(const SddmmArgs a)
                 for (int v = 0; v < NV; ++v) {
                     const int u = v / S::VPC;
                     const float4 r = slot[j * RV + v * 32];
-                    s[u] = fmaf(gcur[v].x, r.x, s[u]); s[u] = fmaf(gcur[v].y, r.y, s[u]);
-                    s[u] = fmaf(gcur[v].z, r.z, s[u]); s[u] = fmaf(gcur[v].w, r.w, s[u]);
+                    comb(s[u], gcur[v], r, v);
                 }
 #pragma unroll
                 for (int u = 0; u < S::U; ++u) p[u * 8 + j] = (vm >> j & 1u) ? s[u] : 0.f;
@@ -427,6 +436,13 @@ sddmm_heads_ring_kernel(const SddmmArgs a)
         if (lane == 0) w = (int)atomicAdd(a.counter, 1u);
         w = __shfl_sync(0xffffffffu, w, 0);
     }
+}
+
+template <int NV, int K>
+__global__ void __maxnreg__(232)         // launched with kSddmmWarps * 32 threads; without a limit ptxas caps some at 128 and spills
+sddmm_heads_ring_kernel(const SddmmArgs a)
+{
+    sddmm_heads_ring_walk<NV, K>(a, SddmmDot());
 }
 
 // Any f, K and alignment: sddmm_plain_kernel with K heads; a lane's dot product restarts at every head boundary

@@ -442,6 +442,89 @@ class PGATMultiHeadAttention(torch.autograd.Function):
         return None, dZ, d_el, d_er, None
 
 
+class PGATv2Attention(torch.autograd.Function):
+    """GATv2 attention (dynamic attention, Brody et al.) over the plan's stored pattern: K = att.shape[0] heads (1, 2, 4
+    or 8) of width d = f / K, concatenated.
+
+        PGATv2Attention.apply(A, XL, XR, att, negative_slope=0.2)
+        s_eh = sum_c att[h, c] * LeakyReLU(XL[col(e), h d + c] + XR[row(e), h d + c]),
+        alpha_.h = softmax of s_.h over each row's stored entries,  out[:, h d:(h+1) d] = A(alpha[:, h]) XL[:, h d:(h+1) d]
+
+    XL and XR are [rows, f] and att is [K, d], fp32 CUDA tensors; out is [rows, f] (rows = m in the "local" layout, n in
+    the "global" one, as PGATMultiHeadAttention). This is PyG GATv2Conv(share_weights=False, concat=True, bias=False,
+    add_self_loops=False) on XL = lin_l(x), XR = lin_r(x); passing one tensor as XL and XR is share_weights=True, and
+    its gradient is the sum of both. One exchange per layer carries XL's halo rows (pgcn_forward_gatv2), which the
+    backward reuses. Gradients for XL, XR and att come from pgcn_backward_gatv2. The plan's resident values are never
+    read or written. Deterministic. The plan must be bound (PgcnPlan.bind_values)."""
+
+    @staticmethod
+    def forward(ctx, A, XL, XR, att, negative_slope=0.2):
+        rows = A.n if A.layout == "global" else A.m
+        if att.dim() != 2:
+            raise ValueError("att must be [heads, f / heads], got %s" % (tuple(att.shape),))
+        K = att.shape[0]
+        if K not in HEADS:
+            raise ValueError("heads=%d: the GATv2 kernels take 1, 2, 4 or 8 heads" % K)
+        XL_own = _check_feat(A, XL, rows, "XL")
+        XR_own = _check_feat(A, XR, rows, "XR")
+        f = XL_own.shape[1]
+        if XR_own.shape[1] != f:
+            raise ValueError("XL and XR must have the same width, got %d and %d" % (f, XR_own.shape[1]))
+        if f % K:
+            raise ValueError("f=%d is not a multiple of heads=%d" % (f, K))
+        if tuple(att.shape) != (K, f // K):
+            raise ValueError("att must be [%d, %d], got %s" % (K, f // K, tuple(att.shape)))
+        if not att.is_cuda or att.dtype != torch.float32:
+            raise TypeError("att must be a float32 CUDA tensor")
+        att_c = att.detach().contiguous()
+        if A.layout == "global":
+            XL_own = XL_own.index_select(0, A.owned_index())
+            XR_own = XR_own.index_select(0, A.owned_index())
+        lp = A.lp
+        dev = XL_own.device
+        slope = float(negative_slope)
+        lib = cabi.load()
+        with torch.cuda.device(dev):
+            if not A._bound:
+                raise RuntimeError("PGATv2Attention reads the plan's value maps: call PgcnPlan.bind_values() once "
+                                   "(set-up, before any CUDA-graph capture)")
+            alpha = torch.empty((lp.nnz(), K), dtype=torch.float32, device=dev)
+            out = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+            XL_halo = torch.empty((lp.h, f), dtype=torch.float32, device=dev)
+            keep = lp.k > 1 and lp.h > 0
+            cabi.check(lib.pgcn_forward_gatv2(A.handle, K, XL_own.data_ptr(), XR_own.data_ptr(), att_c.data_ptr(),
+                                              slope, alpha.data_ptr(), out.data_ptr(),
+                                              XL_halo.data_ptr() if keep else None, f, _stream_ptr()), A.handle)
+            if lp.k > 1:
+                A.count_exchange(backward=False)
+        ctx.plan, ctx.rows, ctx.slope, ctx.heads = A, rows, slope, K
+        ctx.save_for_backward(alpha, XL_own, XL_halo, XR_own, att_c)
+        return _to_layout(A, out, rows)
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        A, rows, slope, K = ctx.plan, ctx.rows, ctx.slope, ctx.heads
+        alpha, XL_own, XL_halo, XR_own, att = ctx.saved_tensors
+        g = _check_feat(A, grad_output, rows, "grad_output")
+        if A.layout == "global":
+            g = g.index_select(0, A.owned_index())
+        lp = A.lp
+        f = g.shape[1]
+        dev = g.device
+        with torch.cuda.device(dev):
+            work = torch.empty_like(alpha)
+            dxl = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+            dxr = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+            datt = torch.empty_like(att)
+            cabi.check(cabi.load().pgcn_backward_gatv2(
+                A.handle, K, alpha.data_ptr(), g.data_ptr(), XL_own.data_ptr(), XL_halo.data_ptr() if lp.h else None,
+                XR_own.data_ptr(), att.data_ptr(), slope, work.data_ptr(), dxl.data_ptr(), dxr.data_ptr(),
+                datt.data_ptr(), f, _stream_ptr()), A.handle)
+            if lp.k > 1:
+                A.count_exchange(backward=True)
+        return None, _to_layout(A, dxl, rows), _to_layout(A, dxr, rows), datt, None
+
+
 # ---- max aggregation -------------------------------------------------------------------------------------------------
 
 def _check_max_plan(plan, what):

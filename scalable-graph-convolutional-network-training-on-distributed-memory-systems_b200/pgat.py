@@ -19,6 +19,10 @@ CPU fallback (the fp64 oracle lives under oracle/ and is test infrastructure).
 layer stays f -> f. K = 1 is the single-head layer above, with the same parameter draws. K > 1: Linear(f, f, bias=False)
 and a (2d x K) attention matrix, both xavier_normal with the relu gain in that order; el[:, h] = Z_h a[:d, h] and
 er[:, h] = Z_h a[d:, h] for head h's slice Z_h of Z (op.PGATMultiHeadAttention).
+
+--v2: GATv2 layers instead (dynamic attention, op.PGATv2Attention), with --heads K as above. Per layer lin_l and lin_r
+(Linear(f, f, bias=False)) and att (K x d), drawn in that order, each xavier_normal with the relu gain; the layer is
+PyG GATv2Conv(share_weights=False, concat=True, bias=False, add_self_loops=False) over the stored pattern.
 """
 import getopt
 import os
@@ -31,7 +35,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import graphio, plan as planmod
-from .op import HEADS, PGATAttention, PGATMultiHeadAttention
+from .op import HEADS, PGATAttention, PGATMultiHeadAttention, PGATv2Attention
 from .pgcn import average_gradients, initialize_parameters, init_process
 
 
@@ -69,8 +73,30 @@ class PGAT(nn.Module):
         return PGATAttention.apply(self.A, Z, el, er, self.negative_slope)
 
 
+class PGATv2(nn.Module):
+    """GATv2 layer f -> f with K heads: out = PGATv2Attention(A, lin_l(H), lin_r(H), att)."""
+
+    def __init__(self, A, in_features, out_features, negative_slope=0.2, heads=1):
+        super().__init__()
+        self.A = A
+        self.negative_slope = negative_slope
+        self.lin_l = nn.Linear(in_features, out_features, bias=False)
+        self.lin_r = nn.Linear(in_features, out_features, bias=False)
+        self.att = nn.Parameter(torch.empty(size=(heads, out_features // heads)))
+        self.reset_parameters()
+
+    def reset_parameters(self):
+        gain = nn.init.calculate_gain("relu")
+        nn.init.xavier_normal_(self.lin_l.weight, gain=gain)
+        nn.init.xavier_normal_(self.lin_r.weight, gain=gain)
+        nn.init.xavier_normal_(self.att, gain=gain)
+
+    def forward(self, H):
+        return PGATv2Attention.apply(self.A, self.lin_l(H), self.lin_r(H), self.att, self.negative_slope)
+
+
 def run(rank, size, nlayers, nfeatures, path_A, path_partvec, backend, transport="auto", out=sys.stdout, seed=None,
-        negative_slope=1.0, epochs=50, heads=1):
+        negative_slope=1.0, epochs=50, heads=1, v2=False):
     if backend != "nccl":
         raise RuntimeError("backend '%s': the H100 PGAT path runs on CUDA devices over NCCL/NVLink only "
                            "(no CPU fallback); use -b nccl" % backend)
@@ -82,7 +108,7 @@ def run(rank, size, nlayers, nfeatures, path_A, path_partvec, backend, transport
     lp_host = planmod.build_local_plan(A, partvec, rank, size)
     n = lp_host.n
     # the multi-head backward gets d_er from an aggregation of width 4 K (PGATMultiHeadAttention)
-    plan = planmod.PgcnPlan(lp_host, nfeatures if heads == 1 else max(nfeatures, 4 * heads), device=device)
+    plan = planmod.PgcnPlan(lp_host, nfeatures if heads == 1 or v2 else max(nfeatures, 4 * heads), device=device)
     used = plan.init_comm(transport=transport)
     plan.bind_values()
     lp = plan.lp
@@ -93,7 +119,8 @@ def run(rank, size, nlayers, nfeatures, path_A, path_partvec, backend, transport
 
     if seed is not None:
         torch.manual_seed(seed)
-    model = nn.Sequential(*[PGAT(plan, nfeatures, nfeatures, negative_slope, heads) for _ in range(nlayers)]).to(device)
+    layer = PGATv2 if v2 else PGAT
+    model = nn.Sequential(*[layer(plan, nfeatures, nfeatures, negative_slope, heads) for _ in range(nlayers)]).to(device)
     if size > 1:
         initialize_parameters(model, size)
     optimizer = torch.optim.Adam(model.parameters(), lr=1e-3)
@@ -131,7 +158,7 @@ def main(argv):
     rank = int(os.environ.get("SLURM_PROCID", os.environ.get("RANK", "0")))
     os.environ["RANK"] = str(rank)
     try:
-        opts, _ = getopt.getopt(argv, "a:p:b:s:l:f:", ["transport=", "seed=", "negative-slope=", "heads="])
+        opts, _ = getopt.getopt(argv, "a:p:b:s:l:f:", ["transport=", "seed=", "negative-slope=", "heads=", "v2"])
     except getopt.GetoptError:
         print("a:p:b:", flush=True)                                       # the reference's usage text
         sys.exit(2)
@@ -158,6 +185,8 @@ def main(argv):
             kw["seed"] = int(arg)
         elif opt == "--negative-slope":
             kw["negative_slope"] = float(arg)
+        elif opt == "--v2":
+            kw["v2"] = True
         elif opt == "--heads":
             try:
                 kw["heads"] = int(arg)
@@ -167,7 +196,7 @@ def main(argv):
     if (path_A is None or path_partvec is None or nlayers is None or nfeatures is None or heads not in HEADS
             or nfeatures % heads):
         print("usage: PGAT.py -a <A.mtx> -p <partvec> -b nccl -s <nparts> -l <nlayers> -f <nfeatures> "
-              "[--seed N] [--negative-slope S] [--heads 1|2|4|8, dividing nfeatures]", flush=True)
+              "[--seed N] [--negative-slope S] [--heads 1|2|4|8, dividing nfeatures] [--v2]", flush=True)
         sys.exit(2)
     os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
     os.environ.setdefault("MASTER_PORT", "29500")
