@@ -21,6 +21,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <string>
+#include <unordered_map>
 #include <vector>
 
 using namespace pgcn;
@@ -158,8 +159,7 @@ struct pgcn_plan {
     int64_t opt_persistent_multi = 0;
     int64_t opt_kernel = 0, opt_ring_slots = 16, opt_ring_epb = 512, opt_ring_long = 0, opt_persistent = 1;
     int64_t opt_ring_tile = 0;       // ring row tile in floats: 0 = tuned (else full width), 64 | 128 | 256
-    bool ring_attr_set[72] = {false};
-    int ring_ctas_per_sm[72] = {0};
+    std::unordered_map<const void*, int> ctas_per_sm;   // kernels opted in to their dynamic shared memory: CTAs per SM
     unsigned int* d_counter = nullptr;     // work-item counter of the persistent ring kernel
     int num_sms = 132;
 
@@ -197,12 +197,6 @@ struct pgcn_plan {
     ValueSet* d_vsets = nullptr;
     int nvsets = 0;
     long long vtotal = 0;                  // entries over all sets
-    bool sddmm_attr_set[5] = {false};      // per f / 128 of the SDDMM ring kernel
-    int sddmm_ctas_per_sm[5] = {0};
-    bool sddmm_heads_attr_set[5][9] = {};  // per f / 128 and head count of the multi-head SDDMM ring kernel
-    int sddmm_heads_ctas_per_sm[5][9] = {};
-    bool gatv2_attr_set[3][9] = {};        // per f / 128 and head count of the GATv2 score ring kernel
-    int gatv2_ctas_per_sm[3][9] = {};
     int* d_rowptr = nullptr;               // m + 1, the forward rowptr (edge softmax)
     int* d_long_rows = nullptr;            // rows of more than kAttnLongRow entries (one CTA each in the edge softmax)
     int nlong_rows = 0;
@@ -335,6 +329,20 @@ void csr_free(DevCsr& c)
     c = DevCsr();
 }
 
+// The matrices the plan launches: forward and transposed records and, when split, the own-column part, each peer's
+// halo block and the transposed row ranges of the pipelined backward
+std::vector<DevCsr*> plan_matrices(pgcn_plan* p)
+{
+    std::vector<DevCsr*> mats = {&p->fwd, &p->tr};
+    if (p->have_split) {
+        mats.push_back(&p->own);
+        mats.push_back(&p->tr_own);
+        for (auto& c : p->halo_q) mats.push_back(&c);
+        for (auto& c : p->tr_halo_q) mats.push_back(&c);
+    }
+    return mats;
+}
+
 // Cut the (compact) row range into row blocks of about `epb` nnz (at most kMaxRowsPerBlock rows); rows longer
 // than `long_row` become ceil(deg/epb) single-row segments with a slot each in the side buffer.
 constexpr int kMaxRowsPerBlock = 128;
@@ -377,20 +385,40 @@ void make_schedule(const int* rp, int nrows_c, int64_t epb, int64_t long_row,
     close(nrows_c);
 }
 
-bool sched_ready(const DevCsr& c, int which, int64_t epb, int64_t long_row)
+// A stream under CUDA graph capture takes only stream-ordered work. Set-up that would allocate, copy synchronously or
+// set a function attribute is refused before any such call, so the caller's capture stays valid.
+int refuse_under_capture(pgcn_plan* p, cudaStream_t st)
 {
-    return c.sched[which].epb == epb && c.sched[which].long_row == long_row;
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    const cudaError_t e = cudaStreamIsCapturing(st, &cs);
+    if (e == cudaSuccess && cs == cudaStreamCaptureStatusNone) return 0;
+    if (e != cudaSuccess) cudaGetLastError();
+    return fail(p, PGCN_ERR_STATE, "this call needs set-up work (schedule upload or kernel attributes) that cannot run "
+                "while the stream is being captured into a CUDA graph: call pgcn_plan_prepare(plan, f) before capturing");
 }
 
-int build_schedule(pgcn_plan* p, DevCsr& c, int which, int64_t epb, int64_t long_row)
+// Matrix c's schedule for the ring (or register) kernel, with the block size and long-row threshold of the current
+// options or the autotune. It is built on first use, which is refused while `st` is being captured.
+int schedule(pgcn_plan* p, DevCsr& c, bool ring, cudaStream_t st, DevCsr::Sched** out)
 {
-    DevCsr::Sched& sc = c.sched[which];
-    if (sched_ready(c, which, epb, long_row)) return 0;
+    DevCsr::Sched& sc = c.sched[ring ? 1 : 0];
+    *out = &sc;
+    int64_t epb, long_row;
+    if (ring) {
+        epb = std::max<int64_t>(c.tuned_epb[1] > 0 ? c.tuned_epb[1] : p->opt_ring_epb, 64);
+        long_row = p->opt_ring_long > 0 ? p->opt_ring_long : 2 * epb;
+    } else {
+        epb = std::max<int64_t>(c.tuned_epb[0] > 0 ? c.tuned_epb[0] : p->opt_epb, 8);
+        long_row = p->opt_long > 0 ? p->opt_long : 4 * epb;
+    }
+    if (sc.epb == epb && sc.long_row == long_row) return 0;
+    int rc = refuse_under_capture(p, st);
+    if (rc) return rc;
 
     std::vector<int4> blocks, longs;
     int nslots = 0;
     make_schedule(c.h_rowptr.data(), c.nrows_c, epb, long_row, blocks, longs, nslots,
-                  which == 1 ? (1 << 30) : kMaxRowsPerBlock, c.row_base);
+                  ring ? (1 << 30) : kMaxRowsPerBlock, c.row_base);
 
     if (p->prepared && sc.epb >= 0) {
         // a graph captured after pgcn_plan_prepare may still launch the old schedule: keep it until pgcn_plan_destroy
@@ -401,7 +429,6 @@ int build_schedule(pgcn_plan* p, DevCsr& c, int which, int64_t epb, int64_t long
         cudaFree(sc.d_blocks); cudaFree(sc.d_long); cudaFree(sc.d_partial); cudaFree(sc.d_apart); cudaFree(sc.d_datt);
     }
     sc.d_blocks = nullptr; sc.d_long = nullptr; sc.d_partial = nullptr; sc.d_apart = nullptr; sc.d_datt = nullptr;
-    int rc;
     if ((rc = upload(p, &sc.d_blocks, blocks.data(), blocks.size()))) return rc;
     if ((rc = upload(p, &sc.d_long, longs.data(), longs.size()))) return rc;
     CU(p, cudaMalloc((void**)&sc.d_partial, std::max<size_t>((size_t)nslots * p->f_max, 1) * sizeof(float)));
@@ -613,6 +640,34 @@ ring_tm_fn pick_ring_tm(int tf, int shape, bool halo)
     return halo ? pick_ring_tm_t<128, true>(shape) : pick_ring_tm_t<128, false>(shape);
 }
 
+// A ring instance of row tile tf, shape and fill mode (2: tensor map, 0: 1-D bulk copies, 1: cp.async): its kernel,
+// dynamic shared memory and warps per CTA
+struct RingInst { const void* fn; size_t smem; int warps; };
+
+RingInst ring_inst(int tf, int shape, int mode, bool halo)
+{
+    const int g = kRingShapes[shape].g, ng = kRingShapes[shape].ng;
+    return {mode == 2 ? (const void*)pick_ring_tm(tf, shape, halo) : (const void*)pick_ring(tf, shape, mode, halo),
+            ring_smem_bytes(tf, g * ng, ng), ring_cta_warps(tf, g * ng, ng)};
+}
+
+// fn(ring instance) for every instance launch_spmm can pick: the tensor-map fill in every shape, the 1-D bulk fill in
+// the two 16-row-slot-group shapes, the cp.async fill (full-width tiles) in shape 0; stops at the first nonzero return.
+template <class F>
+int for_each_ring(F fn)
+{
+    int rc;
+    for (int tf = 64; tf <= 256; tf *= 2)
+        for (int halo = 0; halo < 2; ++halo) {
+            for (int shape = 0; shape < 4; ++shape)
+                if ((rc = fn(ring_inst(tf, shape, 2, halo != 0)))) return rc;
+            for (int shape = 0; shape < 2; ++shape)
+                if ((rc = fn(ring_inst(tf, shape, 0, halo != 0)))) return rc;
+            if (tf >= 128 && (rc = fn(ring_inst(tf, 0, 1, halo != 0)))) return rc;
+        }
+    return 0;
+}
+
 typedef void (*attn_fn)(const AttnArgs);
 
 // the edge softmax instance of K heads (VEC: vector loads of the K values of an entry or row)
@@ -729,12 +784,7 @@ void preload_kernels()
     for (int halo = 0; halo < 2; ++halo)
         for (int lpe = 4; lpe <= 32; lpe *= 2)
             for (int vpl = 1; vpl <= 4; vpl *= 2) { touch_kernel(pick_lpe<4>(lpe, vpl, halo != 0)); touch_kernel(pick_lpe<1>(lpe, vpl, halo != 0)); }
-    for (int tf = 64; tf <= 256; tf *= 2)
-        for (int halo = 0; halo < 2; ++halo) {
-            for (int shape = 0; shape < 4; ++shape) touch_kernel(pick_ring_tm(tf, shape, halo != 0));
-            for (int shape = 0; shape < 2; ++shape) touch_kernel(pick_ring(tf, shape, 0, halo != 0));
-            if (tf >= 128) touch_kernel(pick_ring(tf, 0, 1, halo != 0));
-        }
+    for_each_ring([](const RingInst& ri) { touch_kernel(ri.fn); return 0; });
     touch_kernel(zero_rows_kernel<4>); touch_kernel(zero_rows_kernel<1>);
     touch_kernel(spmm_fixup_kernel<4>); touch_kernel(spmm_fixup_kernel<1>);
     touch_kernel(pack_rows_kernel<4>); touch_kernel(pack_rows_kernel<1>);
@@ -789,49 +839,71 @@ bool use_ring(const pgcn_plan* p, const float* H0, const float* H1, int f)
     return f % 128 == 0 && aligned16(H0) && aligned16(H1);
 }
 
-// Block size and long-row threshold of matrix c's schedule for the ring (or register) kernel under the current options.
-void sched_params(const pgcn_plan* p, const DevCsr& c, bool ring, int64_t* epb, int64_t* long_row)
+// Opt kernel fn in to its dynamic shared memory (> 48 KB) and record its occupancy at `threads` threads, once per plan;
+// *ctas (when not null) = its CTAs per SM. Setting the attribute is refused while `st` is being captured.
+int opt_in(pgcn_plan* p, const void* fn, size_t smem, int threads, cudaStream_t st, int* ctas)
 {
-    if (ring) {
-        *epb = std::max<int64_t>(c.tuned_epb[1] > 0 ? c.tuned_epb[1] : p->opt_ring_epb, 64);
-        *long_row = p->opt_ring_long > 0 ? p->opt_ring_long : 2 * *epb;
-    } else {
-        *epb = std::max<int64_t>(c.tuned_epb[0] > 0 ? c.tuned_epb[0] : p->opt_epb, 8);
-        *long_row = p->opt_long > 0 ? p->opt_long : 4 * *epb;
+    auto it = p->ctas_per_sm.find(fn);
+    if (it == p->ctas_per_sm.end()) {
+        int rc = refuse_under_capture(p, st);
+        if (rc) return rc;
+        CU(p, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        int nb = 0;
+        CU(p, cudaOccupancyMaxActiveBlocksPerMultiprocessorWithFlags(&nb, fn, threads, smem, 0));
+        it = p->ctas_per_sm.emplace(fn, std::max(nb, 1)).first;
     }
+    if (ctas) *ctas = it->second;
+    return 0;
 }
 
-// A stream under CUDA graph capture takes only stream-ordered work. Set-up that would allocate, copy synchronously or
-// set a function attribute is refused before any such call, so the caller's capture stays valid.
-int refuse_under_capture(pgcn_plan* p, cudaStream_t st)
+// Grid of a register-schedule launch: one group of t.lpe lanes per row block, kSpmmThreads / t.lpe groups per CTA, the
+// row's tiles along y.
+dim3 walk_grid(const DevCsr::Sched& sc, const TileCfg& t)
 {
-    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-    const cudaError_t e = cudaStreamIsCapturing(st, &cs);
-    if (e == cudaSuccess && cs == cudaStreamCaptureStatusNone) return 0;
-    if (e != cudaSuccess) cudaGetLastError();
-    return fail(p, PGCN_ERR_STATE, "this call needs set-up work (schedule upload or kernel attributes) that cannot run "
-                "while the stream is being captured into a CUDA graph: call pgcn_plan_prepare(plan, f) before capturing");
+    const int groups_per_cta = kSpmmThreads / t.lpe;
+    return dim3((unsigned)((sc.nblocks + groups_per_cta - 1) / groups_per_cta), (unsigned)t.tiles);
 }
 
-// Opt a ring kernel instance in to its dynamic shared memory (> 48 KB) and record its occupancy, once per plan.
-int ring_attr(pgcn_plan* p, int tf, int shape, int mode, bool halo, cudaStream_t st, int* slot_out, size_t* smem_out)
+const auto no_setup = [](const DevCsr::Sched&) { return 0; };
+
+// One launch over a schedule of matrix c and the launches around it: the schedule, the caller's setup(sc), the
+// zero-fill of the empty rows (beta == 0), launch(args, sc) over the row blocks, then the fixup of the split rows. All
+// set-up runs before the first launch, so a call refused under capture has enqueued nothing. `a` holds the operands,
+// outputs and epilogue (the schedule's fields are filled in here); vw: the vector width of the zero-fill and fixup.
+template <class Setup, class Launch>
+int launch_walk(pgcn_plan* p, DevCsr& c, bool ring, SpmmArgs a, int vw, cudaStream_t st, Setup setup, Launch launch)
 {
-    const int g = kRingShapes[shape].g, ng = kRingShapes[shape].ng;
-    const size_t smem = ring_smem_bytes(tf, g * ng, ng);
-    const int warps = ring_cta_warps(tf, g * ng, ng);
-    const int tslot = tf == 64 ? 0 : (tf == 128 ? 1 : 2);
-    const int slot = ((tslot * 4 + shape) * 3 + mode) * 2 + (halo ? 1 : 0);
-    if (slot_out) *slot_out = slot;
-    if (smem_out) *smem_out = smem;
-    if (p->ring_attr_set[slot]) return 0;
-    int rc = refuse_under_capture(p, st);
-    if (rc) return rc;
-    const void* fptr = mode == 2 ? (const void*)pick_ring_tm(tf, shape, halo) : (const void*)pick_ring(tf, shape, mode, halo);
-    CU(p, cudaFuncSetAttribute(fptr, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int nb = 0;
-    CU(p, cudaOccupancyMaxActiveBlocksPerMultiprocessorWithFlags(&nb, fptr, warps * 32, smem, 0));
-    p->ring_ctas_per_sm[slot] = std::max(nb, 1);
-    p->ring_attr_set[slot] = true;
+    if (c.nrows == 0) return 0;
+    DevCsr::Sched* sc;
+    int rc;
+    if ((rc = schedule(p, c, ring, st, &sc)) || (rc = setup(*sc))) return rc;
+    if (c.nempty > 0 && !a.beta) {
+        ZeroArgs za;
+        za.rows = c.d_empty; za.nrows_empty = c.nempty; za.Z0 = a.Z0; za.Z1 = a.Z1; za.zsplit = a.zsplit; za.f = a.f;
+        const unsigned grid = (unsigned)(((long long)c.nempty * (a.f / vw) + 255) / 256);
+        if (vw == 4) zero_rows_kernel<4><<<grid, 256, 0, st>>>(za);
+        else zero_rows_kernel<1><<<grid, 256, 0, st>>>(za);
+        ++p->launches;
+    }
+    a.blocks = sc->d_blocks; a.nblocks = sc->nblocks;
+    a.pieces = c.d_cw;
+    a.rowids = c.d_rowids;
+    a.partial = sc->d_partial;
+    if (sc->nblocks > 0) {
+        if ((rc = launch(a, *sc))) return rc;
+        ++p->launches;
+    }
+    if (sc->nlong > 0) {
+        FixupArgs fa;
+        fa.long_rows = sc->d_long; fa.nlong = sc->nlong; fa.partial = sc->d_partial;
+        fa.Z0 = a.Z0; fa.Z1 = a.Z1; fa.zsplit = a.zsplit; fa.rowids = c.d_rowids; fa.f = a.f; fa.beta = a.beta;
+        fa.relu = a.relu; fa.final = a.final;
+        const unsigned grid = (unsigned)sc->nlong * (unsigned)((a.f / vw + 31) / 32);
+        if (vw == 4) spmm_fixup_kernel<4><<<grid, 32 * kFixupGroups, 0, st>>>(fa);
+        else spmm_fixup_kernel<1><<<grid, 32 * kFixupGroups, 0, st>>>(fa);
+        ++p->launches;
+    }
+    CU(p, cudaGetLastError());
     return 0;
 }
 
@@ -851,68 +923,61 @@ int launch_spmm(pgcn_plan* p, DevCsr& c, const float* H0, const float* H1, int s
                 float* Z0, float* Z1, int zsplit, int f, int beta, cudaStream_t st, int relu = 0, bool use_final = false,
                 const float* H_odd = nullptr, const HeadArgs* heads = nullptr)
 {
-    if (c.nrows == 0) return 0;
     const bool ring = !heads && use_ring(p, H0, H1, f) && aligned16(Z0) && aligned16(Z1) && (!H_odd || aligned16(H_odd));
-    int64_t epb, long_row;
-    sched_params(p, c, ring, &epb, &long_row);
-    int rc;
-    if (!sched_ready(c, ring ? 1 : 0, epb, long_row) && (rc = refuse_under_capture(p, st))) return rc;
-    if ((rc = build_schedule(p, c, ring ? 1 : 0, epb, long_row))) return rc;
-    const DevCsr::Sched& sc = c.sched[ring ? 1 : 0];
     // multi-head: 4-float vectors also need whole vectors per head
     const int vw = (heads && (f / heads->nh) % 4 != 0) ? 1 : vec_width(f, {H0, H1, H_odd, Z0, Z1});
-    const TileCfg t = heads ? choose_tile_heads(f, vw) : choose_tile(p, f, vw);
-    if (c.nempty > 0 && !beta) {
-        ZeroArgs za;
-        za.rows = c.d_empty; za.nrows_empty = c.nempty; za.Z0 = Z0; za.Z1 = Z1; za.zsplit = zsplit; za.f = f;
-        const long long total = (long long)c.nempty * (f / t.vw);
-        const unsigned grid = (unsigned)((total + 255) / 256);
-        if (t.vw == 4) zero_rows_kernel<4><<<grid, 256, 0, st>>>(za);
-        else zero_rows_kernel<1><<<grid, 256, 0, st>>>(za);
-        ++p->launches;
-    }
-    SpmmArgs a;
-    a.blocks = sc.d_blocks; a.nblocks = sc.nblocks;
-    a.pieces = c.d_cw;
+    const bool halo = (H1 != nullptr);
+    SpmmArgs a = {};
     a.H0 = H0; a.H1 = H1; a.split = split;
     a.Z0 = Z0; a.Z1 = Z1; a.zsplit = zsplit;
-    a.rowids = c.d_rowids;
-    a.partial = sc.d_partial; a.f = f; a.beta = beta;
+    a.f = f; a.beta = beta;
     a.relu = relu; a.final = (relu && use_final) ? c.d_final : nullptr;
     a.H_odd = H_odd; a.epoch = H_odd ? p->d_epoch : nullptr;
-    if (sc.nblocks > 0 && ring) {
-        int mode = p->opt_kernel == 6 ? 1 : (p->opt_kernel == 5 ? 0 : 2);   // default: 2-D tensor-map TMA
-        // row tile: the option, else the tuned width, else the full width (256 floats when f allows, else 128);
-        // a width that does not divide f, and 64-float slices with the cp.async fill, take the full width
-        const int full = (f % 256 == 0) ? 256 : 128;
-        int tf = (int)(p->opt_ring_tile > 0 ? p->opt_ring_tile : (c.tuned_tile > 0 ? c.tuned_tile : full));
-        if (f % tf != 0 || (mode == 1 && tf < 128)) tf = full;
-        const int tiles = f / tf;
-        const bool halo = (H1 != nullptr);
-        // ring shape from the options: ring_slots = 16 | 32 | 64, ring_groups = 2 | 4 (only with 64 slots)
-        const int64_t want_slots = c.tuned_slots > 0 ? c.tuned_slots : p->opt_ring_slots;
-        int shape = want_slots <= 16 ? 0 : (want_slots <= 32 ? 1 : (p->opt_ring_groups == 4 ? 3 : 2));
-        CUtensorMap tm0, tm1, tm_odd;
-        if (mode == 2) {
-            // H0 holds the columns below `split` (all of them when there is no halo slab), H1 the rest
-            bool ok = make_row_map(&tm0, H0, 1 << 30, f, tf, 1);
-            if (ok && H1) ok = make_row_map(&tm1, H1, 1 << 30, f, tf, 1);
-            else if (ok) tm1 = tm0;
-            if (ok && H_odd) ok = make_row_map(&tm_odd, H_odd, 1 << 30, f, tf, 1);
-            else if (ok) tm_odd = tm1;
-            if (!ok) mode = 0;                                   // no driver entry point: 1-D bulk copies
-        }
-        if (mode == 1) shape = 0;
-        if (mode == 0 && shape > 1) shape = 1;
-        ring_fn fn = mode == 2 ? nullptr : pick_ring(tf, shape, mode, halo);
-        ring_tm_fn fn_tm = mode == 2 ? pick_ring_tm(tf, shape, halo) : nullptr;
-        int slot = 0;
-        size_t smem = 0;
-        if ((rc = ring_attr(p, tf, shape, mode, halo, st, &slot, &smem))) return rc;
+    if (!ring) {
+        const TileCfg t = heads ? choose_tile_heads(f, vw) : choose_tile(p, f, vw);
+        return launch_walk(p, c, false, a, vw, st, no_setup, [&](const SpmmArgs& args, const DevCsr::Sched& sc) {
+            if (heads) {
+                SpmmHeadArgs ha;
+                ha.alpha = heads->alpha; ha.amap = heads->map; ha.hd = f / heads->nh;
+                pick_heads(t.lpe, t.vw, halo, heads->nh)<<<walk_grid(sc, t), kSpmmThreads, 0, st>>>(args, ha);
+            } else {
+                spmm_fn fn = (t.vw == 4) ? pick_lpe<4>(t.lpe, t.vpl, halo) : pick_lpe<1>(t.lpe, t.vpl, halo);
+                fn<<<walk_grid(sc, t), kSpmmThreads, 0, st>>>(args);
+            }
+            return 0;
+        });
+    }
+    int mode = p->opt_kernel == 6 ? 1 : (p->opt_kernel == 5 ? 0 : 2);   // default: 2-D tensor-map TMA
+    // row tile: the option, else the tuned width, else the full width (256 floats when f allows, else 128);
+    // a width that does not divide f, and 64-float slices with the cp.async fill, take the full width
+    const int full = (f % 256 == 0) ? 256 : 128;
+    int tf = (int)(p->opt_ring_tile > 0 ? p->opt_ring_tile : (c.tuned_tile > 0 ? c.tuned_tile : full));
+    if (f % tf != 0 || (mode == 1 && tf < 128)) tf = full;
+    const int tiles = f / tf;
+    // ring shape from the options: ring_slots = 16 | 32 | 64, ring_groups = 2 | 4 (only with 64 slots)
+    const int64_t want_slots = c.tuned_slots > 0 ? c.tuned_slots : p->opt_ring_slots;
+    int shape = want_slots <= 16 ? 0 : (want_slots <= 32 ? 1 : (p->opt_ring_groups == 4 ? 3 : 2));
+    CUtensorMap tm0, tm1, tm_odd;
+    if (mode == 2) {
+        // H0 holds the columns below `split` (all of them when there is no halo slab), H1 the rest
+        bool ok = make_row_map(&tm0, H0, 1 << 30, f, tf, 1);
+        if (ok && H1) ok = make_row_map(&tm1, H1, 1 << 30, f, tf, 1);
+        else if (ok) tm1 = tm0;
+        if (ok && H_odd) ok = make_row_map(&tm_odd, H_odd, 1 << 30, f, tf, 1);
+        else if (ok) tm_odd = tm1;
+        if (!ok) mode = 0;                                   // no driver entry point: 1-D bulk copies
+    }
+    if (mode == 1) shape = 0;
+    if (mode == 0 && shape > 1) shape = 1;
+    const RingInst ri = ring_inst(tf, shape, mode, halo);
+    int ctas = 0;
+    auto setup = [&](const DevCsr::Sched& sc) {
+        return sc.nblocks > 0 ? opt_in(p, ri.fn, ri.smem, ri.warps * 32, st, &ctas) : 0;
+    };
+    return launch_walk(p, c, true, a, vw, st, setup, [&](const SpmmArgs& args, const DevCsr::Sched& sc) -> int {
         RingArgs ra;
         ra.counter = nullptr; ra.hub = nullptr; ra.nhub = 0;
-        const int warps = ring_cta_warps(tf, kRingShapes[shape].g * kRingShapes[shape].ng, kRingShapes[shape].ng);
-        dim3 grid((unsigned)((sc.nblocks + warps - 1) / warps), (unsigned)tiles);
+        dim3 grid((unsigned)((sc.nblocks + ri.warps - 1) / ri.warps), (unsigned)tiles);
         // Persistent CTAs own their SM (shared memory + registers) until the whole launch is done; a put / NCCL kernel
         // of the exchange stream would then wait behind the SpMM it is supposed to overlap (measured at 8 GPUs: step =
         // sum of puts + sum of SpMMs). Multi-rank plans with overlap therefore run one block per warp (CTAs retire
@@ -923,40 +988,14 @@ int launch_spmm(pgcn_plan* p, DevCsr& c, const float* H0, const float* H1, int s
             // one counter over all (tile, row block) items, tile-major: the tiles run one after the other
             CU(p, cudaMemsetAsync(p->d_counter, 0, sizeof(unsigned int), st));
             ra.counter = p->d_counter;
-            const unsigned items = (unsigned)(((int64_t)sc.nblocks * tiles + warps - 1) / warps);
-            grid.x = std::min<unsigned>(items, (unsigned)(p->num_sms * p->ring_ctas_per_sm[slot]));
+            const unsigned items = (unsigned)(((int64_t)sc.nblocks * tiles + ri.warps - 1) / ri.warps);
+            grid.x = std::min<unsigned>(items, (unsigned)(p->num_sms * ctas));
             grid.y = 1;
         }
-        if (mode == 2) fn_tm<<<grid, warps * 32, smem, st>>>(a, ra, tm0, tm1, tm_odd);
-        else fn<<<grid, warps * 32, smem, st>>>(a, ra);
-        ++p->launches;
-    } else if (sc.nblocks > 0) {
-        const int groups_per_cta = kSpmmThreads / t.lpe;
-        dim3 grid((unsigned)((sc.nblocks + groups_per_cta - 1) / groups_per_cta), (unsigned)t.tiles);
-        const bool halo = (H1 != nullptr);
-        if (heads) {
-            SpmmHeadArgs ha;
-            ha.alpha = heads->alpha; ha.amap = heads->map; ha.hd = f / heads->nh;
-            pick_heads(t.lpe, t.vw, halo, heads->nh)<<<grid, kSpmmThreads, 0, st>>>(a, ha);
-        } else {
-            spmm_fn fn = (t.vw == 4) ? pick_lpe<4>(t.lpe, t.vpl, halo) : pick_lpe<1>(t.lpe, t.vpl, halo);
-            fn<<<grid, kSpmmThreads, 0, st>>>(a);
-        }
-        ++p->launches;
-    }
-    if (sc.nlong > 0) {
-        FixupArgs fa;
-        fa.long_rows = sc.d_long; fa.nlong = sc.nlong; fa.partial = sc.d_partial;
-        fa.Z0 = Z0; fa.Z1 = Z1; fa.zsplit = zsplit; fa.rowids = c.d_rowids; fa.f = f; fa.beta = beta;
-        fa.relu = a.relu; fa.final = a.final;
-        const int nvec = f / t.vw;
-        const unsigned grid = (unsigned)sc.nlong * (unsigned)((nvec + 31) / 32);
-        if (t.vw == 4) spmm_fixup_kernel<4><<<grid, 32 * kFixupGroups, 0, st>>>(fa);
-        else spmm_fixup_kernel<1><<<grid, 32 * kFixupGroups, 0, st>>>(fa);
-        ++p->launches;
-    }
-    CU(p, cudaGetLastError());
-    return 0;
+        if (mode == 2) pick_ring_tm(tf, shape, halo)<<<grid, ri.warps * 32, ri.smem, st>>>(args, ra, tm0, tm1, tm_odd);
+        else pick_ring(tf, shape, mode, halo)<<<grid, ri.warps * 32, ri.smem, st>>>(args, ra);
+        return 0;
+    });
 }
 
 int check_f(pgcn_plan* p, int f)
@@ -1024,13 +1063,9 @@ int launch_max(pgcn_plan* p, const float* H0, const float* H1, const float* H_od
 {
     DevCsr& c = p->fwd;
     if (c.nrows == 0) return 0;
-    int64_t epb, long_row;
-    sched_params(p, c, false, &epb, &long_row);
+    DevCsr::Sched* sc;
     int rc;
-    if (!sched_ready(c, 0, epb, long_row) && (rc = refuse_under_capture(p, st))) return rc;
-    if ((rc = build_schedule(p, c, 0, epb, long_row))) return rc;
-    DevCsr::Sched& sc = c.sched[0];
-    if ((rc = max_partial(p, sc, st))) return rc;
+    if ((rc = schedule(p, c, false, st, &sc)) || (rc = max_partial(p, *sc, st))) return rc;
     const int vw = vec_width(f, {H0, H1, H_odd, Z, arg});
     const TileCfg t = choose_tile_heads(f, vw);
     if (c.nempty > 0) {
@@ -1041,26 +1076,24 @@ int launch_max(pgcn_plan* p, const float* H0, const float* H1, const float* H_od
         else max_empty_rows_kernel<1><<<grid, 256, 0, st>>>(za);
         ++p->launches;
     }
-    if (sc.nblocks > 0) {
+    if (sc->nblocks > 0) {
         SpmmArgs a;
-        a.blocks = sc.d_blocks; a.nblocks = sc.nblocks;
+        a.blocks = sc->d_blocks; a.nblocks = sc->nblocks;
         a.pieces = c.d_cw;
         a.H0 = H0; a.H1 = H1; a.split = p->m;
         a.Z0 = Z; a.Z1 = nullptr; a.zsplit = p->m;
         a.rowids = c.d_rowids;
-        a.partial = sc.d_partial; a.f = f; a.beta = 0;
+        a.partial = sc->d_partial; a.f = f; a.beta = 0;
         a.relu = 0; a.final = nullptr;
         a.H_odd = H_odd; a.epoch = H_odd ? p->d_epoch : nullptr;
-        const int groups_per_cta = kSpmmThreads / t.lpe;
-        dim3 grid((unsigned)((sc.nblocks + groups_per_cta - 1) / groups_per_cta), (unsigned)t.tiles);
-        pick_max(t.lpe, vw, H1 != nullptr)<<<grid, kSpmmThreads, 0, st>>>(a, arg, sc.d_apart);
+        pick_max(t.lpe, vw, H1 != nullptr)<<<walk_grid(*sc, t), kSpmmThreads, 0, st>>>(a, arg, sc->d_apart);
         ++p->launches;
     }
-    if (sc.nlong > 0) {
+    if (sc->nlong > 0) {
         MaxFixupArgs fa;
-        fa.long_rows = sc.d_long; fa.partial = sc.d_partial; fa.apart = sc.d_apart;
+        fa.long_rows = sc->d_long; fa.partial = sc->d_partial; fa.apart = sc->d_apart;
         fa.Z = Z; fa.arg = arg; fa.rowids = c.d_rowids; fa.f = f;
-        const unsigned grid = (unsigned)sc.nlong * (unsigned)((f / vw + 31) / 32);
+        const unsigned grid = (unsigned)sc->nlong * (unsigned)((f / vw + 31) / 32);
         if (vw == 4) spmm_max_fixup_kernel<4><<<grid, 32 * kFixupGroups, 0, st>>>(fa);
         else spmm_max_fixup_kernel<1><<<grid, 32 * kFixupGroups, 0, st>>>(fa);
         ++p->launches;
@@ -1072,51 +1105,16 @@ int launch_max(pgcn_plan* p, const float* H0, const float* H1, const float* H_od
 // G_own (rows [0, m)) and G_halo (rows [m, m + h)) = gZ routed by arg, on the register schedule of the transposed records.
 int launch_max_backward(pgcn_plan* p, const int* arg, const float* gZ, float* G_own, float* G_halo, int f, cudaStream_t st)
 {
-    DevCsr& c = p->tr;
-    if (c.nrows == 0) return 0;
-    int64_t epb, long_row;
-    sched_params(p, c, false, &epb, &long_row);
-    int rc;
-    if (!sched_ready(c, 0, epb, long_row) && (rc = refuse_under_capture(p, st))) return rc;
-    if ((rc = build_schedule(p, c, 0, epb, long_row))) return rc;
-    const DevCsr::Sched& sc = c.sched[0];
     const int vw = vec_width(f, {gZ, arg, G_own, G_halo});
     const TileCfg t = choose_tile_heads(f, vw);
-    if (c.nempty > 0) {
-        ZeroArgs za;
-        za.rows = c.d_empty; za.nrows_empty = c.nempty; za.Z0 = G_own; za.Z1 = G_halo; za.zsplit = p->m; za.f = f;
-        const unsigned grid = (unsigned)(((long long)c.nempty * (f / vw) + 255) / 256);
-        if (vw == 4) zero_rows_kernel<4><<<grid, 256, 0, st>>>(za);
-        else zero_rows_kernel<1><<<grid, 256, 0, st>>>(za);
-        ++p->launches;
-    }
-    if (sc.nblocks > 0) {
-        SpmmArgs a;
-        a.blocks = sc.d_blocks; a.nblocks = sc.nblocks;
-        a.pieces = c.d_cw;
-        a.H0 = gZ; a.H1 = nullptr; a.split = p->m;
-        a.Z0 = G_own; a.Z1 = G_halo; a.zsplit = p->m;
-        a.rowids = c.d_rowids;
-        a.partial = sc.d_partial; a.f = f; a.beta = 0;
-        a.relu = 0; a.final = nullptr;
-        a.H_odd = nullptr; a.epoch = nullptr;
-        const int groups_per_cta = kSpmmThreads / t.lpe;
-        dim3 grid((unsigned)((sc.nblocks + groups_per_cta - 1) / groups_per_cta), (unsigned)t.tiles);
-        pick_max_bwd(t.lpe, vw)<<<grid, kSpmmThreads, 0, st>>>(a, arg, c.d_vmap);
-        ++p->launches;
-    }
-    if (sc.nlong > 0) {
-        FixupArgs fa;
-        fa.long_rows = sc.d_long; fa.nlong = sc.nlong; fa.partial = sc.d_partial;
-        fa.Z0 = G_own; fa.Z1 = G_halo; fa.zsplit = p->m; fa.rowids = c.d_rowids; fa.f = f; fa.beta = 0;
-        fa.relu = 0; fa.final = nullptr;
-        const unsigned grid = (unsigned)sc.nlong * (unsigned)((f / vw + 31) / 32);
-        if (vw == 4) spmm_fixup_kernel<4><<<grid, 32 * kFixupGroups, 0, st>>>(fa);
-        else spmm_fixup_kernel<1><<<grid, 32 * kFixupGroups, 0, st>>>(fa);
-        ++p->launches;
-    }
-    CU(p, cudaGetLastError());
-    return 0;
+    SpmmArgs a = {};
+    a.H0 = gZ; a.split = p->m;
+    a.Z0 = G_own; a.Z1 = G_halo; a.zsplit = p->m;
+    a.f = f;
+    return launch_walk(p, p->tr, false, a, vw, st, no_setup, [&](const SpmmArgs& args, const DevCsr::Sched& sc) {
+        pick_max_bwd(t.lpe, vw)<<<walk_grid(sc, t), kSpmmThreads, 0, st>>>(args, arg, p->tr.d_vmap);
+        return 0;
+    });
 }
 
 // ---- edge values -----------------------------------------------------------------------------
@@ -1137,56 +1135,53 @@ bool sddmm_use_ring(const pgcn_plan* p, const float* gZ, const float* H0, const 
     return use_ring(p, gZ, H0, f) && f <= 512 && (!H1 || aligned16(H1));
 }
 
-// Opt the SDDMM ring instance of width f in to its dynamic shared memory and record its occupancy, once per plan.
-int sddmm_attr(pgcn_plan* p, int f, cudaStream_t st)
+// The edge launch over the forward records shared by the SDDMM, the multi-head SDDMM and the GATv2 scores: gZ is the
+// row operand, H0 / H1 the column operands (H1: the halo rows, columns >= m), out takes the values of the entries.
+// On the ring schedule, persistent CTAs of ring_fn (its shared memory of width f opted in) take row blocks from the
+// plan's counter; on the register schedule, the plain kernel takes 8 row blocks per CTA. launch(args, grid, threads,
+// smem) launches ring_fn or the plain kernel with the call's further arguments.
+template <class Launch>
+int launch_edges(pgcn_plan* p, bool ring, const void* ring_fn, const float* gZ, const float* H0, const float* H1,
+                 float* out, int f, cudaStream_t st, Launch launch)
 {
-    const int nv = f / 128;
-    if (p->sddmm_attr_set[nv]) return 0;
-    int rc = refuse_under_capture(p, st);
-    if (rc) return rc;
-    const void* fptr = (const void*)pick_sddmm(nv);
-    const size_t smem = sddmm_smem_bytes(nv);
-    CU(p, cudaFuncSetAttribute(fptr, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int nb = 0;
-    CU(p, cudaOccupancyMaxActiveBlocksPerMultiprocessorWithFlags(&nb, fptr, kSddmmWarps * 32, smem, 0));
-    p->sddmm_ctas_per_sm[nv] = std::max(nb, 1);
-    p->sddmm_attr_set[nv] = true;
+    DevCsr& c = p->fwd;
+    if (c.nnz == 0 || c.nrows == 0) return 0;
+    DevCsr::Sched* sc;
+    int rc = schedule(p, c, ring, st, &sc);
+    if (rc || sc->nblocks == 0) return rc;
+    SddmmArgs a;
+    a.blocks = sc->d_blocks; a.nblocks = sc->nblocks;
+    a.pieces = c.d_cw;
+    a.gZ = gZ; a.H0 = H0; a.H1 = H1; a.split = p->m;
+    a.rowids = c.d_rowids;
+    a.dvals = out; a.f = f;
+    a.counter = nullptr;
+    if (ring) {
+        const size_t smem = sddmm_smem_bytes(f / 128);
+        int ctas = 0;
+        if ((rc = opt_in(p, ring_fn, smem, kSddmmWarps * 32, st, &ctas))) return rc;
+        CU(p, cudaMemsetAsync(p->d_counter, 0, sizeof(unsigned int), st));
+        a.counter = p->d_counter;
+        const unsigned nctas = (unsigned)((sc->nblocks + kSddmmWarps - 1) / kSddmmWarps);
+        launch(a, std::min<unsigned>(nctas, (unsigned)(p->num_sms * ctas)), kSddmmWarps * 32, smem);
+    } else {
+        launch(a, (unsigned)((sc->nblocks + 7) / 8), 256, (size_t)0);
+    }
+    ++p->launches;
+    CU(p, cudaGetLastError());
     return 0;
 }
 
 // dvals = SDDMM over the forward matrix (H1: the halo rows, columns >= m)
 int launch_sddmm(pgcn_plan* p, const float* gZ, const float* H0, const float* H1, float* dvals, int f, cudaStream_t st)
 {
-    DevCsr& c = p->fwd;
-    if (c.nnz == 0 || c.nrows == 0) return 0;
     const bool ring = sddmm_use_ring(p, gZ, H0, H1, f);
-    int64_t epb, long_row;
-    sched_params(p, c, ring, &epb, &long_row);
-    int rc;
-    if (!sched_ready(c, ring ? 1 : 0, epb, long_row) && (rc = refuse_under_capture(p, st))) return rc;
-    if ((rc = build_schedule(p, c, ring ? 1 : 0, epb, long_row))) return rc;
-    const DevCsr::Sched& sc = c.sched[ring ? 1 : 0];
-    SddmmArgs a;
-    a.blocks = sc.d_blocks; a.nblocks = sc.nblocks;
-    a.pieces = c.d_cw;
-    a.gZ = gZ; a.H0 = H0; a.H1 = H1; a.split = p->m;
-    a.rowids = c.d_rowids;
-    a.dvals = dvals; a.f = f;
-    a.counter = nullptr;
-    if (sc.nblocks == 0) return 0;
-    if (ring) {
-        if ((rc = sddmm_attr(p, f, st))) return rc;
-        CU(p, cudaMemsetAsync(p->d_counter, 0, sizeof(unsigned int), st));
-        a.counter = p->d_counter;
-        const unsigned ctas = (unsigned)((sc.nblocks + kSddmmWarps - 1) / kSddmmWarps);
-        const unsigned grid = std::min<unsigned>(ctas, (unsigned)(p->num_sms * p->sddmm_ctas_per_sm[f / 128]));
-        pick_sddmm(f / 128)<<<grid, kSddmmWarps * 32, sddmm_smem_bytes(f / 128), st>>>(a);
-    } else {
-        sddmm_plain_kernel<<<(unsigned)((sc.nblocks + 7) / 8), 256, 0, st>>>(a);
-    }
-    ++p->launches;
-    CU(p, cudaGetLastError());
-    return 0;
+    const sddmm_fn fn = pick_sddmm(f / 128);
+    return launch_edges(p, ring, (const void*)fn, gZ, H0, H1, dvals, f, st,
+                        [&](const SddmmArgs& a, unsigned grid, int threads, size_t smem) {
+        if (ring) fn<<<grid, threads, smem, st>>>(a);
+        else sddmm_plain_kernel<<<grid, threads, smem, st>>>(a);
+    });
 }
 
 // The multi-head SDDMM ring instance serves f = 128, 256 or 512 with 2, 4 or 8 heads of at least 4 floats and 16-byte
@@ -1196,58 +1191,18 @@ bool sddmm_heads_use_ring(const pgcn_plan* p, const float* gZ, const float* H0, 
     return k > 1 && (f == 128 || f == 256 || f == 512) && (f / k) % 4 == 0 && sddmm_use_ring(p, gZ, H0, H1, f);
 }
 
-int sddmm_heads_attr(pgcn_plan* p, int f, int k, cudaStream_t st)
-{
-    const int nv = f / 128;
-    if (p->sddmm_heads_attr_set[nv][k]) return 0;
-    int rc = refuse_under_capture(p, st);
-    if (rc) return rc;
-    const void* fptr = (const void*)pick_sddmm_heads(nv, k);
-    const size_t smem = sddmm_smem_bytes(nv);
-    CU(p, cudaFuncSetAttribute(fptr, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int nb = 0;
-    CU(p, cudaOccupancyMaxActiveBlocksPerMultiprocessorWithFlags(&nb, fptr, kSddmmWarps * 32, smem, 0));
-    p->sddmm_heads_ctas_per_sm[nv][k] = std::max(nb, 1);
-    p->sddmm_heads_attr_set[nv][k] = true;
-    return 0;
-}
-
 // dalpha (nnz x k) = the SDDMM per head over the forward matrix; k == 1 is launch_sddmm
 int launch_sddmm_heads(pgcn_plan* p, int k, const float* gZ, const float* H0, const float* H1, float* dalpha, int f,
                        cudaStream_t st)
 {
     if (k == 1) return launch_sddmm(p, gZ, H0, H1, dalpha, f, st);
-    DevCsr& c = p->fwd;
-    if (c.nnz == 0 || c.nrows == 0) return 0;
     const bool ring = sddmm_heads_use_ring(p, gZ, H0, H1, f, k);
-    int64_t epb, long_row;
-    sched_params(p, c, ring, &epb, &long_row);
-    int rc;
-    if (!sched_ready(c, ring ? 1 : 0, epb, long_row) && (rc = refuse_under_capture(p, st))) return rc;
-    if ((rc = build_schedule(p, c, ring ? 1 : 0, epb, long_row))) return rc;
-    const DevCsr::Sched& sc = c.sched[ring ? 1 : 0];
-    SddmmArgs a;
-    a.blocks = sc.d_blocks; a.nblocks = sc.nblocks;
-    a.pieces = c.d_cw;
-    a.gZ = gZ; a.H0 = H0; a.H1 = H1; a.split = p->m;
-    a.rowids = c.d_rowids;
-    a.dvals = dalpha; a.f = f;
-    a.counter = nullptr;
-    if (sc.nblocks == 0) return 0;
-    if (ring) {
-        const int nv = f / 128;
-        if ((rc = sddmm_heads_attr(p, f, k, st))) return rc;
-        CU(p, cudaMemsetAsync(p->d_counter, 0, sizeof(unsigned int), st));
-        a.counter = p->d_counter;
-        const unsigned ctas = (unsigned)((sc.nblocks + kSddmmWarps - 1) / kSddmmWarps);
-        const unsigned grid = std::min<unsigned>(ctas, (unsigned)(p->num_sms * p->sddmm_heads_ctas_per_sm[nv][k]));
-        pick_sddmm_heads(nv, k)<<<grid, kSddmmWarps * 32, sddmm_smem_bytes(nv), st>>>(a);
-    } else {
-        sddmm_plain_heads_kernel<<<(unsigned)((sc.nblocks + 7) / 8), 256, 0, st>>>(a, k);
-    }
-    ++p->launches;
-    CU(p, cudaGetLastError());
-    return 0;
+    const sddmm_fn fn = pick_sddmm_heads(f / 128, k);
+    return launch_edges(p, ring, (const void*)fn, gZ, H0, H1, dalpha, f, st,
+                        [&](const SddmmArgs& a, unsigned grid, int threads, size_t smem) {
+        if (ring) fn<<<grid, threads, smem, st>>>(a);
+        else sddmm_plain_heads_kernel<<<grid, threads, smem, st>>>(a, k);
+    });
 }
 
 // ---- GATv2 ----------------------------------------------------------------------------------
@@ -1272,108 +1227,34 @@ bool gatv2_use_ring(const pgcn_plan* p, const float* xr, const float* xl, const 
     return (f == 128 || f == 256) && sddmm_use_ring(p, xr, xl, H1, f) && aligned16(H1_odd) && aligned16(att);
 }
 
-int gatv2_attr(pgcn_plan* p, int f, int k, cudaStream_t st)
-{
-    const int nv = f / 128;
-    if (p->gatv2_attr_set[nv][k]) return 0;
-    int rc = refuse_under_capture(p, st);
-    if (rc) return rc;
-    const void* fptr = (const void*)pick_gatv2_ring(nv, k);
-    const size_t smem = sddmm_smem_bytes(nv);
-    CU(p, cudaFuncSetAttribute(fptr, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int nb = 0;
-    CU(p, cudaOccupancyMaxActiveBlocksPerMultiprocessorWithFlags(&nb, fptr, kSddmmWarps * 32, smem, 0));
-    p->gatv2_ctas_per_sm[nv][k] = std::max(nb, 1);
-    p->gatv2_attr_set[nv][k] = true;
-    return 0;
-}
-
 // scores (nnz x k, forward CSR order) of the forward records, written into `out`; H1 / H1_odd: the halo slab of the
 // call and its odd-epoch twin on the peer transport (or null)
 int launch_gatv2_score(pgcn_plan* p, int k, const float* xr, const float* xl, const float* H1, const float* H1_odd,
                        const float* att, float slope, float* out, int f, cudaStream_t st)
 {
-    DevCsr& c = p->fwd;
-    if (c.nnz == 0 || c.nrows == 0) return 0;
     const bool ring = gatv2_use_ring(p, xr, xl, H1, H1_odd, att, f);
-    int64_t epb, long_row;
-    sched_params(p, c, ring, &epb, &long_row);
-    int rc;
-    if (!sched_ready(c, ring ? 1 : 0, epb, long_row) && (rc = refuse_under_capture(p, st))) return rc;
-    if ((rc = build_schedule(p, c, ring ? 1 : 0, epb, long_row))) return rc;
-    const DevCsr::Sched& sc = c.sched[ring ? 1 : 0];
-    if (sc.nblocks == 0) return 0;
-    SddmmArgs a;
-    a.blocks = sc.d_blocks; a.nblocks = sc.nblocks;
-    a.pieces = c.d_cw;
-    a.gZ = xr; a.H0 = xl; a.H1 = H1; a.split = p->m;
-    a.rowids = c.d_rowids;
-    a.dvals = out; a.f = f;
-    a.counter = nullptr;
+    const gatv2_score_fn fn = pick_gatv2_ring(f / 128, k);
     const Gatv2Halo hl = {H1_odd, H1_odd ? p->d_epoch : nullptr};
-    if (ring) {
-        const int nv = f / 128;
-        if ((rc = gatv2_attr(p, f, k, st))) return rc;
-        CU(p, cudaMemsetAsync(p->d_counter, 0, sizeof(unsigned int), st));
-        a.counter = p->d_counter;
-        const unsigned ctas = (unsigned)((sc.nblocks + kSddmmWarps - 1) / kSddmmWarps);
-        const unsigned grid = std::min<unsigned>(ctas, (unsigned)(p->num_sms * p->gatv2_ctas_per_sm[nv][k]));
-        pick_gatv2_ring(nv, k)<<<grid, kSddmmWarps * 32, sddmm_smem_bytes(nv), st>>>(a, hl, att, slope);
-    } else {
-        gatv2_score_plain_kernel<<<(unsigned)((sc.nblocks + 7) / 8), 256, 0, st>>>(a, hl, att, slope, k);
-    }
-    ++p->launches;
-    CU(p, cudaGetLastError());
-    return 0;
+    return launch_edges(p, ring, (const void*)fn, xr, xl, H1, out, f, st,
+                        [&](const SddmmArgs& a, unsigned grid, int threads, size_t smem) {
+        if (ring) fn<<<grid, threads, smem, st>>>(a, hl, att, slope);
+        else gatv2_score_plain_kernel<<<grid, threads, smem, st>>>(a, hl, att, slope, k);
+    });
 }
 
 // One of the two backward walks on the register schedule of c (the forward records: dxr and the datt partials; the
 // transposed ones: dxl and the halo partials), its empty rows and its split rows. vw: as the multi-head aggregation.
-int launch_gatv2_walk(pgcn_plan* p, DevCsr& c, bool col, int k, const SpmmArgs& a0, Gatv2BwdArgs g,
+int launch_gatv2_walk(pgcn_plan* p, DevCsr& c, bool col, int k, const SpmmArgs& a, Gatv2BwdArgs g,
                       std::initializer_list<const void*> ops, cudaStream_t st)
 {
-    const int f = a0.f;
-    int64_t epb, long_row;
-    sched_params(p, c, false, &epb, &long_row);
-    int rc;
-    if (!sched_ready(c, 0, epb, long_row) && (rc = refuse_under_capture(p, st))) return rc;
-    if ((rc = build_schedule(p, c, 0, epb, long_row))) return rc;
-    DevCsr::Sched& sc = c.sched[0];
-    if (!col && (rc = gatv2_partial(p, sc, st))) return rc;
-    const int vw = (f / k) % 4 != 0 ? 1 : vec_width(f, ops);
-    const TileCfg t = choose_tile_heads(f, vw);
-    if (c.nempty > 0) {
-        ZeroArgs za;
-        za.rows = c.d_empty; za.nrows_empty = c.nempty; za.Z0 = a0.Z0; za.Z1 = a0.Z1; za.zsplit = a0.zsplit; za.f = f;
-        const unsigned grid = (unsigned)(((long long)c.nempty * (f / vw) + 255) / 256);
-        if (vw == 4) zero_rows_kernel<4><<<grid, 256, 0, st>>>(za);
-        else zero_rows_kernel<1><<<grid, 256, 0, st>>>(za);
-        ++p->launches;
-    }
-    if (sc.nblocks > 0) {
-        SpmmArgs a = a0;
-        a.blocks = sc.d_blocks; a.nblocks = sc.nblocks;
-        a.pieces = c.d_cw;
-        a.rowids = c.d_rowids;
-        a.partial = sc.d_partial;
+    const int vw = (a.f / k) % 4 != 0 ? 1 : vec_width(a.f, ops);
+    const TileCfg t = choose_tile_heads(a.f, vw);
+    auto setup = [&](DevCsr::Sched& sc) { return col ? 0 : gatv2_partial(p, sc, st); };
+    return launch_walk(p, c, false, a, vw, st, setup, [&](const SpmmArgs& args, const DevCsr::Sched& sc) {
         g.datt_part = sc.d_datt;
-        const int groups_per_cta = kSpmmThreads / t.lpe;
-        dim3 grid((unsigned)((sc.nblocks + groups_per_cta - 1) / groups_per_cta), (unsigned)t.tiles);
-        pick_gatv2_bwd(t.lpe, vw, k, col, a.H1 != nullptr)<<<grid, kSpmmThreads, 0, st>>>(a, g);
-        ++p->launches;
-    }
-    if (sc.nlong > 0) {
-        FixupArgs fa;
-        fa.long_rows = sc.d_long; fa.nlong = sc.nlong; fa.partial = sc.d_partial;
-        fa.Z0 = a0.Z0; fa.Z1 = a0.Z1; fa.zsplit = a0.zsplit; fa.rowids = c.d_rowids; fa.f = f; fa.beta = 0;
-        fa.relu = 0; fa.final = nullptr;
-        const unsigned grid = (unsigned)sc.nlong * (unsigned)((f / vw + 31) / 32);
-        if (vw == 4) spmm_fixup_kernel<4><<<grid, 32 * kFixupGroups, 0, st>>>(fa);
-        else spmm_fixup_kernel<1><<<grid, 32 * kFixupGroups, 0, st>>>(fa);
-        ++p->launches;
-    }
-    CU(p, cudaGetLastError());
-    return 0;
+        pick_gatv2_bwd(t.lpe, vw, k, col, args.H1 != nullptr)<<<walk_grid(sc, t), kSpmmThreads, 0, st>>>(args, g);
+        return 0;
+    });
 }
 
 // dxr (m x f) and datt (f) from dscore (nnz x k) on the forward records
@@ -1540,6 +1421,129 @@ int advance_epoch(pgcn_plan* p, cudaStream_t st)
     ++p->launches;
     CU(p, cudaGetLastError());
     return 0;
+}
+
+// The transport of a multi-rank call at width f, and the slabs its exchanges land in: the peer transport when it is set
+// up and the rows are whole 16-byte vectors (its slabs are double-buffered: the _odd twin serves odd exchange epochs),
+// else NCCL, which needs pgcn_comm_init, into the plan's own slabs.
+struct Transport {
+    bool p2p;
+    float* halo; const float* halo_odd;       // forward: the halo rows
+    float* rrecv; const float* rrecv_odd;     // backward: the partials the peers send back
+};
+
+int transport(pgcn_plan* p, int f, Transport* x)
+{
+    x->p2p = p->p2p && f % 4 == 0;
+    if (!x->p2p && !p->comm) return fail(p, PGCN_ERR_STATE, "k=%d: call pgcn_comm_init or pgcn_p2p_import first", p->k);
+    x->halo = x->p2p ? arena_ptr(p->arena, p->off_fwd[0]) : p->d_halo_slab;
+    x->halo_odd = x->p2p ? arena_ptr(p->arena, p->off_fwd[1]) : nullptr;
+    x->rrecv = x->p2p ? arena_ptr(p->arena, p->off_bwd[0]) : p->d_rrecv_slab;
+    x->rrecv_odd = x->p2p ? arena_ptr(p->arena, p->off_bwd[1]) : nullptr;
+    return 0;
+}
+
+// Exchange schedule shared by both transports and both directions: at step i = 1 .. k-1 a rank sends to
+// (rank + i) % k and receives from (rank - i) % k — every pair is active exactly once per step, and a receiver
+// sees its sources arrive one after the other, so each block can be consumed while the next is in flight.
+inline int step_dst(const pgcn_plan* p, int i) { return (p->rank + i) % p->k; }
+inline int step_src(const pgcn_plan* p, int i) { return (p->rank - i + p->k) % p->k; }
+
+int nccl_step(pgcn_plan* p, const float* send, float* recv, int f, int reverse, int i, cudaStream_t st)
+{
+    const std::vector<int64_t>& so = reverse ? p->recv_off : p->send_off;
+    const std::vector<int64_t>& ro = reverse ? p->send_off : p->recv_off;
+    const int d = step_dst(p, i), s = step_src(p, i);
+    const int64_t ns = so[d + 1] - so[d], nr = ro[s + 1] - ro[s];
+    if (ns == 0 && nr == 0) return 0;
+    NC(p, g_nccl.GroupStart());
+    if (ns > 0) NC(p, g_nccl.Send(send + (size_t)so[d] * f, (size_t)ns * f, ncclFloat_, d, p->comm, st));
+    if (nr > 0) NC(p, g_nccl.Recv(recv + (size_t)ro[s] * f, (size_t)nr * f, ncclFloat_, s, p->comm, st));
+    NC(p, g_nccl.GroupEnd());
+    return 0;
+}
+
+// Send half of the forward exchange, shared by pgcn_forward and the unsplit forward: the owned rows leave for every peer
+// in step order. Peer transport: the device epoch advances on `st` (every call of the plan that exchanges does this
+// once, which is what picks the slab parity) and the rows are stored into each peer's slab of the new parity. NCCL: they
+// are packed and sent, and each source's block is received into the halo slab. With `split` the sends run on the
+// exchange stream, after `st`'s earlier work; ev_step[i] (NCCL) and ev_b (peer transport) mark their progress.
+int forward_send(pgcn_plan* p, const float* H_own, int f, bool use_p2p, bool split, cudaStream_t st)
+{
+    int rc;
+    if (use_p2p && (rc = advance_epoch(p, st))) return rc;
+    cudaStream_t cs = split ? p->comm_stream : st;
+    if (split) {
+        CU(p, cudaEventRecord(p->ev_a, st));
+        CU(p, cudaStreamWaitEvent(cs, p->ev_a, 0));
+    }
+    if (use_p2p) {
+        for (int i = 1; i < p->k; ++i)
+            if ((rc = p2p_put(p, step_dst(p, i), H_own, f, false, cs))) return rc;
+        if (split) CU(p, cudaEventRecord(p->ev_b, cs));                   // H_own is free for the caller after this
+    } else {
+        if ((rc = launch_pack(p, H_own, p->d_send_slab, f, cs))) return rc;
+        for (int i = 1; i < p->k; ++i) {
+            if ((rc = nccl_step(p, p->d_send_slab, p->d_halo_slab, f, 0, i, cs))) return rc;
+            if (split) CU(p, cudaEventRecord(p->ev_step[(size_t)i], cs));
+        }
+    }
+    return 0;
+}
+
+// Peer transport: `st` waits for every source's rows (NCCL receives on the stream that needs them).
+int p2p_wait_all(pgcn_plan* p, cudaStream_t st)
+{
+    int rc;
+    for (int i = 1; i < p->k; ++i)
+        if ((rc = p2p_wait(p, step_src(p, i), st))) return rc;
+    return 0;
+}
+
+// Copy the halo rows (h x f) the last forward exchange delivered into dst; halo_odd: the peer transport's odd-epoch twin
+// of the slab, picked from the device epoch. Nothing to copy on one rank, without halo rows or without dst.
+int copy_halo(pgcn_plan* p, const float* halo, const float* halo_odd, float* dst, int f, cudaStream_t st)
+{
+    if (p->k == 1 || p->h == 0 || !dst) return 0;
+    const long long n = (long long)p->h * f;
+    copy_halo_kernel<<<grid_for(n, p->num_sms), 256, 0, st>>>(halo, halo_odd, halo_odd ? p->d_epoch : nullptr, dst, n);
+    ++p->launches;
+    CU(p, cudaGetLastError());
+    return 0;
+}
+
+// The unsplit forward exchange (pgcn_forward without its per-source overlap, both transports): every source's rows have
+// landed before launch(halo, halo_odd) runs on `st`. halo is the slab the rows land in, halo_odd its odd-epoch twin on
+// the peer transport (else null); on one rank there is no exchange.
+template <class Launch>
+int unsplit_forward(pgcn_plan* p, const float* H_own, int f, cudaStream_t st, Launch launch)
+{
+    if (p->k == 1) return launch(p->d_halo_slab, (const float*)nullptr);
+    Transport x;
+    int rc;
+    if ((rc = transport(p, f, &x)) || (rc = forward_send(p, H_own, f, x.p2p, false, st))) return rc;
+    if (x.p2p && (rc = p2p_wait_all(p, st))) return rc;
+    return launch(x.halo, x.halo_odd);
+}
+
+// The unsplit backward exchange (pgcn_backward without its per-peer pipelining): launch() writes the rows of A^T gZ,
+// [0, m) into G_own and the halo partials into the reverse send slab; they go back to their owners and every rank adds
+// what it receives into G_own in a fixed order.
+template <class Launch>
+int unsplit_backward(pgcn_plan* p, float* G_own, int f, cudaStream_t st, Launch launch)
+{
+    if (p->k == 1) return launch();
+    Transport x;
+    int rc;
+    if ((rc = transport(p, f, &x))) return rc;
+    if (x.p2p && (rc = advance_epoch(p, st))) return rc;
+    if ((rc = launch())) return rc;
+    for (int i = 1; i < p->k; ++i) {
+        if (x.p2p) { if ((rc = p2p_put(p, step_dst(p, i), p->d_hsend_slab, f, true, st))) return rc; }
+        else if ((rc = nccl_step(p, p->d_hsend_slab, x.rrecv, f, 1, i, st))) return rc;
+    }
+    if (x.p2p && (rc = p2p_wait_all(p, st))) return rc;
+    return launch_unpack(p, x.rrecv, G_own, f, st, x.rrecv_odd);
 }
 
 }  // namespace
@@ -1784,13 +1788,10 @@ int pgcn_plan_set_option(pgcn_plan* p, const char* name, int64_t value)
 {
     if (!p || !name) return fail(p, PGCN_ERR_INVALID, "null argument");
     const std::string n(name);
-    auto clear_tuned = [&]() {
-        DevCsr* all[] = {&p->fwd, &p->tr, &p->own, &p->tr_own};
-        for (DevCsr* c : all) { c->tuned_epb[0] = c->tuned_epb[1] = 0; c->tuned_slots = 0; c->tuned_tile = 0; }
-        for (auto& c : p->halo_q) { c.tuned_epb[0] = c.tuned_epb[1] = 0; c.tuned_slots = 0; c.tuned_tile = 0; }
-        for (auto& c : p->tr_halo_q) { c.tuned_epb[0] = c.tuned_epb[1] = 0; c.tuned_slots = 0; c.tuned_tile = 0; }
-    };
-    if (n == "edges_per_block" || n == "ring_edges_per_block" || n == "ring_slots") clear_tuned();   // explicit beats tuned
+    if (n == "edges_per_block" || n == "ring_edges_per_block" || n == "ring_slots")   // explicit beats tuned
+        for (DevCsr* c : plan_matrices(p)) {
+            c->tuned_epb[0] = c->tuned_epb[1] = 0; c->tuned_slots = 0; c->tuned_tile = 0;
+        }
     if (n == "edges_per_block") p->opt_epb = value;
     else if (n == "kernel") p->opt_kernel = value;
     else if (n == "ring_slots") p->opt_ring_slots = value;
@@ -1997,44 +1998,31 @@ int pgcn_plan_prepare(pgcn_plan* p, int32_t f)
     if (rc) return rc;
     CU(p, cudaSetDevice(p->device));
     preload_kernels();
-    std::vector<DevCsr*> mats = {&p->fwd, &p->tr};
-    if (p->have_split) {
-        mats.push_back(&p->own);
-        mats.push_back(&p->tr_own);
-        for (auto& c : p->halo_q) mats.push_back(&c);
-        for (auto& c : p->tr_halo_q) mats.push_back(&c);
-    }
+    cudaStream_t st = p->host_stream;
     const bool ring = p->opt_kernel != 4 && f % 128 == 0;
-    for (DevCsr* c : mats) {
-        if (c->nrows == 0) continue;
-        for (int which = 0; which < (ring ? 2 : 1); ++which) {
-            int64_t epb, long_row;
-            sched_params(p, *c, which == 1, &epb, &long_row);
-            if ((rc = build_schedule(p, *c, which, epb, long_row))) return rc;
-        }
-    }
-    if (ring)
-        for (int tf = 64; tf <= 256; tf *= 2)
-            for (int halo = 0; halo < 2; ++halo) {
-                for (int shape = 0; shape < 4; ++shape)
-                    if ((rc = ring_attr(p, tf, shape, 2, halo != 0, p->host_stream, nullptr, nullptr))) return rc;
-                for (int shape = 0; shape < 2; ++shape)
-                    if ((rc = ring_attr(p, tf, shape, 0, halo != 0, p->host_stream, nullptr, nullptr))) return rc;
-                if (tf >= 128 && (rc = ring_attr(p, tf, 0, 1, halo != 0, p->host_stream, nullptr, nullptr))) return rc;
-            }
-    // pgcn_sddmm walks the forward matrix's schedules (built above); its ring instance of width f needs its attribute
-    if (ring && f <= 512 && (rc = sddmm_attr(p, f, p->host_stream))) return rc;
-    // the multi-head calls: the register schedules (built above) and the multi-head SDDMM ring instances of width f
+    DevCsr::Sched* sc;
+    for (DevCsr* c : plan_matrices(p))
+        if (c->nrows > 0 && ((rc = schedule(p, *c, false, st, &sc)) || (ring && (rc = schedule(p, *c, true, st, &sc)))))
+            return rc;
+    auto ring_opt_in = [&](const RingInst& ri) { return opt_in(p, ri.fn, ri.smem, ri.warps * 32, st, nullptr); };
+    if (ring && (rc = for_each_ring(ring_opt_in))) return rc;
+    // the ring instances of the edge calls at width f (they walk the forward matrix's schedules, built above)
+    auto edge_opt_in = [&](const void* fn) {
+        return opt_in(p, fn, sddmm_smem_bytes(f / 128), kSddmmWarps * 32, st, nullptr);
+    };
+    // pgcn_sddmm
+    if (ring && f <= 512 && (rc = edge_opt_in((const void*)pick_sddmm(f / 128)))) return rc;
+    // the multi-head SDDMM
     if (ring && (f == 128 || f == 256 || f == 512))
         for (int k = 2; k <= 8; k *= 2)
-            if ((f / k) % 4 == 0 && (rc = sddmm_heads_attr(p, f, k, p->host_stream))) return rc;
+            if ((f / k) % 4 == 0 && (rc = edge_opt_in((const void*)pick_sddmm_heads(f / 128, k)))) return rc;
     // the max calls of a bound plan: the register schedules (built above) and the entries of the forward's split rows
-    if (p->bound && (rc = max_partial(p, p->fwd.sched[0], p->host_stream))) return rc;
+    if (p->bound && (rc = max_partial(p, p->fwd.sched[0], st))) return rc;
     // the GATv2 calls: the score ring instances of width f and the datt partials of a bound plan
     if (ring && (f == 128 || f == 256))
         for (int k = 1; k <= 8; k *= 2)
-            if ((rc = gatv2_attr(p, f, k, p->host_stream))) return rc;
-    if (p->bound && (rc = gatv2_partial(p, p->fwd.sched[0], p->host_stream))) return rc;
+            if ((rc = edge_opt_in((const void*)pick_gatv2_ring(f / 128, k)))) return rc;
+    if (p->bound && (rc = gatv2_partial(p, p->fwd.sched[0], st))) return rc;
     p->prepared = true;
     return 0;
 }
@@ -2327,64 +2315,6 @@ int pgcn_unpack_add(pgcn_plan* p, const float* recv_slab, float* G_own, int32_t 
     return launch_unpack(p, recv_slab, G_own, f, (cudaStream_t)stream);
 }
 
-// Exchange schedule shared by both transports and both directions: at step i = 1 .. k-1 a rank sends to
-// (rank + i) % k and receives from (rank - i) % k — every pair is active exactly once per step, and a receiver
-// sees its sources arrive one after the other, so each block can be consumed while the next is in flight.
-static inline int step_dst(const pgcn_plan* p, int i) { return (p->rank + i) % p->k; }
-static inline int step_src(const pgcn_plan* p, int i) { return (p->rank - i + p->k) % p->k; }
-
-static int nccl_step(pgcn_plan* p, const float* send, float* recv, int f, int reverse, int i, cudaStream_t st)
-{
-    const std::vector<int64_t>& so = reverse ? p->recv_off : p->send_off;
-    const std::vector<int64_t>& ro = reverse ? p->send_off : p->recv_off;
-    const int d = step_dst(p, i), s = step_src(p, i);
-    const int64_t ns = so[d + 1] - so[d], nr = ro[s + 1] - ro[s];
-    if (ns == 0 && nr == 0) return 0;
-    NC(p, g_nccl.GroupStart());
-    if (ns > 0) NC(p, g_nccl.Send(send + (size_t)so[d] * f, (size_t)ns * f, ncclFloat_, d, p->comm, st));
-    if (nr > 0) NC(p, g_nccl.Recv(recv + (size_t)ro[s] * f, (size_t)nr * f, ncclFloat_, s, p->comm, st));
-    NC(p, g_nccl.GroupEnd());
-    return 0;
-}
-
-// Send half of the forward exchange, shared by pgcn_forward and pgcn_halo_rows: the owned rows leave for every peer in
-// step order. Peer transport: the device epoch advances on `st` (every call of the plan that exchanges does this once,
-// which is what picks the slab parity) and the rows are stored into each peer's slab of the new parity. NCCL: they are
-// packed and sent, and each source's block is received into the halo slab. With `split` the sends run on the exchange
-// stream, after `st`'s earlier work; ev_step[i] (NCCL) and ev_b (peer transport) mark their progress.
-static int forward_send(pgcn_plan* p, const float* H_own, int f, bool use_p2p, bool split, cudaStream_t st)
-{
-    int rc;
-    if (use_p2p && (rc = advance_epoch(p, st))) return rc;
-    cudaStream_t cs = split ? p->comm_stream : st;
-    if (split) {
-        CU(p, cudaEventRecord(p->ev_a, st));
-        CU(p, cudaStreamWaitEvent(cs, p->ev_a, 0));
-    }
-    if (use_p2p) {
-        for (int i = 1; i < p->k; ++i)
-            if ((rc = p2p_put(p, step_dst(p, i), H_own, f, false, cs))) return rc;
-        if (split) CU(p, cudaEventRecord(p->ev_b, cs));                   // H_own is free for the caller after this
-    } else {
-        if ((rc = launch_pack(p, H_own, p->d_send_slab, f, cs))) return rc;
-        for (int i = 1; i < p->k; ++i) {
-            if ((rc = nccl_step(p, p->d_send_slab, p->d_halo_slab, f, 0, i, cs))) return rc;
-            if (split) CU(p, cudaEventRecord(p->ev_step[(size_t)i], cs));
-        }
-    }
-    return 0;
-}
-
-// Wait half of an unsplit forward exchange: `st` waits for every source's rows (NCCL received them on `st` already).
-static int forward_wait_all(pgcn_plan* p, bool use_p2p, cudaStream_t st)
-{
-    int rc;
-    if (use_p2p)
-        for (int i = 1; i < p->k; ++i)
-            if ((rc = p2p_wait(p, step_src(p, i), st))) return rc;
-    return 0;
-}
-
 int pgcn_forward(pgcn_plan* p, const float* H_own, float* Z, int32_t f, void* stream)
 {
     int rc = check_f(p, f);
@@ -2392,33 +2322,26 @@ int pgcn_forward(pgcn_plan* p, const float* H_own, float* Z, int32_t f, void* st
     if (p->m > 0 && (!H_own || !Z)) return fail(p, PGCN_ERR_INVALID, "null H_own/Z");
     cudaStream_t st = (cudaStream_t)stream;
     const int relu = (int)p->opt_relu;
-    if (p->k == 1)
-        return launch_spmm(p, p->fwd, H_own, p->h > 0 ? p->d_halo_slab : nullptr, p->m, Z, nullptr, p->m, f, 0, st, relu);
-
-    const bool use_p2p = p->p2p && (f % 4 == 0);
-    if (!use_p2p && !p->comm) return fail(p, PGCN_ERR_STATE, "k=%d: call pgcn_comm_init or pgcn_p2p_import first", p->k);
-    const bool split = p->have_split && p->opt_overlap;
-    const int k = p->k;
-    float* halo = use_p2p ? arena_ptr(p->arena, p->off_fwd[0]) : p->d_halo_slab;
-    const float* halo_odd = use_p2p ? arena_ptr(p->arena, p->off_fwd[1]) : nullptr;
-    if ((rc = forward_send(p, H_own, f, use_p2p, split, st))) return rc;
-    if (!split) {
-        // no overlap requested (or nothing to split): wait for every block, then one pass over [own | halo]
-        if ((rc = forward_wait_all(p, use_p2p, st))) return rc;
-        return launch_spmm(p, p->fwd, H_own, p->h > 0 ? halo : nullptr, p->m, Z, nullptr, p->m, f, 0, st, relu, false,
-                           p->h > 0 ? halo_odd : nullptr);
-    }
+    if (!p->have_split || !p->opt_overlap)
+        // one rank, no overlap requested or nothing to split: every block has landed before one pass over [own | halo]
+        return unsplit_forward(p, H_own, f, st, [&](float* halo, const float* halo_odd) {
+            return launch_spmm(p, p->fwd, H_own, p->h > 0 ? halo : nullptr, p->m, Z, nullptr, p->m, f, 0, st, relu, false,
+                               p->h > 0 ? halo_odd : nullptr);
+        });
+    Transport x;
+    if ((rc = transport(p, f, &x)) || (rc = forward_send(p, H_own, f, x.p2p, true, st))) return rc;
     // ---- compute side: own columns while the rows travel, then each source's block as soon as it has landed
     if ((rc = launch_spmm(p, p->own, H_own, nullptr, p->m, Z, nullptr, p->m, f, 0, st, relu, true))) return rc;
-    for (int i = 1; i < k; ++i) {
+    for (int i = 1; i < p->k; ++i) {
         const int src = step_src(p, i);
-        if (use_p2p) { if ((rc = p2p_wait(p, src, st))) return rc; }
+        if (x.p2p) { if ((rc = p2p_wait(p, src, st))) return rc; }
         else CU(p, cudaStreamWaitEvent(st, p->ev_step[(size_t)i], 0));
         if (p->halo_q[(size_t)src].nrows == 0) continue;
-        if ((rc = launch_spmm(p, p->halo_q[(size_t)src], halo, nullptr, p->h, Z, nullptr, p->m, f, 1, st, relu, true, halo_odd)))
+        if ((rc = launch_spmm(p, p->halo_q[(size_t)src], x.halo, nullptr, p->h, Z, nullptr, p->m, f, 1, st, relu, true,
+                              x.halo_odd)))
             return rc;
     }
-    if (use_p2p) CU(p, cudaStreamWaitEvent(st, p->ev_b, 0));
+    if (x.p2p) CU(p, cudaStreamWaitEvent(st, p->ev_b, 0));
     return 0;
 }
 
@@ -2429,50 +2352,30 @@ int pgcn_backward(pgcn_plan* p, const float* gZ, float* G_own, int32_t f, void* 
     if (p->m > 0 && (!gZ || !G_own)) return fail(p, PGCN_ERR_INVALID, "null gZ/G_own");
     cudaStream_t st = (cudaStream_t)stream;
     // A^T g : rows [0,m) -> G_own, rows [m,m+h) -> halo partials, already in reverse wire order
-    if (p->k == 1) return launch_spmm(p, p->tr, gZ, nullptr, p->m, G_own, p->d_hsend_slab, p->m, f, 0, st);
-
-    const bool use_p2p = p->p2p && (f % 4 == 0);
-    if (!use_p2p && !p->comm) return fail(p, PGCN_ERR_STATE, "k=%d: call pgcn_comm_init or pgcn_p2p_import first", p->k);
-    const bool split = p->have_split && p->opt_overlap;
-    const int k = p->k;
-    float* rrecv = p->d_rrecv_slab;
-    const float* rrecv_odd = nullptr;
-    if (use_p2p) {
-        if ((rc = advance_epoch(p, st))) return rc;
-        rrecv = arena_ptr(p->arena, p->off_bwd[0]);
-        rrecv_odd = arena_ptr(p->arena, p->off_bwd[1]);
-    }
-    if (!split) {
-        if ((rc = launch_spmm(p, p->tr, gZ, nullptr, p->m, G_own, p->d_hsend_slab, p->m, f, 0, st))) return rc;
-        for (int i = 1; i < k; ++i) {
-            if (use_p2p) { if ((rc = p2p_put(p, step_dst(p, i), p->d_hsend_slab, f, true, st))) return rc; }
-            else if ((rc = nccl_step(p, p->d_hsend_slab, rrecv, f, 1, i, st))) return rc;
-        }
-        if (use_p2p)
-            for (int i = 1; i < k; ++i)
-                if ((rc = p2p_wait(p, step_src(p, i), st))) return rc;
-        return launch_unpack(p, rrecv, G_own, f, st, rrecv_odd);
-    }
+    if (!p->have_split || !p->opt_overlap)
+        return unsplit_backward(p, G_own, f, st, [&]() {
+            return launch_spmm(p, p->tr, gZ, nullptr, p->m, G_own, p->d_hsend_slab, p->m, f, 0, st);
+        });
+    Transport x;
+    if ((rc = transport(p, f, &x))) return rc;
+    if (x.p2p && (rc = advance_epoch(p, st))) return rc;
     // ---- pipelined: the partials owed to each peer are computed first (in step order) and leave on the exchange
     // stream while the next peer's rows, and finally the own rows of A^T g, are still being computed
     cudaStream_t cs = p->comm_stream;
-    for (int i = 1; i < k; ++i) {
+    for (int i = 1; i < p->k; ++i) {
         const int dst = step_dst(p, i);
         if (p->tr_halo_q[(size_t)dst].nrows > 0)
             if ((rc = launch_spmm(p, p->tr_halo_q[(size_t)dst], gZ, nullptr, p->m, G_own, p->d_hsend_slab, p->m, f, 0, st))) return rc;
         CU(p, cudaEventRecord(p->ev_step[(size_t)i], st));
         CU(p, cudaStreamWaitEvent(cs, p->ev_step[(size_t)i], 0));
-        if (use_p2p) { if ((rc = p2p_put(p, dst, p->d_hsend_slab, f, true, cs))) return rc; }
-        else if ((rc = nccl_step(p, p->d_hsend_slab, rrecv, f, 1, i, cs))) return rc;
+        if (x.p2p) { if ((rc = p2p_put(p, dst, p->d_hsend_slab, f, true, cs))) return rc; }
+        else if ((rc = nccl_step(p, p->d_hsend_slab, x.rrecv, f, 1, i, cs))) return rc;
     }
     CU(p, cudaEventRecord(p->ev_b, cs));
     if ((rc = launch_spmm(p, p->tr_own, gZ, nullptr, p->m, G_own, p->d_hsend_slab, p->m, f, 0, st))) return rc;
-    if (use_p2p) {
-        for (int i = 1; i < k; ++i)
-            if ((rc = p2p_wait(p, step_src(p, i), st))) return rc;
-    }
+    if (x.p2p && (rc = p2p_wait_all(p, st))) return rc;
     CU(p, cudaStreamWaitEvent(st, p->ev_b, 0));      // NCCL: all blocks received; p2p: the send slab is free again
-    return launch_unpack(p, rrecv, G_own, f, st, rrecv_odd);
+    return launch_unpack(p, x.rrecv, G_own, f, st, x.rrecv_odd);
 }
 
 int pgcn_forward_keep_halo(pgcn_plan* p, const float* H_own, float* Z, float* H_halo_out, int32_t f, void* stream)
@@ -2484,15 +2387,9 @@ int pgcn_forward_keep_halo(pgcn_plan* p, const float* H_own, float* Z, float* H_
     if (p->k == 1 || p->h == 0) return 0;
     // the stream has waited for every source's rows; the peer transport's rows sit in the slab of this call's parity,
     // which the next fused call of the same parity overwrites: copy them now, picking the slab from the device epoch
-    cudaStream_t st = (cudaStream_t)stream;
-    const bool use_p2p = p->p2p && (f % 4 == 0);
-    const float* src = use_p2p ? arena_ptr(p->arena, p->off_fwd[0]) : p->d_halo_slab;
-    const float* src_odd = use_p2p ? arena_ptr(p->arena, p->off_fwd[1]) : nullptr;
-    const long long n = (long long)p->h * f;
-    copy_halo_kernel<<<grid_for(n, p->num_sms), 256, 0, st>>>(src, src_odd, use_p2p ? p->d_epoch : nullptr, H_halo_out, n);
-    ++p->launches;
-    CU(p, cudaGetLastError());
-    return 0;
+    Transport x;
+    if ((rc = transport(p, f, &x))) return rc;
+    return copy_halo(p, x.halo, x.halo_odd, H_halo_out, f, (cudaStream_t)stream);
 }
 
 int pgcn_sddmm(pgcn_plan* p, const float* gZ, const float* H_own, const float* H_halo, float* dvals, int32_t f, void* stream)
@@ -2514,19 +2411,10 @@ int pgcn_halo_rows(pgcn_plan* p, const float* X_own, float* X_halo_out, int32_t 
     if (p->k == 1) return 0;
     if (p->m > 0 && !X_own) return fail(p, PGCN_ERR_INVALID, "null X_own");
     if (p->h > 0 && !X_halo_out) return fail(p, PGCN_ERR_INVALID, "h=%d but X_halo_out is null", p->h);
-    const bool use_p2p = p->p2p && (w % 4 == 0);
-    if (!use_p2p && !p->comm) return fail(p, PGCN_ERR_STATE, "k=%d: call pgcn_comm_init or pgcn_p2p_import first", p->k);
     cudaStream_t st = (cudaStream_t)stream;
-    if ((rc = forward_send(p, X_own, w, use_p2p, false, st))) return rc;
-    if ((rc = forward_wait_all(p, use_p2p, st))) return rc;
-    if (p->h == 0) return 0;
-    const float* src = use_p2p ? arena_ptr(p->arena, p->off_fwd[0]) : p->d_halo_slab;
-    const float* src_odd = use_p2p ? arena_ptr(p->arena, p->off_fwd[1]) : nullptr;
-    const long long n = (long long)p->h * w;
-    copy_halo_kernel<<<grid_for(n, p->num_sms), 256, 0, st>>>(src, src_odd, use_p2p ? p->d_epoch : nullptr, X_halo_out, n);
-    ++p->launches;
-    CU(p, cudaGetLastError());
-    return 0;
+    return unsplit_forward(p, X_own, w, st, [&](float* halo, const float* halo_odd) {
+        return copy_halo(p, halo, halo_odd, X_halo_out, w, st);
+    });
 }
 
 static int attn_check(pgcn_plan* p, const char* what, const float* el, const float* er_own, const float* er_halo)
@@ -2640,55 +2528,6 @@ int pgcn_edge_softmax_backward_heads(pgcn_plan* p, int32_t heads, const float* e
                        attn_vec(heads, {el, er_own, a.er_halo, alpha, dalpha, dpre, d_el}));
 }
 
-extern "C++" {
-
-// The unsplit forward exchange of the multi-head and max calls (pgcn_forward without its per-source overlap, both
-// transports): every source's rows have landed before launch(halo, halo_odd) runs on `st`. halo is the slab the rows
-// land in, halo_odd its odd-epoch twin on the peer transport (else null); on one rank there is no exchange.
-template <class Launch>
-static int unsplit_forward(pgcn_plan* p, const float* H_own, int f, cudaStream_t st, Launch launch)
-{
-    if (p->k == 1) return launch(p->d_halo_slab, (const float*)nullptr);
-    const bool use_p2p = p->p2p && (f % 4 == 0);
-    if (!use_p2p && !p->comm) return fail(p, PGCN_ERR_STATE, "k=%d: call pgcn_comm_init or pgcn_p2p_import first", p->k);
-    float* halo = use_p2p ? arena_ptr(p->arena, p->off_fwd[0]) : p->d_halo_slab;
-    const float* halo_odd = use_p2p ? arena_ptr(p->arena, p->off_fwd[1]) : nullptr;
-    int rc;
-    if ((rc = forward_send(p, H_own, f, use_p2p, false, st))) return rc;
-    if ((rc = forward_wait_all(p, use_p2p, st))) return rc;
-    return launch(halo, halo_odd);
-}
-
-// The unsplit backward exchange of the multi-head and max calls (pgcn_backward without its per-peer pipelining):
-// launch() writes the rows of A^T gZ, [0, m) into G_own and the halo partials into the reverse send slab; they go back
-// to their owners and every rank adds what it receives into G_own in a fixed order.
-template <class Launch>
-static int unsplit_backward(pgcn_plan* p, float* G_own, int f, cudaStream_t st, Launch launch)
-{
-    if (p->k == 1) return launch();
-    const bool use_p2p = p->p2p && (f % 4 == 0);
-    if (!use_p2p && !p->comm) return fail(p, PGCN_ERR_STATE, "k=%d: call pgcn_comm_init or pgcn_p2p_import first", p->k);
-    int rc;
-    float* rrecv = p->d_rrecv_slab;
-    const float* rrecv_odd = nullptr;
-    if (use_p2p) {
-        if ((rc = advance_epoch(p, st))) return rc;
-        rrecv = arena_ptr(p->arena, p->off_bwd[0]);
-        rrecv_odd = arena_ptr(p->arena, p->off_bwd[1]);
-    }
-    if ((rc = launch())) return rc;
-    for (int i = 1; i < p->k; ++i) {
-        if (use_p2p) { if ((rc = p2p_put(p, step_dst(p, i), p->d_hsend_slab, f, true, st))) return rc; }
-        else if ((rc = nccl_step(p, p->d_hsend_slab, rrecv, f, 1, i, st))) return rc;
-    }
-    if (use_p2p)
-        for (int i = 1; i < p->k; ++i)
-            if ((rc = p2p_wait(p, step_src(p, i), st))) return rc;
-    return launch_unpack(p, rrecv, G_own, f, st, rrecv_odd);
-}
-
-}  // extern "C++"
-
 // The unsplit forward exchange, then one multi-head launch over [H_own | halo slab of the call's parity], then the halo
 // copy. The plan's resident values are not read.
 int pgcn_forward_heads(pgcn_plan* p, int32_t heads, const float* alpha, const float* H_own, float* Z, float* H_halo_out,
@@ -2703,13 +2542,7 @@ int pgcn_forward_heads(pgcn_plan* p, int32_t heads, const float* alpha, const fl
     return unsplit_forward(p, H_own, f, st, [&](float* halo, const float* halo_odd) -> int {
         int rc2 = launch_spmm(p, p->fwd, H_own, p->h > 0 ? halo : nullptr, p->m, Z, nullptr, p->m, f, 0, st, 0, false,
                               p->h > 0 ? halo_odd : nullptr, &ha);
-        if (rc2 || p->k == 1 || !H_halo_out || p->h == 0) return rc2;
-        const long long n = (long long)p->h * f;
-        copy_halo_kernel<<<grid_for(n, p->num_sms), 256, 0, st>>>(halo, halo_odd, halo_odd ? p->d_epoch : nullptr,
-                                                                  H_halo_out, n);
-        ++p->launches;
-        CU(p, cudaGetLastError());
-        return 0;
+        return rc2 ? rc2 : copy_halo(p, halo, halo_odd, H_halo_out, f, st);
     });
 }
 
@@ -2806,13 +2639,7 @@ int pgcn_forward_gatv2(pgcn_plan* p, int32_t heads, const float* xl_own, const f
         if (rc2 || (rc2 = launch_softmax_raw(p, false, heads, nullptr, alpha, st))) return rc2;
         if ((rc2 = launch_spmm(p, p->fwd, xl_own, H1, p->m, Z, nullptr, p->m, f, 0, st, 0, false, H1_odd, &ha)))
             return rc2;
-        if (p->k == 1 || !xl_halo_out || p->h == 0) return 0;
-        const long long n = (long long)p->h * f;
-        copy_halo_kernel<<<grid_for(n, p->num_sms), 256, 0, st>>>(halo, halo_odd, halo_odd ? p->d_epoch : nullptr,
-                                                                  xl_halo_out, n);
-        ++p->launches;
-        CU(p, cudaGetLastError());
-        return 0;
+        return copy_halo(p, halo, halo_odd, xl_halo_out, f, st);
     });
 }
 

@@ -4,6 +4,7 @@ capture) and replayed on new inputs: every replay equals an eager call on the sa
   * one rank: PSpMM forward + backward and PSpMMRelu, register kernel (f = 16, 100) and ring kernel (f = 128, 256:
     64-float slices, full width, autotuned), "local" and "global" layouts;
   * a capture that would need set-up work is refused with an error naming prepare, and leaves plan and stream usable;
+    a refused call has enqueued no kernel (a matrix with empty rows, whose zero-fill comes after all set-up);
   * several ranks on this GPU over the peer transport (plan.link_local_plans), eager calls and replays mixed so that the
     device-resident exchange epoch takes both parities in both directions;
   * schedules replaced after the capture are retired, not freed, and the replay still computes the old options;
@@ -120,6 +121,36 @@ def test_capture_before_prepare_is_refused(f):
     xn = x.cpu().numpy()
     assert_close_fp32(z.cpu().numpy(), orc.truth_forward(A, xn), fp32_tol(A, xn, int(orc.row_degree(A).max())),
                       "eager after refused capture f=%d" % f)
+    plan.close()
+
+
+def test_refused_capture_enqueues_nothing():
+    """A capture refused because a ring instance lacks its shared-memory opt-in (the schedule itself is built) leaves
+    no kernel in the caller's graph: the zero-fill of the empty rows comes after all set-up."""
+    import scipy.sparse as sp
+    A = sp.coo_matrix(one_rank_matrix("rmat"))
+    keep = (A.row < 10) | (A.row >= 20)                      # rows 10..19 without entries
+    A = sp.csr_matrix((A.data[keep], (A.row[keep], A.col[keep])), shape=A.shape)
+    n, f = A.shape[0], 128
+    assert (orc.row_degree(A) == 0).sum() == 10
+    plan = planmod.build_plan(A, np.zeros(n, dtype=np.int64), 0, 1, f, device=dev())
+    x = rand(np.random.RandomState(2), n, f)
+    PSpMM.apply(plan, x)                                     # eager: ring schedule and the 16-slot instance
+    torch.cuda.synchronize()
+    plan.set_option("ring_slots", 32)                        # same schedule, a ring instance not opted in yet
+    launches = plan.launch_count()
+    s = torch.cuda.Stream()
+    graph = torch.cuda.CUDAGraph()
+    with pytest.raises(RuntimeError, match="pgcn_plan_prepare"):
+        with torch.cuda.graph(graph, stream=s):
+            PSpMM.apply(plan, x)
+    assert plan.launch_count() == launches, "the refused call enqueued %d kernels" % (plan.launch_count() - launches)
+    with torch.cuda.stream(s):                              # the capture was not invalidated: plan and stream still work
+        z = PSpMM.apply(plan, x)
+    s.synchronize()
+    xn = x.cpu().numpy()
+    assert_close_fp32(z.cpu().numpy(), orc.truth_forward(A, xn), fp32_tol(A, xn, int(orc.row_degree(A).max())),
+                      "eager after refused capture with empty rows")
     plan.close()
 
 
