@@ -465,10 +465,12 @@ TileCfg choose_tile(const pgcn_plan* p, int f, int vw)
 
 typedef void (*spmm_fn)(const SpmmArgs);
 
+// choose_tile takes lpe = pow2ceil(tile_vecs) below 32 lanes, which covers the tile: only LPE = 32 has VPL 2 and 4
 template <int LPE, int VW>
 spmm_fn pick_vpl(int vpl, bool halo)
 {
-    switch (vpl) {
+    if constexpr (LPE < 32) return halo ? spmm_rowblock_kernel<LPE, 1, VW, true> : spmm_rowblock_kernel<LPE, 1, VW, false>;
+    else switch (vpl) {
         case 1: return halo ? spmm_rowblock_kernel<LPE, 1, VW, true> : spmm_rowblock_kernel<LPE, 1, VW, false>;
         case 2: return halo ? spmm_rowblock_kernel<LPE, 2, VW, true> : spmm_rowblock_kernel<LPE, 2, VW, false>;
         default: return halo ? spmm_rowblock_kernel<LPE, 4, VW, true> : spmm_rowblock_kernel<LPE, 4, VW, false>;
@@ -490,6 +492,8 @@ spmm_fn pick_lpe(int lpe, int vpl, bool halo)
 // blockIdx.y tiles of LPE vectors), NH heads staged per chunk.
 typedef void (*spmm_heads_fn)(const SpmmArgs, const SpmmHeadArgs);
 
+// 8 heads need f >= 8 floats, i.e. 8 or more lanes of one vector (choose_tile_heads): LPE = 4 has no 8-head instance
+// (null: the launch fails with an error instead of running a wrong shape)
 template <int LPE, int VW, bool HALO>
 spmm_heads_fn pick_heads_nh(int nh)
 {
@@ -497,7 +501,9 @@ spmm_heads_fn pick_heads_nh(int nh)
         case 1: return spmm_heads_kernel<LPE, VW, HALO, 1>;
         case 2: return spmm_heads_kernel<LPE, VW, HALO, 2>;
         case 4: return spmm_heads_kernel<LPE, VW, HALO, 4>;
-        default: return spmm_heads_kernel<LPE, VW, HALO, 8>;
+        default:
+            if constexpr (LPE > 4) return spmm_heads_kernel<LPE, VW, HALO, 8>;
+            else return nullptr;
     }
 }
 
@@ -730,7 +736,7 @@ attn_fn pick_softmax_raw_k(bool vec, bool backward)
 attn_fn pick_softmax_raw(int k, bool vec, bool backward)
 {
     switch (k) {
-        case 1: return pick_softmax_raw_k<1>(false, backward);
+        case 1: return backward ? edge_softmax_raw_backward_kernel<1, false> : edge_softmax_raw_kernel<1, false>;
         case 2: return pick_softmax_raw_k<2>(vec, backward);
         case 4: return pick_softmax_raw_k<4>(vec, backward);
         default: return pick_softmax_raw_k<8>(vec, backward);
@@ -749,8 +755,11 @@ gatv2_bwd_fn pick_gatv2_bwd_nh(int nh, bool col, bool halo)
                            : (halo ? gatv2_row_backward_kernel<LPE, VW, true, 2> : gatv2_row_backward_kernel<LPE, VW, false, 2>);
         case 4: return col ? gatv2_col_backward_kernel<LPE, VW, 4>
                            : (halo ? gatv2_row_backward_kernel<LPE, VW, true, 4> : gatv2_row_backward_kernel<LPE, VW, false, 4>);
-        default: return col ? gatv2_col_backward_kernel<LPE, VW, 8>
-                            : (halo ? gatv2_row_backward_kernel<LPE, VW, true, 8> : gatv2_row_backward_kernel<LPE, VW, false, 8>);
+        default:   // no 8-head instance at LPE = 4, as pick_heads_nh
+            if constexpr (LPE > 4)
+                return col ? gatv2_col_backward_kernel<LPE, VW, 8>
+                           : (halo ? gatv2_row_backward_kernel<LPE, VW, true, 8> : gatv2_row_backward_kernel<LPE, VW, false, 8>);
+            else return nullptr;
     }
 }
 template <int VW>
@@ -774,7 +783,11 @@ gatv2_bwd_fn pick_gatv2_bwd(int lpe, int vw, int nh, bool col, bool halo)
 // when the ranks it waits for live in the SAME process (single-process multi-rank use: tests, smoke) — their put
 // kernels would never be enqueued. Touching every kernel once, when the peer transport is set up, removes the hazard.
 template <class F>
-void touch_kernel(F fn) { cudaFuncAttributes fa; if (cudaFuncGetAttributes(&fa, (const void*)fn) != cudaSuccess) cudaGetLastError(); }
+void touch_kernel(F fn)
+{
+    cudaFuncAttributes fa;
+    if (fn && cudaFuncGetAttributes(&fa, (const void*)fn) != cudaSuccess) cudaGetLastError();   // null: no such instance
+}
 
 void preload_kernels()
 {
