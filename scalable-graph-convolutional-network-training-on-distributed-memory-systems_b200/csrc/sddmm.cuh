@@ -84,160 +84,6 @@ __host__ __device__ constexpr size_t sddmm_warp_bytes(int nv)
 }
 __host__ __device__ constexpr size_t sddmm_smem_bytes(int nv) { return sddmm_warp_bytes(nv) * kSddmmWarps + 128; }
 
-// Sum 8 per-lane partials over the 32 lanes of the warp with a transposing butterfly: each step halves the values a
-// lane holds and doubles the lanes that share each of them (4 + 2 + 1 shuffles), then two plain steps finish the sum.
-// 9 shuffles for 8 edges; lane l returns the sum of edge (l >> 2) & 7. Every sum is added in one fixed order.
-__device__ __forceinline__ float sddmm_reduce8(const float (&p)[8], int lane)
-{
-    const bool b4 = lane & 16, b3 = lane & 8, b2 = lane & 4;
-    float q4[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const float keep = b4 ? p[i + 4] : p[i], send = b4 ? p[i] : p[i + 4];
-        q4[i] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
-    }
-    float q2[2];
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-        const float keep = b3 ? q4[i + 2] : q4[i], send = b3 ? q4[i] : q4[i + 2];
-        q2[i] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
-    }
-    float q = (b2 ? q2[1] : q2[0]) + __shfl_xor_sync(0xffffffffu, b2 ? q2[0] : q2[1], 4);
-    q += __shfl_xor_sync(0xffffffffu, q, 2);
-    q += __shfl_xor_sync(0xffffffffu, q, 1);
-    return q;
-}
-
-// NV = f / 128: what one lane holds of a row (NV float4, 512 bytes apart).
-// A warp walks one row block of the forward schedule at a time (persistent CTAs take blocks from a counter) in
-// globally aligned groups of 8 entries. Per group: lanes 0..7 read their entry's column and row-end / cold bits (one
-// group ahead) and fire one bulk copy of the whole H row each into the group's 8 slots; lane 0 arms the group's
-// mbarrier. Consumption: per edge, NV x LDS.128 and 4 NV FFMA against the warp's current gZ row, held in registers
-// (the next row's gZ is loaded one row ahead); the 8 partials go through the transposing butterfly and lanes 0, 4, .., 28
-// store the 8 results (32 contiguous bytes). Entries are independent: split rows need no fixup.
-template <int NV>
-__global__ void __launch_bounds__(kSddmmWarps * 32)
-sddmm_ring_kernel(const SddmmArgs a)
-{
-    constexpr int G = kSddmmG, NG = kSddmmNG, NS = G * NG;
-    constexpr uint32_t RB = NV * 512;                                    // bytes of one row
-    constexpr int RV = RB / 16;                                          // float4 per row slot
-    extern __shared__ __align__(128) unsigned char sddmm_smem[];
-
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    unsigned char* wbase = sddmm_smem + (size_t)warp * sddmm_warp_bytes(NV);
-    const uint32_t s_data = smem_u32(wbase);
-    const uint32_t s_bar = s_data + NS * RB;
-    const float4* data_gen = reinterpret_cast<const float4*>(wbase) + lane;
-
-    if (lane == 0) {
-#pragma unroll
-        for (int i = 0; i < NG; ++i) mbar_init(s_bar + i * 8, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    }
-    __syncwarp();
-
-    const unsigned long long pol_hot = l2_policy_evict_last();
-    const unsigned long long pol_cold = l2_policy_evict_first();
-    const size_t pitch = (size_t)a.f * 4;
-    const unsigned usplit = a.H1 ? (unsigned)a.split : 0xffffffffu;
-    const char* hb0 = reinterpret_cast<const char*>(a.H0);
-    const char* hb1 = a.H1 ? reinterpret_cast<const char*>(a.H1) - (size_t)a.split * pitch : hb0;
-    uint32_t gpar = 0;                                                   // phase parity of each group barrier
-
-    auto load_g = [&](float4 (&g)[NV], int row) {
-        const int orow = a.rowids ? __ldg(a.rowids + row) : row;
-        const float4* gp = reinterpret_cast<const float4*>(a.gZ + (size_t)(unsigned)orow * a.f) + lane;
-#pragma unroll
-        for (int v = 0; v < NV; ++v) g[v] = __ldg(gp + v * 32);
-    };
-
-    int w;
-    if (lane == 0) w = (int)atomicAdd(a.counter, 1u);
-    w = __shfl_sync(0xffffffffu, w, 0);
-    while (w < a.nblocks) {
-        const int4 b = __ldg(a.blocks + w);
-        const bool seg = b.y < 0;
-        const int e0 = b.z, e1 = b.w;
-        int row = b.x;
-        const int row_last = seg ? b.x : b.x + b.y - 1;
-        const int gA = e0 / G, gB = (e1 - 1) / G;
-
-        float4 gcur[NV], gnext[NV];
-        load_g(gcur, row);
-        if (row < row_last) load_g(gnext, row + 1);
-
-        // lane j < 8: column and {valid, row end, cold} bits of entry 8 gi + j
-        auto fetch = [&](int gi, int& col, uint32_t& bits) {
-            col = 0; bits = 0;
-            const int e = gi * G + lane;
-            if (lane < G && gi <= gB && e >= e0 && e < e1) {
-                const int* pc = a.pieces + (size_t)(e >> 5) * kPieceInts;
-                col = __ldg(pc + (e & 31));
-                const uint2 m = __ldg(reinterpret_cast<const uint2*>(pc + 64));
-                bits = 1u | (((m.x >> (e & 31)) & 1u) << 1) | (((m.y >> (e & 31)) & 1u) << 2);
-            }
-        };
-        uint32_t vmask[NG], emask[NG];
-        auto issue = [&](int sg, int col, uint32_t bits) {
-            const uint32_t vm = __ballot_sync(0xffffffffu, bits & 1u) & 0xffu;
-            const uint32_t em = __ballot_sync(0xffffffffu, (bits >> 1) & 1u) & 0xffu;
-            reg_set(vmask, sg, vm);
-            reg_set(emask, sg, seg ? 0u : em);
-            if (vm == 0) return;
-            if (lane == 0) mbar_expect_tx(s_bar + sg * 8, (uint32_t)__popc(vm) * RB);
-            if (bits & 1u) {
-                const unsigned cj = (unsigned)col;
-                bulk_g2s(s_data + (sg * G + lane) * RB, (cj >= usplit ? hb1 : hb0) + (size_t)cj * pitch, RB, s_bar + sg * 8,
-                         (bits & 4u) ? pol_cold : pol_hot);
-            }
-        };
-
-        int ncol;
-        uint32_t nbits;
-#pragma unroll
-        for (int i = 0; i < NG; ++i) { fetch(gA + i, ncol, nbits); issue(i, ncol, nbits); }
-        fetch(gA + NG, ncol, nbits);
-
-#pragma unroll 1
-        for (int gi = gA; gi <= gB; ++gi) {
-            const int sg = (gi - gA) % NG;
-            const uint32_t vm = reg_get(vmask, sg), em = reg_get(emask, sg);
-            mbar_wait(s_bar + sg * 8, (gpar >> sg) & 1);
-            gpar ^= 1u << sg;
-            const float4* slot = data_gen + (size_t)(sg * G) * RV;
-            float p[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                float s = 0.f;
-#pragma unroll
-                for (int v = 0; v < NV; ++v) {
-                    const float4 r = slot[j * RV + v * 32];
-                    s = fmaf(gcur[v].x, r.x, s); s = fmaf(gcur[v].y, r.y, s);
-                    s = fmaf(gcur[v].z, r.z, s); s = fmaf(gcur[v].w, r.w, s);
-                }
-                p[j] = (vm >> j & 1u) ? s : 0.f;                         // slots of masked entries hold stale rows
-                if (em >> j & 1u) {                                      // row end: the next row's gZ takes over
-                    ++row;
-#pragma unroll
-                    for (int v = 0; v < NV; ++v) gcur[v] = gnext[v];
-                    if (row < row_last) load_g(gnext, row + 1);
-                }
-            }
-            const float d = sddmm_reduce8(p, lane);
-            const int je = (lane >> 2) & 7;
-            if ((lane & 3) == 0 && (vm >> je & 1u)) a.dvals[(size_t)gi * G + je] = d;
-            __syncwarp();                                                // every lane is done with these slots
-            issue(sg, ncol, nbits);                                      // group gi + NG into the freed slots
-            fetch(gi + NG + 1, ncol, nbits);
-        }
-
-        if (lane == 0) w = (int)atomicAdd(a.counter, 1u);
-        w = __shfl_sync(0xffffffffu, w, 0);
-    }
-}
-
 // ---- multi-head SDDMM ----------------------------------------------------------------------------------------------
 //
 //     dalpha[e, h] = < gZ[row(e), h d:(h+1) d], [H_own ; H_halo][col(e), h d:(h+1) d] >        d = f / K
@@ -445,10 +291,25 @@ sddmm_heads_ring_kernel(const SddmmArgs a)
     sddmm_heads_ring_walk<NV, K>(a, SddmmDot());
 }
 
-// Any f, K and alignment: sddmm_plain_kernel with K heads; a lane's dot product restarts at every head boundary
-// (K = 1: the same products in the same order as sddmm_plain_kernel).
-__global__ void __launch_bounds__(256)
-sddmm_plain_heads_kernel(const SddmmArgs a, int K)
+// NV = f / 128: what one lane holds of a row (NV float4, 512 bytes apart).
+// A warp walks one row block of the forward schedule at a time (persistent CTAs take blocks from a counter) in
+// globally aligned groups of 8 entries. Per group: lanes 0..7 read their entry's column and row-end / cold bits (one
+// group ahead) and fire one bulk copy of the whole H row each into the group's 8 slots; lane 0 arms the group's
+// mbarrier. Consumption: per edge, NV x LDS.128 and 4 NV FFMA against the warp's current gZ row, held in registers
+// (the next row's gZ is loaded one row ahead); the 8 partials go through the transposing butterfly (sddmm_heads_ring_walk
+// at K = 1: 4 + 2 + 1 transposing shuffles over all 32 lanes, then two plain ones) and lanes 0, 4, .., 28 store the 8
+// results (32 contiguous bytes). Entries are independent: split rows need no fixup.
+template <int NV>
+__global__ void __launch_bounds__(kSddmmWarps * 32)
+sddmm_ring_kernel(const SddmmArgs a)
+{
+    sddmm_heads_ring_walk<NV, 1>(a, SddmmDot());
+}
+
+// Any f, K and alignment: one warp per row block of the register kernel's schedule, one lane per edge (32 edges at a
+// time, rows from a ballot of the row-end bits), each lane a sequential fp32 dot product per head over its d = f / K
+// features.
+__device__ __forceinline__ void sddmm_plain_walk(const SddmmArgs& a, int K)
 {
     const int lane = threadIdx.x & 31;
     const int w = (int)((blockIdx.x * (unsigned)blockDim.x + threadIdx.x) >> 5);
@@ -483,39 +344,16 @@ sddmm_plain_heads_kernel(const SddmmArgs a, int K)
     }
 }
 
-// Any f and alignment: one warp per row block of the register kernel's schedule, one lane per edge (32 edges at a time,
-// rows from a ballot of the row-end bits), each lane a sequential fp32 dot product over the f features.
 __global__ void __launch_bounds__(256)
 sddmm_plain_kernel(const SddmmArgs a)
 {
-    const int lane = threadIdx.x & 31;
-    const int w = (int)((blockIdx.x * (unsigned)blockDim.x + threadIdx.x) >> 5);
-    if (w >= a.nblocks) return;
-    const int4 b = __ldg(a.blocks + w);
-    const bool seg = b.y < 0;
-    int row = b.x;
-    for (int e = b.z; e < b.w; e += 32) {
-        const int ei = e + lane;
-        const bool ok = ei < b.w;
-        int col = 0;
-        bool end = false;
-        if (ok) {
-            const int* pc = a.pieces + (size_t)(ei >> 5) * kPieceInts;
-            col = __ldg(pc + (ei & 31));
-            end = !seg && ((__ldg(reinterpret_cast<const unsigned*>(pc + 64)) >> (ei & 31)) & 1u);
-        }
-        const unsigned ends = __ballot_sync(0xffffffffu, end);
-        if (ok) {
-            const int r = row + __popc(ends & ((1u << lane) - 1u));
-            const int orow = a.rowids ? __ldg(a.rowids + r) : r;
-            const float* g = a.gZ + (size_t)(unsigned)orow * a.f;
-            const float* hrow = (a.H1 && col >= a.split) ? a.H1 + (size_t)(col - a.split) * a.f : a.H0 + (size_t)col * a.f;
-            float s = 0.f;
-            for (int c = 0; c < a.f; ++c) s = fmaf(__ldg(g + c), __ldg(hrow + c), s);
-            a.dvals[ei] = s;
-        }
-        row += __popc(ends);
-    }
+    sddmm_plain_walk(a, 1);
+}
+
+__global__ void __launch_bounds__(256)
+sddmm_plain_heads_kernel(const SddmmArgs a, int K)
+{
+    sddmm_plain_walk(a, K);
 }
 
 }  // namespace pgcn

@@ -367,14 +367,8 @@ __device__ __forceinline__ float* spmm_head_smem()
 // blockIdx.y tiles) and another weight. Vector v of a lane is weighted by alpha[map(e) * NH + head], head = (its first
 // float) / hd, instead of the entry's value: the same rows, segments, flushes and summation order. The NH weights of a
 // chunk's entries are staged in shared memory next to s_cw, and the next chunk's are in flight in registers.
-// Registers: 4 CTAs of 256 threads per SM instead of 6 (the NH staged weights in flight).
-//
-// Per chunk of LPE edges a lane group stages its (column|flags, value) pairs in shared memory, so
-// the inner loop costs one broadcast LDS.64 per edge instead of two divergence-guarded shuffles;
-// the H row address is one IMAD.WIDE.U32 (32-bit column x row pitch in bytes + 64-bit base); the
-// own/halo base is a select, not a branch; full chunks run a predicate-free loop. Two gathers are in
-// flight per lane group (register double buffer A/B); the next chunk's index pairs are already in
-// flight in registers while the current chunk is processed.
+// Registers: 4 CTAs of 256 threads per SM instead of 6 (the NH staged weights in flight). The chunk staging and the
+// register double buffer are spmm_rowblock_kernel's (see its comment).
 template <int LPE, int VW, bool HALO, int NH>
 __global__ void __launch_bounds__(kSpmmThreads, 4)
 spmm_heads_kernel(const SpmmArgs a, const SpmmHeadArgs ha)
