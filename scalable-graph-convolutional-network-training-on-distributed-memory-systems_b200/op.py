@@ -14,6 +14,8 @@ Layouts (plan.layout):
              precondition Q0 that they are zero), Z is [n, f] with non-owned rows exactly 0.
 
 All arithmetic happens in libpgcn_b200.so on the current CUDA stream; there is no CPU path.
+Every operator takes its inputs through _own / _own_scores, returns its outputs through _to_layout and makes each C
+call through _call, so an operator is its validation and its sequence of C calls.
 """
 import torch
 
@@ -24,11 +26,28 @@ def _stream_ptr():
     return torch.cuda.current_stream().cuda_stream
 
 
-def _check_feat(plan, H, rows, what):
-    if not H.is_cuda:
+def _ptr(x):
+    return None if x is None else x.data_ptr()
+
+
+def _call(plan, dev, name, *args, exchange=None):
+    """lib.<name>(plan, *args, stream) on `dev`'s current stream, its status checked. exchange=False / True: the call ran
+    the forward / backward exchange, which plan.stats counts (nothing on one rank)."""
+    with torch.cuda.device(dev):
+        cabi.check(getattr(cabi.load(), name)(plan.handle, *args, _stream_ptr()), plan.handle)
+    if exchange is not None:
+        plan.count_exchange(backward=exchange)
+
+
+def _check_f32(x, what):
+    if not x.is_cuda:
         raise RuntimeError("%s must be a CUDA tensor: the PGCN H100 path has no CPU fallback" % what)
-    if H.dtype != torch.float32:
-        raise TypeError("%s must be float32, got %s" % (what, H.dtype))
+    if x.dtype != torch.float32:
+        raise TypeError("%s must be float32, got %s" % (what, x.dtype))
+
+
+def _check_feat(plan, H, rows, what):
+    _check_f32(H, what)
     if H.dim() != 2 or H.shape[0] != rows:
         raise ValueError("%s must be [%d, f], got %s" % (what, rows, tuple(H.shape)))
     if H.shape[1] > plan.f_max:
@@ -36,39 +55,99 @@ def _check_feat(plan, H, rows, what):
     return H.contiguous()
 
 
+def _rows(plan):
+    return plan.n if plan.layout == "global" else plan.m
+
+
+def _owned(plan, x):
+    return x.index_select(0, plan.owned_index()) if plan.layout == "global" else x.contiguous()
+
+
+def _own(plan, x, what):
+    """x, a [rows, f] feature tensor in the plan's layout, checked: its owned rows [m, f], contiguous."""
+    return _owned(plan, _check_feat(plan, x, _rows(plan), what))
+
+
+def _own_scores(plan, x, what, heads=None):
+    """x, per-row scores [rows] (heads None) or [rows, heads] in the plan's layout, checked: its owned rows, contiguous."""
+    shape = (_rows(plan),) if heads is None else (_rows(plan), heads)
+    _check_f32(x, what)
+    if tuple(x.shape) != shape:
+        raise ValueError("%s must be [%s], got %s" % (what, ", ".join(map(str, shape)), tuple(x.shape)))
+    return _owned(plan, x.detach())
+
+
+def _to_layout(plan, x_own):
+    """x_own [m, ...] in the plan's layout: itself in "local", [n, ...] with zero rows where other ranks own them in
+    "global"."""
+    if plan.layout != "global":
+        return x_own
+    out = torch.zeros((plan.n,) + tuple(x_own.shape[1:]), dtype=torch.float32, device=x_own.device)
+    out.index_copy_(0, plan.owned_index(), x_own)
+    return out
+
+
+def _require_bound(plan, what):
+    if not plan._bound:
+        raise RuntimeError("%s: call PgcnPlan.bind_values() once (set-up, before any CUDA-graph capture)" % what)
+
+
+def _aggregate(plan, H_own, keep_halo=False):
+    """(Z, H_halo): Z [m, f] = A [H_own; H_halo] with the plan's resident values, exchange included. keep_halo: H_halo is
+    the [h, f] halo rows the exchange brought (pgcn_forward_keep_halo) where there are any; otherwise None."""
+    lp, f, dev = plan.lp, H_own.shape[1], H_own.device
+    Z = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+    if keep_halo and lp.k > 1 and lp.h > 0:
+        H_halo = torch.empty((lp.h, f), dtype=torch.float32, device=dev)
+        _call(plan, dev, "pgcn_forward_keep_halo", H_own.data_ptr(), Z.data_ptr(), H_halo.data_ptr(), f, exchange=False)
+        return Z, H_halo
+    _call(plan, dev, "pgcn_forward", H_own.data_ptr(), Z.data_ptr(), f, exchange=False)
+    return Z, None
+
+
+def _aggregate_t(plan, gZ_own):
+    """G [m, f] = A^T gZ_own with the plan's resident values, the halo partials summed at their owners."""
+    f = gZ_own.shape[1]
+    G = torch.empty((plan.lp.m, f), dtype=torch.float32, device=gZ_own.device)
+    _call(plan, gZ_own.device, "pgcn_backward", gZ_own.data_ptr(), G.data_ptr(), f, exchange=True)
+    return G
+
+
+def _score_halo(plan, s_own):
+    """Per-row scores of the halo columns from their owners: s_own [m] or [m, K] gives [h] or [h, K]. pgcn_halo_rows
+    carries rows padded to a multiple of 4 floats, the width the peer transport takes; [m] travels as column 0 of 4."""
+    lp, dev = plan.lp, s_own.device
+    if lp.k == 1:
+        return torch.empty((lp.h,) + tuple(s_own.shape[1:]), dtype=torch.float32, device=dev)
+    K = s_own.shape[1] if s_own.dim() == 2 else 1
+    col = slice(0, K) if s_own.dim() == 2 else 0
+    w = (K + 3) // 4 * 4
+    padded = torch.zeros((lp.m, w), dtype=torch.float32, device=dev)
+    padded[:, col] = s_own
+    halo = torch.empty((lp.h, w), dtype=torch.float32, device=dev)
+    _call(plan, dev, "pgcn_halo_rows", padded.data_ptr(), halo.data_ptr(), w, exchange=False)
+    return halo[:, col].contiguous()
+
+
 def aggregate_forward(plan, H_own, relu=False):
     """Z_own = (A * H)[owned rows]; H_own, Z_own are [m, f]. relu=True: Z_own = max(0, .), clamped inside the store of
     the launch that writes each row last (plan option "relu")."""
     H_own = _check_feat(plan, H_own, plan.m, "H")
-    f = H_own.shape[1]
-    Z = torch.empty((plan.m, f), dtype=torch.float32, device=H_own.device)
-    lib = cabi.load()
-    with torch.cuda.device(H_own.device):
-        plan.use_values(None)             # PSpMM / PSpMMRelu aggregate with the plan's own values
+    plan.use_values(None)                 # PSpMM / PSpMMRelu aggregate with the plan's own values
+    if relu:
+        plan.set_option("relu", 1)
+    try:
+        return _aggregate(plan, H_own)[0]
+    finally:
         if relu:
-            plan.set_option("relu", 1)
-        try:
-            cabi.check(lib.pgcn_forward(plan.handle, H_own.data_ptr(), Z.data_ptr(), f, _stream_ptr()), plan.handle)
-        finally:
-            if relu:
-                plan.set_option("relu", 0)
-    if plan.lp.k > 1:
-        plan.count_exchange(backward=False)
-    return Z
+            plan.set_option("relu", 0)
 
 
 def aggregate_backward(plan, gZ_own):
     """G_own = (A^T * gZ)[owned rows] with every peer's contribution added; [m, f]."""
     gZ_own = _check_feat(plan, gZ_own, plan.m, "grad_output")
-    f = gZ_own.shape[1]
-    G = torch.empty((plan.m, f), dtype=torch.float32, device=gZ_own.device)
-    lib = cabi.load()
-    with torch.cuda.device(gZ_own.device):
-        plan.use_values(None)
-        cabi.check(lib.pgcn_backward(plan.handle, gZ_own.data_ptr(), G.data_ptr(), f, _stream_ptr()), plan.handle)
-    if plan.lp.k > 1:
-        plan.count_exchange(backward=True)
-    return G
+    plan.use_values(None)
+    return _aggregate_t(plan, gZ_own)
 
 
 class PSpMM(torch.autograd.Function):
@@ -77,24 +156,12 @@ class PSpMM(torch.autograd.Function):
     @staticmethod
     def forward(ctx, A, H):
         ctx.plan = A
-        if A.layout == "global":
-            _check_feat(A, H, A.n, "H")
-            Z_own = aggregate_forward(A, H.index_select(0, A.owned_index()))
-            Z = torch.zeros((A.n, H.shape[1]), dtype=torch.float32, device=H.device)
-            Z.index_copy_(0, A.owned_index(), Z_own)
-            return Z
-        return aggregate_forward(A, H)
+        return _to_layout(A, aggregate_forward(A, _own(A, H, "H")))
 
     @staticmethod
     def backward(ctx, grad_output):
         A = ctx.plan
-        if A.layout == "global":
-            g = _check_feat(A, grad_output, A.n, "grad_output")
-            G_own = aggregate_backward(A, g.index_select(0, A.owned_index()))
-            G = torch.zeros((A.n, g.shape[1]), dtype=torch.float32, device=g.device)
-            G.index_copy_(0, A.owned_index(), G_own)
-            return None, G
-        return None, aggregate_backward(A, grad_output)
+        return None, _to_layout(A, aggregate_backward(A, _own(A, grad_output, "grad_output")))
 
 
 class PSpMMRelu(torch.autograd.Function):
@@ -137,84 +204,26 @@ class PSpMMWeighted(torch.autograd.Function):
         from .plan import check_values
         check_values(A, vals)
         ctx.plan = A
-        ctx.glob = A.layout == "global"
-        if ctx.glob:
-            _check_feat(A, H, A.n, "H")
-            H_own = H.index_select(0, A.owned_index())
-        else:
-            H_own = _check_feat(A, H, A.m, "H")
-        lp = A.lp
-        f = H_own.shape[1]
+        H_own = _own(A, H, "H")
         want_dvals = ctx.needs_input_grad[1]
-        keep = want_dvals and lp.k > 1 and lp.h > 0
-        Z = torch.empty((lp.m, f), dtype=torch.float32, device=H_own.device)
-        H_halo = torch.empty((lp.h, f), dtype=torch.float32, device=H_own.device) if keep else None
-        lib = cabi.load()
-        with torch.cuda.device(H_own.device):
-            A.use_values(vals)
-            if keep:
-                cabi.check(lib.pgcn_forward_keep_halo(A.handle, H_own.data_ptr(), Z.data_ptr(), H_halo.data_ptr(), f,
-                                                      _stream_ptr()), A.handle)
-            else:
-                cabi.check(lib.pgcn_forward(A.handle, H_own.data_ptr(), Z.data_ptr(), f, _stream_ptr()), A.handle)
-        if lp.k > 1:
-            A.count_exchange(backward=False)
+        A.use_values(vals)
+        Z, H_halo = _aggregate(A, H_own, keep_halo=want_dvals)
         ctx.save_for_backward(vals, H_own if want_dvals else None, H_halo)
-        if ctx.glob:
-            Zg = torch.zeros((A.n, f), dtype=torch.float32, device=H.device)
-            Zg.index_copy_(0, A.owned_index(), Z)
-            return Zg
-        return Z
+        return _to_layout(A, Z)
 
     @staticmethod
     def backward(ctx, grad_output):
         A = ctx.plan
         vals, H_own, H_halo = ctx.saved_tensors
-        if ctx.glob:
-            g = _check_feat(A, grad_output, A.n, "grad_output").index_select(0, A.owned_index())
-        else:
-            g = _check_feat(A, grad_output, A.m, "grad_output")
-        lp = A.lp
-        f = g.shape[1]
-        lib = cabi.load()
+        g = _own(A, grad_output, "grad_output")
         dvals = dH = None
-        with torch.cuda.device(g.device):
-            if ctx.needs_input_grad[2]:
-                A.use_values(vals)
-                G = torch.empty((lp.m, f), dtype=torch.float32, device=g.device)
-                cabi.check(lib.pgcn_backward(A.handle, g.data_ptr(), G.data_ptr(), f, _stream_ptr()), A.handle)
-                if lp.k > 1:
-                    A.count_exchange(backward=True)
-                if ctx.glob:
-                    dH = torch.zeros((A.n, f), dtype=torch.float32, device=g.device)
-                    dH.index_copy_(0, A.owned_index(), G)
-                else:
-                    dH = G
-            if ctx.needs_input_grad[1]:
-                dvals = torch.empty((lp.nnz(),), dtype=torch.float32, device=g.device)
-                cabi.check(lib.pgcn_sddmm(A.handle, g.data_ptr(), H_own.data_ptr(),
-                                          H_halo.data_ptr() if H_halo is not None else None, dvals.data_ptr(), f,
-                                          _stream_ptr()), A.handle)
+        if ctx.needs_input_grad[2]:
+            A.use_values(vals)
+            dH = _to_layout(A, _aggregate_t(A, g))
+        if ctx.needs_input_grad[1]:
+            dvals = torch.empty((A.lp.nnz(),), dtype=torch.float32, device=g.device)
+            _call(A, g.device, "pgcn_sddmm", g.data_ptr(), H_own.data_ptr(), _ptr(H_halo), dvals.data_ptr(), g.shape[1])
         return None, dvals, dH
-
-
-def _check_scores(plan, x, rows, what):
-    if not x.is_cuda:
-        raise RuntimeError("%s must be a CUDA tensor: the PGCN H100 path has no CPU fallback" % what)
-    if x.dtype != torch.float32:
-        raise TypeError("%s must be float32, got %s" % (what, x.dtype))
-    if x.dim() != 1 or x.shape[0] != rows:
-        raise ValueError("%s must be [%d], got %s" % (what, rows, tuple(x.shape)))
-    x = x.detach()
-    return (x.index_select(0, plan.owned_index()) if plan.layout == "global" else x).contiguous()
-
-
-def _to_layout(plan, x_own, rows):
-    if plan.layout != "global":
-        return x_own
-    out = torch.zeros((rows,) + tuple(x_own.shape[1:]), dtype=torch.float32, device=x_own.device)
-    out.index_copy_(0, plan.owned_index(), x_own)
-    return out
 
 
 class PGATAttention(torch.autograd.Function):
@@ -235,101 +244,47 @@ class PGATAttention(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, A, Z, el, er, negative_slope=0.2):
-        rows = A.n if A.layout == "global" else A.m
-        Z_own = _check_feat(A, Z, rows, "Z")
-        if A.layout == "global":
-            Z_own = Z_own.index_select(0, A.owned_index())
-        el_own = _check_scores(A, el, rows, "el")
-        er_own = _check_scores(A, er, rows, "er")
-        lp = A.lp
-        f = Z_own.shape[1]
-        dev = Z_own.device
-        slope = float(negative_slope)
-        lib = cabi.load()
-        with torch.cuda.device(dev):
-            if not A._bound:
-                raise RuntimeError("PGATAttention sets the plan's edge values: call PgcnPlan.bind_values() once (set-up, "
-                                   "before any CUDA-graph capture)")
-            er_halo = torch.empty((lp.h,), dtype=torch.float32, device=dev)
-            if lp.k > 1:
-                er4 = torch.zeros((lp.m, 4), dtype=torch.float32, device=dev)
-                er4[:, 0] = er_own
-                er_halo4 = torch.empty((lp.h, 4), dtype=torch.float32, device=dev)
-                cabi.check(lib.pgcn_halo_rows(A.handle, er4.data_ptr(), er_halo4.data_ptr(), 4, _stream_ptr()),
-                           A.handle)
-                A.count_exchange(backward=False)
-                er_halo = er_halo4[:, 0].contiguous()
-            alpha = torch.empty((lp.nnz(),), dtype=torch.float32, device=dev)
-            cabi.check(lib.pgcn_edge_softmax(A.handle, el_own.data_ptr(), er_own.data_ptr(), er_halo.data_ptr(), slope,
-                                             alpha.data_ptr(), _stream_ptr()), A.handle)
-            out = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
-            Z_halo = torch.empty((lp.h, f), dtype=torch.float32, device=dev)
-            A.use_values(alpha)
-            if lp.k > 1 and lp.h > 0:
-                cabi.check(lib.pgcn_forward_keep_halo(A.handle, Z_own.data_ptr(), out.data_ptr(), Z_halo.data_ptr(), f,
-                                                      _stream_ptr()), A.handle)
-            else:
-                cabi.check(lib.pgcn_forward(A.handle, Z_own.data_ptr(), out.data_ptr(), f, _stream_ptr()), A.handle)
-            if lp.k > 1:
-                A.count_exchange(backward=False)
-        ctx.plan, ctx.rows, ctx.slope = A, rows, slope
+        Z_own = _own(A, Z, "Z")
+        el_own = _own_scores(A, el, "el")
+        er_own = _own_scores(A, er, "er")
+        _require_bound(A, "PGATAttention sets the plan's edge values")
+        lp, dev, slope = A.lp, Z_own.device, float(negative_slope)
+        er_halo = _score_halo(A, er_own)
+        alpha = torch.empty((lp.nnz(),), dtype=torch.float32, device=dev)
+        _call(A, dev, "pgcn_edge_softmax", el_own.data_ptr(), er_own.data_ptr(), er_halo.data_ptr(), slope,
+              alpha.data_ptr())
+        A.use_values(alpha)
+        out, Z_halo = _aggregate(A, Z_own, keep_halo=True)
+        ctx.plan, ctx.slope = A, slope
         ctx.save_for_backward(alpha, Z_own, Z_halo, el_own, er_own, er_halo)
-        return _to_layout(A, out, rows)
+        return _to_layout(A, out)
 
     @staticmethod
     def backward(ctx, grad_output):
-        A, rows, slope = ctx.plan, ctx.rows, ctx.slope
+        A, slope = ctx.plan, ctx.slope
         alpha, Z_own, Z_halo, el_own, er_own, er_halo = ctx.saved_tensors
-        g = _check_feat(A, grad_output, rows, "grad_output")
-        if A.layout == "global":
-            g = g.index_select(0, A.owned_index())
-        lp = A.lp
-        f = g.shape[1]
-        dev = g.device
-        lib = cabi.load()
+        g = _own(A, grad_output, "grad_output")
+        lp, f, dev = A.lp, g.shape[1], g.device
         dZ = d_el = d_er = None
-        with torch.cuda.device(dev):
-            if ctx.needs_input_grad[1]:
-                A.use_values(alpha)
-                G = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
-                cabi.check(lib.pgcn_backward(A.handle, g.data_ptr(), G.data_ptr(), f, _stream_ptr()), A.handle)
-                if lp.k > 1:
-                    A.count_exchange(backward=True)
-                dZ = _to_layout(A, G, rows)
-            if ctx.needs_input_grad[2] or ctx.needs_input_grad[3]:
-                dalpha = torch.empty_like(alpha)
-                cabi.check(lib.pgcn_sddmm(A.handle, g.data_ptr(), Z_own.data_ptr(), Z_halo.data_ptr(),
-                                          dalpha.data_ptr(), f, _stream_ptr()), A.handle)
-                dpre = torch.empty_like(alpha)
-                gel = torch.empty((lp.m,), dtype=torch.float32, device=dev)
-                cabi.check(lib.pgcn_edge_softmax_backward(A.handle, el_own.data_ptr(), er_own.data_ptr(),
-                                                          er_halo.data_ptr(), alpha.data_ptr(), dalpha.data_ptr(),
-                                                          slope, dpre.data_ptr(), gel.data_ptr(), _stream_ptr()),
-                           A.handle)
-                d_el = _to_layout(A, gel, rows) if ctx.needs_input_grad[2] else None
-                if ctx.needs_input_grad[3]:
-                    A.use_values(dpre)
-                    ones = torch.ones((lp.m, 4), dtype=torch.float32, device=dev)
-                    D = torch.empty((lp.m, 4), dtype=torch.float32, device=dev)
-                    cabi.check(lib.pgcn_backward(A.handle, ones.data_ptr(), D.data_ptr(), 4, _stream_ptr()), A.handle)
-                    if lp.k > 1:
-                        A.count_exchange(backward=True)
-                    d_er = _to_layout(A, D[:, 0].contiguous(), rows)
+        if ctx.needs_input_grad[1]:
+            A.use_values(alpha)
+            dZ = _to_layout(A, _aggregate_t(A, g))
+        if ctx.needs_input_grad[2] or ctx.needs_input_grad[3]:
+            dalpha = torch.empty_like(alpha)
+            _call(A, dev, "pgcn_sddmm", g.data_ptr(), Z_own.data_ptr(), _ptr(Z_halo), dalpha.data_ptr(), f)
+            dpre = torch.empty_like(alpha)
+            gel = torch.empty((lp.m,), dtype=torch.float32, device=dev)
+            _call(A, dev, "pgcn_edge_softmax_backward", el_own.data_ptr(), er_own.data_ptr(), er_halo.data_ptr(),
+                  alpha.data_ptr(), dalpha.data_ptr(), slope, dpre.data_ptr(), gel.data_ptr())
+            d_el = _to_layout(A, gel) if ctx.needs_input_grad[2] else None
+            if ctx.needs_input_grad[3]:
+                A.use_values(dpre)
+                ones = torch.ones((lp.m, 4), dtype=torch.float32, device=dev)
+                d_er = _to_layout(A, _aggregate_t(A, ones)[:, 0].contiguous())
         return None, dZ, d_el, d_er, None
 
 
 HEADS = (1, 2, 4, 8)
-
-
-def _check_head_scores(plan, x, rows, heads, what):
-    if not x.is_cuda:
-        raise RuntimeError("%s must be a CUDA tensor: the PGCN H100 path has no CPU fallback" % what)
-    if x.dtype != torch.float32:
-        raise TypeError("%s must be float32, got %s" % (what, x.dtype))
-    if x.dim() != 2 or x.shape[0] != rows or x.shape[1] != heads:
-        raise ValueError("%s must be [%d, %d], got %s" % (what, rows, heads, tuple(x.shape)))
-    x = x.detach()
-    return (x.index_select(0, plan.owned_index()) if plan.layout == "global" else x).contiguous()
 
 
 class PGATMultiHeadAttention(torch.autograd.Function):
@@ -351,94 +306,59 @@ class PGATMultiHeadAttention(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, A, Z, el, er, negative_slope=0.2):
-        rows = A.n if A.layout == "global" else A.m
         if el.dim() != 2:
-            raise ValueError("el must be [%d, heads], got %s" % (rows, tuple(el.shape)))
+            raise ValueError("el must be [%d, heads], got %s" % (_rows(A), tuple(el.shape)))
         K = el.shape[1]
         if K not in HEADS:
             raise ValueError("heads=%d: the multi-head kernels take 1, 2, 4 or 8 heads" % K)
-        Z_own = _check_feat(A, Z, rows, "Z")
+        Z_own = _own(A, Z, "Z")
         f = Z_own.shape[1]
         if f % K:
             raise ValueError("f=%d is not a multiple of heads=%d" % (f, K))
         if A.f_max < 4 * K:
             raise ValueError("heads=%d: the backward aggregates rows of 4 x heads = %d floats, the plan's f_max is %d"
                              % (K, 4 * K, A.f_max))
-        if A.layout == "global":
-            Z_own = Z_own.index_select(0, A.owned_index())
-        el_own = _check_head_scores(A, el, rows, K, "el")
-        er_own = _check_head_scores(A, er, rows, K, "er")
-        lp = A.lp
-        dev = Z_own.device
-        slope = float(negative_slope)
-        lib = cabi.load()
-        with torch.cuda.device(dev):
-            if not A._bound:
-                raise RuntimeError("PGATMultiHeadAttention reads the plan's value maps: call PgcnPlan.bind_values() once "
-                                   "(set-up, before any CUDA-graph capture)")
-            er_halo = torch.empty((lp.h, K), dtype=torch.float32, device=dev)
-            if lp.k > 1:
-                w = (K + 3) // 4 * 4
-                erw = torch.zeros((lp.m, w), dtype=torch.float32, device=dev)
-                erw[:, :K] = er_own
-                er_halo_w = torch.empty((lp.h, w), dtype=torch.float32, device=dev)
-                cabi.check(lib.pgcn_halo_rows(A.handle, erw.data_ptr(), er_halo_w.data_ptr(), w, _stream_ptr()),
-                           A.handle)
-                A.count_exchange(backward=False)
-                er_halo = er_halo_w[:, :K].contiguous()
-            alpha = torch.empty((lp.nnz(), K), dtype=torch.float32, device=dev)
-            cabi.check(lib.pgcn_edge_softmax_heads(A.handle, K, el_own.data_ptr(), er_own.data_ptr(), er_halo.data_ptr(),
-                                                   slope, alpha.data_ptr(), _stream_ptr()), A.handle)
-            out = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
-            Z_halo = torch.empty((lp.h, f), dtype=torch.float32, device=dev)
-            keep = lp.k > 1 and lp.h > 0
-            cabi.check(lib.pgcn_forward_heads(A.handle, K, alpha.data_ptr(), Z_own.data_ptr(), out.data_ptr(),
-                                              Z_halo.data_ptr() if keep else None, f, _stream_ptr()), A.handle)
-            if lp.k > 1:
-                A.count_exchange(backward=False)
-        ctx.plan, ctx.rows, ctx.slope, ctx.heads = A, rows, slope, K
+        el_own = _own_scores(A, el, "el", K)
+        er_own = _own_scores(A, er, "er", K)
+        _require_bound(A, "PGATMultiHeadAttention reads the plan's value maps")
+        lp, dev, slope = A.lp, Z_own.device, float(negative_slope)
+        er_halo = _score_halo(A, er_own)
+        alpha = torch.empty((lp.nnz(), K), dtype=torch.float32, device=dev)
+        _call(A, dev, "pgcn_edge_softmax_heads", K, el_own.data_ptr(), er_own.data_ptr(), er_halo.data_ptr(), slope,
+              alpha.data_ptr())
+        out = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+        Z_halo = torch.empty((lp.h, f), dtype=torch.float32, device=dev) if lp.k > 1 and lp.h > 0 else None
+        _call(A, dev, "pgcn_forward_heads", K, alpha.data_ptr(), Z_own.data_ptr(), out.data_ptr(), _ptr(Z_halo), f,
+              exchange=False)
+        ctx.plan, ctx.slope, ctx.heads = A, slope, K
         ctx.save_for_backward(alpha, Z_own, Z_halo, el_own, er_own, er_halo)
-        return _to_layout(A, out, rows)
+        return _to_layout(A, out)
 
     @staticmethod
     def backward(ctx, grad_output):
-        A, rows, slope, K = ctx.plan, ctx.rows, ctx.slope, ctx.heads
+        A, slope, K = ctx.plan, ctx.slope, ctx.heads
         alpha, Z_own, Z_halo, el_own, er_own, er_halo = ctx.saved_tensors
-        g = _check_feat(A, grad_output, rows, "grad_output")
-        if A.layout == "global":
-            g = g.index_select(0, A.owned_index())
-        lp = A.lp
-        f = g.shape[1]
-        dev = g.device
-        lib = cabi.load()
+        g = _own(A, grad_output, "grad_output")
+        lp, f, dev = A.lp, g.shape[1], g.device
         dZ = d_el = d_er = None
-        with torch.cuda.device(dev):
-            if ctx.needs_input_grad[1]:
-                G = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
-                cabi.check(lib.pgcn_backward_heads(A.handle, K, alpha.data_ptr(), g.data_ptr(), G.data_ptr(), f,
-                                                   _stream_ptr()), A.handle)
-                if lp.k > 1:
-                    A.count_exchange(backward=True)
-                dZ = _to_layout(A, G, rows)
-            if ctx.needs_input_grad[2] or ctx.needs_input_grad[3]:
-                dalpha = torch.empty_like(alpha)
-                cabi.check(lib.pgcn_sddmm_heads(A.handle, K, g.data_ptr(), Z_own.data_ptr(), Z_halo.data_ptr(),
-                                                dalpha.data_ptr(), f, _stream_ptr()), A.handle)
-                dpre = torch.empty_like(alpha)
-                gel = torch.empty((lp.m, K), dtype=torch.float32, device=dev)
-                cabi.check(lib.pgcn_edge_softmax_backward_heads(A.handle, K, el_own.data_ptr(), er_own.data_ptr(),
-                                                                er_halo.data_ptr(), alpha.data_ptr(), dalpha.data_ptr(),
-                                                                slope, dpre.data_ptr(), gel.data_ptr(), _stream_ptr()),
-                           A.handle)
-                d_el = _to_layout(A, gel, rows) if ctx.needs_input_grad[2] else None
-                if ctx.needs_input_grad[3]:
-                    ones = torch.ones((lp.m, 4 * K), dtype=torch.float32, device=dev)
-                    D = torch.empty((lp.m, 4 * K), dtype=torch.float32, device=dev)
-                    cabi.check(lib.pgcn_backward_heads(A.handle, K, dpre.data_ptr(), ones.data_ptr(), D.data_ptr(),
-                                                       4 * K, _stream_ptr()), A.handle)
-                    if lp.k > 1:
-                        A.count_exchange(backward=True)
-                    d_er = _to_layout(A, D[:, 0::4].contiguous(), rows)
+        if ctx.needs_input_grad[1]:
+            G = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+            _call(A, dev, "pgcn_backward_heads", K, alpha.data_ptr(), g.data_ptr(), G.data_ptr(), f, exchange=True)
+            dZ = _to_layout(A, G)
+        if ctx.needs_input_grad[2] or ctx.needs_input_grad[3]:
+            dalpha = torch.empty_like(alpha)
+            _call(A, dev, "pgcn_sddmm_heads", K, g.data_ptr(), Z_own.data_ptr(), _ptr(Z_halo), dalpha.data_ptr(), f)
+            dpre = torch.empty_like(alpha)
+            gel = torch.empty((lp.m, K), dtype=torch.float32, device=dev)
+            _call(A, dev, "pgcn_edge_softmax_backward_heads", K, el_own.data_ptr(), er_own.data_ptr(), er_halo.data_ptr(),
+                  alpha.data_ptr(), dalpha.data_ptr(), slope, dpre.data_ptr(), gel.data_ptr())
+            d_el = _to_layout(A, gel) if ctx.needs_input_grad[2] else None
+            if ctx.needs_input_grad[3]:
+                ones = torch.ones((lp.m, 4 * K), dtype=torch.float32, device=dev)
+                D = torch.empty((lp.m, 4 * K), dtype=torch.float32, device=dev)
+                _call(A, dev, "pgcn_backward_heads", K, dpre.data_ptr(), ones.data_ptr(), D.data_ptr(), 4 * K,
+                      exchange=True)
+                d_er = _to_layout(A, D[:, 0::4].contiguous())
         return None, dZ, d_el, d_er, None
 
 
@@ -459,14 +379,13 @@ class PGATv2Attention(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, A, XL, XR, att, negative_slope=0.2):
-        rows = A.n if A.layout == "global" else A.m
         if att.dim() != 2:
             raise ValueError("att must be [heads, f / heads], got %s" % (tuple(att.shape),))
         K = att.shape[0]
         if K not in HEADS:
             raise ValueError("heads=%d: the GATv2 kernels take 1, 2, 4 or 8 heads" % K)
-        XL_own = _check_feat(A, XL, rows, "XL")
-        XR_own = _check_feat(A, XR, rows, "XR")
+        XL_own = _own(A, XL, "XL")
+        XR_own = _own(A, XR, "XR")
         f = XL_own.shape[1]
         if XR_own.shape[1] != f:
             raise ValueError("XL and XR must have the same width, got %d and %d" % (f, XR_own.shape[1]))
@@ -477,76 +396,45 @@ class PGATv2Attention(torch.autograd.Function):
         if not att.is_cuda or att.dtype != torch.float32:
             raise TypeError("att must be a float32 CUDA tensor")
         att_c = att.detach().contiguous()
-        if A.layout == "global":
-            XL_own = XL_own.index_select(0, A.owned_index())
-            XR_own = XR_own.index_select(0, A.owned_index())
-        lp = A.lp
-        dev = XL_own.device
-        slope = float(negative_slope)
-        lib = cabi.load()
-        with torch.cuda.device(dev):
-            if not A._bound:
-                raise RuntimeError("PGATv2Attention reads the plan's value maps: call PgcnPlan.bind_values() once "
-                                   "(set-up, before any CUDA-graph capture)")
-            alpha = torch.empty((lp.nnz(), K), dtype=torch.float32, device=dev)
-            out = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
-            XL_halo = torch.empty((lp.h, f), dtype=torch.float32, device=dev)
-            keep = lp.k > 1 and lp.h > 0
-            cabi.check(lib.pgcn_forward_gatv2(A.handle, K, XL_own.data_ptr(), XR_own.data_ptr(), att_c.data_ptr(),
-                                              slope, alpha.data_ptr(), out.data_ptr(),
-                                              XL_halo.data_ptr() if keep else None, f, _stream_ptr()), A.handle)
-            if lp.k > 1:
-                A.count_exchange(backward=False)
-        ctx.plan, ctx.rows, ctx.slope, ctx.heads = A, rows, slope, K
+        _require_bound(A, "PGATv2Attention reads the plan's value maps")
+        lp, dev, slope = A.lp, XL_own.device, float(negative_slope)
+        alpha = torch.empty((lp.nnz(), K), dtype=torch.float32, device=dev)
+        out = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+        XL_halo = torch.empty((lp.h, f), dtype=torch.float32, device=dev) if lp.k > 1 and lp.h > 0 else None
+        _call(A, dev, "pgcn_forward_gatv2", K, XL_own.data_ptr(), XR_own.data_ptr(), att_c.data_ptr(), slope,
+              alpha.data_ptr(), out.data_ptr(), _ptr(XL_halo), f, exchange=False)
+        ctx.plan, ctx.slope, ctx.heads = A, slope, K
         ctx.save_for_backward(alpha, XL_own, XL_halo, XR_own, att_c)
-        return _to_layout(A, out, rows)
+        return _to_layout(A, out)
 
     @staticmethod
     def backward(ctx, grad_output):
-        A, rows, slope, K = ctx.plan, ctx.rows, ctx.slope, ctx.heads
+        A, slope, K = ctx.plan, ctx.slope, ctx.heads
         alpha, XL_own, XL_halo, XR_own, att = ctx.saved_tensors
-        g = _check_feat(A, grad_output, rows, "grad_output")
-        if A.layout == "global":
-            g = g.index_select(0, A.owned_index())
-        lp = A.lp
-        f = g.shape[1]
-        dev = g.device
-        with torch.cuda.device(dev):
-            work = torch.empty_like(alpha)
-            dxl = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
-            dxr = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
-            datt = torch.empty_like(att)
-            cabi.check(cabi.load().pgcn_backward_gatv2(
-                A.handle, K, alpha.data_ptr(), g.data_ptr(), XL_own.data_ptr(), XL_halo.data_ptr() if lp.h else None,
-                XR_own.data_ptr(), att.data_ptr(), slope, work.data_ptr(), dxl.data_ptr(), dxr.data_ptr(),
-                datt.data_ptr(), f, _stream_ptr()), A.handle)
-            if lp.k > 1:
-                A.count_exchange(backward=True)
-        return None, _to_layout(A, dxl, rows), _to_layout(A, dxr, rows), datt, None
+        g = _own(A, grad_output, "grad_output")
+        lp, f, dev = A.lp, g.shape[1], g.device
+        work = torch.empty_like(alpha)
+        dxl = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+        dxr = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+        datt = torch.empty_like(att)
+        _call(A, dev, "pgcn_backward_gatv2", K, alpha.data_ptr(), g.data_ptr(), XL_own.data_ptr(), _ptr(XL_halo),
+              XR_own.data_ptr(), att.data_ptr(), slope, work.data_ptr(), dxl.data_ptr(), dxr.data_ptr(),
+              datt.data_ptr(), f, exchange=True)
+        return None, _to_layout(A, dxl), _to_layout(A, dxr), datt, None
 
 
 # ---- max aggregation -------------------------------------------------------------------------------------------------
-
-def _check_max_plan(plan, what):
-    if not plan._bound:
-        raise RuntimeError("%s walks the transposed records through the plan's value maps: call PgcnPlan.bind_values() "
-                           "once (set-up, before any CUDA-graph capture)" % what)
-
 
 def aggregate_max(plan, H_own):
     """(Z_own, arg): the element-wise maximum over each owned row's stored entries of [H_own ; H_halo] (pgcn_forward_max).
     Z_own is [m, f] fp32, arg [m, f] int32: the winning entry, the first in forward CSR order (lp.colidx's order) with
     the largest value, NaN above every number; lp.colidx[arg] is its local column. Rows without an entry give 0 / -1."""
     H_own = _check_feat(plan, H_own, plan.m, "H")
-    _check_max_plan(plan, "aggregate_max")
+    _require_bound(plan, "aggregate_max walks the transposed records through the plan's value maps")
     f = H_own.shape[1]
     Z = torch.empty((plan.m, f), dtype=torch.float32, device=H_own.device)
     arg = torch.empty((plan.m, f), dtype=torch.int32, device=H_own.device)
-    with torch.cuda.device(H_own.device):
-        cabi.check(cabi.load().pgcn_forward_max(plan.handle, H_own.data_ptr(), Z.data_ptr(), arg.data_ptr(), f,
-                                                _stream_ptr()), plan.handle)
-    if plan.lp.k > 1:
-        plan.count_exchange(backward=False)
+    _call(plan, H_own.device, "pgcn_forward_max", H_own.data_ptr(), Z.data_ptr(), arg.data_ptr(), f, exchange=False)
     return Z, arg
 
 
@@ -554,18 +442,14 @@ def aggregate_max_backward(plan, arg, gZ_own):
     """G_own [m, f]: gZ routed to the winning entries named by `arg` (aggregate_max's), summed per column on its owner
     (pgcn_backward_max)."""
     gZ_own = _check_feat(plan, gZ_own, plan.m, "grad_output")
-    _check_max_plan(plan, "aggregate_max_backward")
+    _require_bound(plan, "aggregate_max_backward walks the transposed records through the plan's value maps")
     f = gZ_own.shape[1]
     if arg.dtype != torch.int32 or arg.device != gZ_own.device or tuple(arg.shape) != (plan.m, f):
         raise ValueError("arg must be int32 [%d, %d] on %s, got %s %s on %s"
                          % (plan.m, f, gZ_own.device, arg.dtype, tuple(arg.shape), arg.device))
     arg = arg.contiguous()
     G = torch.empty((plan.m, f), dtype=torch.float32, device=gZ_own.device)
-    with torch.cuda.device(gZ_own.device):
-        cabi.check(cabi.load().pgcn_backward_max(plan.handle, arg.data_ptr(), gZ_own.data_ptr(), G.data_ptr(), f,
-                                                 _stream_ptr()), plan.handle)
-    if plan.lp.k > 1:
-        plan.count_exchange(backward=True)
+    _call(plan, gZ_own.device, "pgcn_backward_max", arg.data_ptr(), gZ_own.data_ptr(), G.data_ptr(), f, exchange=True)
     return G
 
 
@@ -578,23 +462,16 @@ class PSpMMMax(torch.autograd.Function):
     @staticmethod
     def forward(ctx, A, H):
         ctx.plan = A
-        _check_max_plan(A, "PSpMMMax")
-        if A.layout == "global":
-            _check_feat(A, H, A.n, "H")
-            Z_own, arg = aggregate_max(A, H.index_select(0, A.owned_index()))
-        else:
-            Z_own, arg = aggregate_max(A, H)
+        _require_bound(A, "PSpMMMax walks the transposed records through the plan's value maps")
+        Z_own, arg = aggregate_max(A, _own(A, H, "H"))
         ctx.save_for_backward(arg)
-        return _to_layout(A, Z_own, A.n)
+        return _to_layout(A, Z_own)
 
     @staticmethod
     def backward(ctx, grad_output):
         A = ctx.plan
         (arg,) = ctx.saved_tensors
-        if A.layout == "global":
-            g = _check_feat(A, grad_output, A.n, "grad_output").index_select(0, A.owned_index())
-            return None, _to_layout(A, aggregate_max_backward(A, arg, g), A.n)
-        return None, aggregate_max_backward(A, arg, grad_output)
+        return None, _to_layout(A, aggregate_max_backward(A, arg, _own(A, grad_output, "grad_output")))
 
 
 # ---- the pieces, individually callable (NCCL transport), mirroring communicate_fgm ----------------
@@ -606,20 +483,16 @@ def spmm_local(plan, H_own, H_halo=None, transpose=False):
     H_own = _check_feat(plan, H_own, lp.m, "H_own")
     f = H_own.shape[1]
     dev = H_own.device
-    lib = cabi.load()
-    with torch.cuda.device(dev):
-        if not transpose:
-            if lp.h:
-                H_halo = _check_feat(plan, H_halo, lp.h, "H_halo")
-            Z = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
-            cabi.check(lib.pgcn_spmm(plan.handle, 0, H_own.data_ptr(), H_halo.data_ptr() if lp.h else None,
-                                     Z.data_ptr(), None, f, _stream_ptr()), plan.handle)
-            return Z
-        G = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
-        Gh = torch.empty((lp.h, f), dtype=torch.float32, device=dev)
-        cabi.check(lib.pgcn_spmm(plan.handle, 1, H_own.data_ptr(), None, G.data_ptr(),
-                                 Gh.data_ptr() if lp.h else None, f, _stream_ptr()), plan.handle)
-        return G, Gh
+    if not transpose:
+        if lp.h:
+            H_halo = _check_feat(plan, H_halo, lp.h, "H_halo")
+        Z = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+        _call(plan, dev, "pgcn_spmm", 0, H_own.data_ptr(), H_halo.data_ptr() if lp.h else None, Z.data_ptr(), None, f)
+        return Z
+    G = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+    Gh = torch.empty((lp.h, f), dtype=torch.float32, device=dev)
+    _call(plan, dev, "pgcn_spmm", 1, H_own.data_ptr(), None, G.data_ptr(), Gh.data_ptr() if lp.h else None, f)
+    return G, Gh
 
 
 def spmm_split(plan, H_own, H_halo):
@@ -630,10 +503,8 @@ def spmm_split(plan, H_own, H_halo):
     H_halo = _check_feat(plan, H_halo, lp.h, "H_halo")
     f = H_own.shape[1]
     Z = torch.empty((lp.m, f), dtype=torch.float32, device=H_own.device)
-    lib = cabi.load()
-    with torch.cuda.device(H_own.device):
-        cabi.check(lib.pgcn_spmm(plan.handle, 2, H_own.data_ptr(), None, Z.data_ptr(), None, f, _stream_ptr()), plan.handle)
-        cabi.check(lib.pgcn_spmm(plan.handle, 3, None, H_halo.data_ptr(), Z.data_ptr(), None, f, _stream_ptr()), plan.handle)
+    _call(plan, H_own.device, "pgcn_spmm", 2, H_own.data_ptr(), None, Z.data_ptr(), None, f)
+    _call(plan, H_own.device, "pgcn_spmm", 3, None, H_halo.data_ptr(), Z.data_ptr(), None, f)
     return Z
 
 
@@ -642,8 +513,7 @@ def pack_rows(plan, H_own):
     H_own = _check_feat(plan, H_own, plan.lp.m, "H_own")
     f = H_own.shape[1]
     slab = torch.empty((plan.lp.S, f), dtype=torch.float32, device=H_own.device)
-    with torch.cuda.device(H_own.device):
-        cabi.check(cabi.load().pgcn_pack(plan.handle, H_own.data_ptr(), slab.data_ptr(), f, _stream_ptr()), plan.handle)
+    _call(plan, H_own.device, "pgcn_pack", H_own.data_ptr(), slab.data_ptr(), f)
     return slab
 
 
@@ -655,10 +525,8 @@ def exchange_rows(plan, send_slab, backward=False):
     send_slab = _check_feat(plan, send_slab, rows_out, "send_slab")
     f = send_slab.shape[1]
     recv = torch.empty((rows_in, f), dtype=torch.float32, device=send_slab.device)
-    with torch.cuda.device(send_slab.device):
-        cabi.check(cabi.load().pgcn_exchange(plan.handle, send_slab.data_ptr(), recv.data_ptr(), f,
-                                             1 if backward else 0, _stream_ptr()), plan.handle)
-    plan.count_exchange(backward=backward)
+    _call(plan, send_slab.device, "pgcn_exchange", send_slab.data_ptr(), recv.data_ptr(), f, 1 if backward else 0,
+          exchange=backward)
     return recv
 
 
@@ -669,9 +537,7 @@ def unpack_add(plan, recv_slab, G_own):
         # in/out argument: a silent .contiguous() copy would accumulate into a temporary and leave G_own unchanged
         raise ValueError("G_own is updated in place and must be contiguous")
     G_own = _check_feat(plan, G_own, plan.lp.m, "G_own")
-    with torch.cuda.device(G_own.device):
-        cabi.check(cabi.load().pgcn_unpack_add(plan.handle, recv_slab.data_ptr(), G_own.data_ptr(),
-                                               G_own.shape[1], _stream_ptr()), plan.handle)
+    _call(plan, G_own.device, "pgcn_unpack_add", recv_slab.data_ptr(), G_own.data_ptr(), G_own.shape[1])
     return G_own
 
 

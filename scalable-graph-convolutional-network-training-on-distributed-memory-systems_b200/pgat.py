@@ -24,19 +24,13 @@ er[:, h] = Z_h a[d:, h] for head h's slice Z_h of Z (op.PGATMultiHeadAttention).
 (Linear(f, f, bias=False)) and att (K x d), drawn in that order, each xavier_normal with the relu gain; the layer is
 PyG GATv2Conv(share_weights=False, concat=True, bias=False, add_self_loops=False) over the stored pattern.
 """
-import getopt
-import os
 import sys
-import time
 
 import torch
-import torch.distributed as dist
 import torch.nn as nn
-import torch.nn.functional as F
 
-from . import graphio, plan as planmod
 from .op import HEADS, PGATAttention, PGATMultiHeadAttention, PGATv2Attention
-from .pgcn import average_gradients, initialize_parameters, init_process
+from .pgcn import launch, parse_args, train
 
 
 class PGAT(nn.Module):
@@ -97,111 +91,33 @@ class PGATv2(nn.Module):
 
 def run(rank, size, nlayers, nfeatures, path_A, path_partvec, backend, transport="auto", out=sys.stdout, seed=None,
         negative_slope=1.0, epochs=50, heads=1, v2=False):
-    if backend != "nccl":
-        raise RuntimeError("backend '%s': the H100 PGAT path runs on CUDA devices over NCCL/NVLink only "
-                           "(no CPU fallback); use -b nccl" % backend)
-    device = torch.device("cuda", rank % torch.cuda.device_count())
-    torch.cuda.set_device(device)
-    A = graphio.read_adjacency(path_A)
-    partvec = graphio.read_partvec(path_partvec, A.shape[0])
-    graphio.check_partvec(partvec, size)
-    lp_host = planmod.build_local_plan(A, partvec, rank, size)
-    n = lp_host.n
-    # the multi-head backward gets d_er from an aggregation of width 4 K (PGATMultiHeadAttention)
-    plan = planmod.PgcnPlan(lp_host, nfeatures if heads == 1 or v2 else max(nfeatures, 4 * heads), device=device)
-    used = plan.init_comm(transport=transport)
-    plan.bind_values()
-    lp = plan.lp
-
-    own = torch.from_numpy(lp.owned).to(device)
-    H = own.to(torch.float32).unsqueeze(1).repeat(1, nfeatures).contiguous().requires_grad_(True)
-    labels = own % nfeatures
-
-    if seed is not None:
-        torch.manual_seed(seed)
     layer = PGATv2 if v2 else PGAT
-    model = nn.Sequential(*[layer(plan, nfeatures, nfeatures, negative_slope, heads) for _ in range(nlayers)]).to(device)
-    if size > 1:
-        initialize_parameters(model, size)
-    optimizer = torch.optim.Adam(model.parameters(), lr=1e-3)
+    # the multi-head backward gets d_er from an aggregation of width 4 K (PGATMultiHeadAttention)
+    f_max = nfeatures if heads == 1 or v2 else max(nfeatures, 4 * heads)
+    return train(rank, size, nlayers, nfeatures, path_A, path_partvec, backend, "PGAT",
+                 lambda plan: layer(plan, nfeatures, nfeatures, negative_slope, heads), f_max, True,
+                 transport=transport, out=out, seed=seed, epochs=epochs)
 
-    torch.cuda.synchronize()
-    start = time.time()
-    losses = []
-    for ep in range(epochs):
-        logits = model(H)
-        loss = F.nll_loss(F.log_softmax(logits, 1), labels, reduction="sum") / n
-        optimizer.zero_grad()
-        loss.backward()
-        if size > 1:
-            average_gradients(model, size)
-        optimizer.step()
-        total = loss.detach().clone()
-        if size > 1:
-            dist.all_reduce(total, op=dist.ReduceOp.SUM)
-        losses.append(float(total))
-        if rank == 0:
-            print("Epoch {:05d} | Loss {:.4f}".format(ep, losses[-1]), file=out, flush=True)
-    torch.cuda.synchronize()
-    elapsed = torch.tensor([time.time() - start], device=device)
-    if size > 1:
-        dist.all_reduce(elapsed, op=dist.ReduceOp.MAX)
-    if rank == 0:
-        print("Elapsed time {:.4f}".format(elapsed.item()), file=out, flush=True)
-    result = {"losses": losses, "elapsed": float(elapsed.item()), "transport": used, "stats": dict(plan.stats)}
-    plan.close()
-    return result
+
+USAGE = ("usage: PGAT.py -a <A.mtx> -p <partvec> -b nccl -s <nparts> -l <nlayers> -f <nfeatures> "
+         "[--seed N] [--negative-slope S] [--heads 1|2|4|8, dividing nfeatures] [--v2]")
+
+
+def _heads(arg):
+    try:
+        return int(arg)
+    except ValueError:
+        return -1                         # refused with the usage text, as any other head count outside HEADS
+
+
+def _valid(size, nlayers, nfeatures, kw):
+    heads = kw.get("heads", 1)
+    return heads in HEADS and nfeatures % heads == 0
 
 
 def main(argv):
-    size = int(os.environ.get("SLURM_NPROCS", os.environ.get("WORLD_SIZE", "1")))
-    rank = int(os.environ.get("SLURM_PROCID", os.environ.get("RANK", "0")))
-    os.environ["RANK"] = str(rank)
-    try:
-        opts, _ = getopt.getopt(argv, "a:p:b:s:l:f:", ["transport=", "seed=", "negative-slope=", "heads=", "v2"])
-    except getopt.GetoptError:
-        print("a:p:b:", flush=True)                                       # the reference's usage text
-        sys.exit(2)
-    path_A = path_partvec = None
-    backend = "nccl"
-    nlayers = nfeatures = None
-    kw = {}
-    for opt, arg in opts:
-        if opt == "-a":
-            path_A = arg
-        elif opt == "-p":
-            path_partvec = arg
-        elif opt == "-b":
-            backend = arg
-        elif opt == "-s":
-            size = int(arg)
-        elif opt == "-l":
-            nlayers = int(arg)
-        elif opt == "-f":
-            nfeatures = int(arg)
-        elif opt == "--transport":
-            kw["transport"] = arg
-        elif opt == "--seed":
-            kw["seed"] = int(arg)
-        elif opt == "--negative-slope":
-            kw["negative_slope"] = float(arg)
-        elif opt == "--v2":
-            kw["v2"] = True
-        elif opt == "--heads":
-            try:
-                kw["heads"] = int(arg)
-            except ValueError:
-                kw["heads"] = -1
-    heads = kw.get("heads", 1)
-    if (path_A is None or path_partvec is None or nlayers is None or nfeatures is None or heads not in HEADS
-            or nfeatures % heads):
-        print("usage: PGAT.py -a <A.mtx> -p <partvec> -b nccl -s <nparts> -l <nlayers> -f <nfeatures> "
-              "[--seed N] [--negative-slope S] [--heads 1|2|4|8, dividing nfeatures] [--v2]", flush=True)
-        sys.exit(2)
-    os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
-    os.environ.setdefault("MASTER_PORT", "29500")
-    os.environ["WORLD_SIZE"] = str(size)
-    init_process(rank, size, run, nlayers, nfeatures, path_A, path_partvec, backend, **kw)
+    options = {"--negative-slope": ("negative_slope", float), "--heads": ("heads", _heads), "--v2": ("v2", None)}
+    launch(run, *parse_args(argv, USAGE, options, _valid))
 
 
 if __name__ == "__main__":

@@ -29,7 +29,7 @@ import torch.distributed as dist
 import torch.nn as nn
 import torch.nn.functional as F
 
-from . import graphio, plan as planmod
+from . import plan as planmod
 from .op import PSpMM, PSpMMRelu, communicate_fgm, spmm_local, aggregate_backward
 
 
@@ -79,6 +79,69 @@ def initialize_parameters(model, world_size):
         param.data /= world_size
 
 
+def _cuda_device(rank, backend, name):
+    if backend != "nccl":
+        raise RuntimeError("backend '%s': the H100 %s path runs on CUDA devices over NCCL/NVLink only "
+                           "(no CPU fallback); use -b nccl" % (backend, name))
+    device = torch.device("cuda", rank % torch.cuda.device_count())      # GPU/PGCN.py:169
+    torch.cuda.set_device(device)
+    return device
+
+
+def train(rank, size, nlayers, nfeatures, path_A, path_partvec, backend, name, layer, f_max, grad_H,
+          transport="auto", out=sys.stdout, seed=None, epochs=50):
+    """The training loop of PGAT.py and PSAGE.py (`name`): a bound plan of width f_max, inputs H[i, :] = i (requiring
+    grad when grad_H) and labels i % f, nlayers layers `layer(plan)` (f -> f) built under `seed` and averaged over
+    ranks, Adam lr 1e-3, `epochs` epochs of the loss sum_owned nll / n with gradients averaged over ranks. Rank 0 prints
+    `Epoch {:05d} | Loss {:.4f}` (the all-reduced loss) per epoch and `Elapsed time {:.4f}`. Returns the losses, the
+    elapsed time, the transport and plan.stats."""
+    device = _cuda_device(rank, backend, name)
+    lp_host = planmod.read_local_plan(path_A, path_partvec, rank, size)
+    n = lp_host.n
+    plan = planmod.PgcnPlan(lp_host, f_max, device=device)
+    used = plan.init_comm(transport=transport)
+    plan.bind_values()
+    lp = plan.lp
+
+    own = torch.from_numpy(lp.owned).to(device)
+    H = own.to(torch.float32).unsqueeze(1).repeat(1, nfeatures).contiguous().requires_grad_(grad_H)
+    labels = own % nfeatures
+
+    if seed is not None:
+        torch.manual_seed(seed)
+    model = nn.Sequential(*[layer(plan) for _ in range(nlayers)]).to(device)
+    if size > 1:
+        initialize_parameters(model, size)
+    optimizer = torch.optim.Adam(model.parameters(), lr=1e-3)
+
+    torch.cuda.synchronize()
+    start = time.time()
+    losses = []
+    for ep in range(epochs):
+        logits = model(H)
+        loss = F.nll_loss(F.log_softmax(logits, 1), labels, reduction="sum") / n
+        optimizer.zero_grad()
+        loss.backward()
+        if size > 1:
+            average_gradients(model, size)
+        optimizer.step()
+        total = loss.detach().clone()
+        if size > 1:
+            dist.all_reduce(total, op=dist.ReduceOp.SUM)
+        losses.append(float(total))
+        if rank == 0:
+            print("Epoch {:05d} | Loss {:.4f}".format(ep, losses[-1]), file=out, flush=True)
+    torch.cuda.synchronize()
+    elapsed = torch.tensor([time.time() - start], device=device)
+    if size > 1:
+        dist.all_reduce(elapsed, op=dist.ReduceOp.MAX)
+    if rank == 0:
+        print("Elapsed time {:.4f}".format(elapsed.item()), file=out, flush=True)
+    result = {"losses": losses, "elapsed": float(elapsed.item()), "transport": used, "stats": dict(plan.stats)}
+    plan.close()
+    return result
+
+
 def reference_loss(logits_own, labels_own, n):
     """F.nll_loss(log_softmax(logits), labels) over ALL n rows as the reference computes it
     (GPU/PGCN.py:204-205), from the owned rows: non-owned rows are all-zero logits -> nll = log f."""
@@ -89,19 +152,12 @@ def reference_loss(logits_own, labels_own, n):
 
 def run(rank, size, nlayers, nfeatures, path_A, path_partvec, backend, ref_quirks=False, transport="auto",
         out=sys.stdout, seed=None, fused=False):
-    if backend != "nccl":
-        raise RuntimeError("backend '%s': the H100 PGCN path runs on CUDA devices over NCCL/NVLink only "
-                           "(no CPU fallback); use -b nccl" % backend)
-    device = torch.device("cuda", rank % torch.cuda.device_count())      # GPU/PGCN.py:169
-    torch.cuda.set_device(device)
+    device = _cuda_device(rank, backend, "PGCN")
     cache = os.environ.get("PGCN_PLAN_CACHE")
     if cache:                                                            # optional on-disk plan cache (§8f rank 2)
         lp_host = planmod.cached_local_plan(path_A, path_partvec, rank, size, cache)
     else:
-        A = graphio.read_adjacency(path_A)                               # :171
-        partvec = graphio.read_partvec(path_partvec, A.shape[0])         # :172-173
-        graphio.check_partvec(partvec, size)
-        lp_host = planmod.build_local_plan(A, partvec, rank, size)       # :175-176
+        lp_host = planmod.read_local_plan(path_A, path_partvec, rank, size)
     n = lp_host.n
     plan = planmod.PgcnPlan(lp_host, nfeatures, device=device)           # :178-182
     if ref_quirks:
@@ -171,14 +227,21 @@ def init_process(rank, size, fn, nlayers, nfeatures, path_A, path_partvec, backe
         dist.destroy_process_group()
 
 
-def main(argv):
-    size = int(os.environ.get("SLURM_NPROCS", os.environ.get("WORLD_SIZE", "1")))      # GPU/PGCN.py:258-260
+def parse_args(argv, usage, options=None, valid=None, unknown_flag_text="a:p:b:"):
+    """The command line of every trainer: rank and size from SLURM_PROCID / SLURM_NPROCS (GPU/PGCN.py:258-260) with
+    torchrun's RANK / WORLD_SIZE as a fallback, the flags -a -p -b -s -l -f (:262-278), --transport, --seed and the
+    trainer's own `options`, {"--name": (keyword, type)} with type None for a switch. Returns (rank, size, args, kw):
+    the positional arguments of `run` after rank and size, and its keywords. An unknown flag prints `unknown_flag_text`
+    (by default the reference's, :264); a missing flag, or options that valid(size, nlayers, nfeatures, kw) refuses,
+    print `usage`; both exit with status 2. A malformed number raises ValueError."""
+    size = int(os.environ.get("SLURM_NPROCS", os.environ.get("WORLD_SIZE", "1")))
     rank = int(os.environ.get("SLURM_PROCID", os.environ.get("RANK", "0")))
     os.environ["RANK"] = str(rank)
+    options = dict(options or {}, **{"--transport": ("transport", str), "--seed": ("seed", int)})
     try:
-        opts, _ = getopt.getopt(argv, "a:p:b:s:l:f:", ["ref-quirks", "transport=", "seed=", "fused"])
+        opts, _ = getopt.getopt(argv, "a:p:b:s:l:f:", [o[2:] + ("=" if t else "") for o, (_, t) in options.items()])
     except getopt.GetoptError:
-        print("a:p:b:", flush=True)                                       # the reference's usage text, :264
+        print(unknown_flag_text, flush=True)
         sys.exit(2)
     path_A = path_partvec = None
     backend = "nccl"
@@ -197,21 +260,31 @@ def main(argv):
             nlayers = int(arg)
         elif opt == "-f":
             nfeatures = int(arg)
-        elif opt == "--ref-quirks":
-            kw["ref_quirks"] = True
-        elif opt == "--transport":
-            kw["transport"] = arg
-        elif opt == "--seed":
-            kw["seed"] = int(arg)
-        elif opt == "--fused":
-            kw["fused"] = True           # relu(A (H W^T)) with the clamp fused into the aggregation (SURVEY §8f rank 1)
-    if path_A is None or path_partvec is None or nlayers is None or nfeatures is None:
-        print("usage: PGCN.py -a <A.mtx> -p <partvec> -b nccl -s <nparts> -l <nlayers> -f <nfeatures>", flush=True)
+        else:
+            key, typ = options[opt]
+            kw[key] = typ(arg) if typ else True
+    if (path_A is None or path_partvec is None or nlayers is None or nfeatures is None
+            or (valid is not None and not valid(size, nlayers, nfeatures, kw))):
+        print(usage, flush=True)
         sys.exit(2)
+    return rank, size, (nlayers, nfeatures, path_A, path_partvec, backend), kw
+
+
+def launch(fn, rank, size, args, kw):
+    """fn(rank, size, *args, **kw) in the process group, with the rendezvous at MASTER_ADDR / MASTER_PORT (default
+    127.0.0.1:29500)."""
     os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
     os.environ.setdefault("MASTER_PORT", "29500")
     os.environ["WORLD_SIZE"] = str(size)
-    init_process(rank, size, run, nlayers, nfeatures, path_A, path_partvec, backend, **kw)
+    init_process(rank, size, fn, *args, **kw)
+
+
+USAGE = "usage: PGCN.py -a <A.mtx> -p <partvec> -b nccl -s <nparts> -l <nlayers> -f <nfeatures>"
+
+
+def main(argv):
+    # --fused: relu(A (H W^T)) with the clamp fused into the aggregation (SURVEY §8f rank 1)
+    launch(run, *parse_args(argv, USAGE, {"--ref-quirks": ("ref_quirks", None), "--fused": ("fused", None)}))
 
 
 if __name__ == "__main__":

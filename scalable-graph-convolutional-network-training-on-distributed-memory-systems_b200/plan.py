@@ -175,11 +175,19 @@ def load_local_plan(path):
     return lp
 
 
+def read_local_plan(path_A, path_partvec, rank, size):
+    """build_local_plan of the MatrixMarket matrix at path_A and the part vector at path_partvec, which must name a
+    part below `size` for every row (GPU/PGCN.py:171-176)."""
+    from . import graphio
+    A = graphio.read_adjacency(path_A)
+    pv = graphio.check_partvec(graphio.read_partvec(path_partvec, A.shape[0]), size)
+    return build_local_plan(A, pv, rank, size)
+
+
 def cached_local_plan(path_A, path_partvec, rank, size, cache_dir):
     """build_local_plan with an on-disk cache keyed by the two input files (size + mtime), rank and size."""
     import hashlib
     import os
-    from . import graphio
     sa, sp_ = os.stat(path_A), os.stat(path_partvec)
     key = hashlib.sha1(repr([PLAN_FORMAT_VERSION, os.path.abspath(path_A), sa.st_size, sa.st_mtime_ns,
                              os.path.abspath(path_partvec), sp_.st_size, sp_.st_mtime_ns,
@@ -190,9 +198,7 @@ def cached_local_plan(path_A, path_partvec, rank, size, cache_dir):
         lp = load_local_plan(path)
         if lp.k == size and lp.rank == rank:
             return lp
-    A = graphio.read_adjacency(path_A)
-    pv = graphio.check_partvec(graphio.read_partvec(path_partvec, A.shape[0]), size)
-    lp = build_local_plan(A, pv, rank, size)
+    lp = read_local_plan(path_A, path_partvec, rank, size)
     tmp = path + ".%d.tmp.npz" % os.getpid()
     save_local_plan(tmp, lp)
     os.replace(tmp, path)
