@@ -41,6 +41,24 @@ def inputs(n, f):
     return np.repeat(np.arange(n, dtype=np.float64)[:, None], f, axis=1), np.arange(n) % f
 
 
+def train(params, logits, n, f, k, epochs, lr):
+    """The loss curve the trainers print: sum_all nll / n against the labels of inputs(n, f), gradients averaged over
+    k ranks, Adam(lr). params: per layer, a tuple of fp64 leaf tensors; logits(params) gives the n x f output."""
+    labels = torch.from_numpy(inputs(n, f)[1])
+    flat = [t for p in params for t in p]
+    opt = torch.optim.Adam(flat, lr=lr)
+    losses = []
+    for _ in range(epochs):
+        loss = F.nll_loss(F.log_softmax(logits(params), 1), labels, reduction="sum") / n
+        opt.zero_grad()
+        loss.backward()
+        for t in flat:
+            t.grad /= k
+        opt.step()
+        losses.append(float(loss))
+    return losses
+
+
 # ---- intended semantics --------------------------------------------------------------------------------------------
 
 def edge_softmax(rows, scores, n):
@@ -79,23 +97,10 @@ def intended_training(A, nlayers, f, seed, slope, k=1, epochs=50, lr=1e-3):
     n = A.shape[0]
     A = sp.csr_matrix(A)
     A.sum_duplicates()
-    H, labels = inputs(n, f)
-    labels = torch.from_numpy(labels)
+    H, _ = inputs(n, f)
     params = [(torch.tensor(W, requires_grad=True), torch.tensor(a, requires_grad=True))
               for W, a in init_params(nlayers, f, seed)]
-    flat = [t for p in params for t in p]
-    opt = torch.optim.Adam(flat, lr=lr)
-    losses = []
-    for _ in range(epochs):
-        logits = intended_forward(A, H, params, slope)
-        loss = F.nll_loss(F.log_softmax(logits, 1), labels, reduction="sum") / n
-        opt.zero_grad()
-        loss.backward()
-        for t in flat:
-            t.grad /= k
-        opt.step()
-        losses.append(float(loss))
-    return losses
+    return train(params, lambda ps: intended_forward(A, H, ps, slope), n, f, k, epochs, lr)
 
 
 # ---- literal semantics (the reference's computation on one rank) --------------------------------------------------

@@ -93,22 +93,12 @@ def intended_training(A, nlayers, f, seed, slope, heads, k=1, epochs=50, lr=1e-3
     A.sum_duplicates()
     C = A.tocoo()
     rows, cols = torch.from_numpy(C.row.astype(np.int64)), torch.from_numpy(C.col.astype(np.int64))
-    H, labels = po.inputs(n, f)
-    X0 = torch.as_tensor(H, dtype=torch.float64)
-    labels = torch.from_numpy(labels)
+    X0 = torch.as_tensor(po.inputs(n, f)[0], dtype=torch.float64)
     params = [tuple(torch.tensor(x, requires_grad=True) for x in layer) for layer in init_params(nlayers, f, seed, heads)]
-    flat = [t for p in params for t in p]
-    opt = torch.optim.Adam(flat, lr=lr)
-    losses = []
-    for _ in range(epochs):
+
+    def logits(ps):
         X = X0
-        for Wl, Wr, att in params:
+        for Wl, Wr, att in ps:
             X = forward_torch(rows, cols, n, X @ Wl.T, X @ Wr.T, att, slope)
-        loss = F.nll_loss(F.log_softmax(X, 1), labels, reduction="sum") / n
-        opt.zero_grad()
-        loss.backward()
-        for t in flat:
-            t.grad /= k
-        opt.step()
-        losses.append(float(loss))
-    return losses
+        return X
+    return po.train(params, logits, n, f, k, epochs, lr)

@@ -11,7 +11,6 @@ import numpy as np
 import scipy.sparse as sp
 import torch
 import torch.nn as nn
-import torch.nn.functional as F
 
 from oracle import pgat_oracle as po
 
@@ -72,20 +71,7 @@ def intended_training(A, nlayers, f, seed, slope, k=1, epochs=50, lr=1e-3, heads
     n = A.shape[0]
     A = sp.csr_matrix(A)
     A.sum_duplicates()
-    H, labels = po.inputs(n, f)
-    labels = torch.from_numpy(labels)
+    H, _ = po.inputs(n, f)
     params = [(torch.tensor(W, requires_grad=True), torch.tensor(a, requires_grad=True))
               for W, a in init_params(nlayers, f, seed, heads)]
-    flat = [t for p in params for t in p]
-    opt = torch.optim.Adam(flat, lr=lr)
-    losses = []
-    for _ in range(epochs):
-        logits = intended_forward(A, H, params, slope, heads)
-        loss = F.nll_loss(F.log_softmax(logits, 1), labels, reduction="sum") / n
-        opt.zero_grad()
-        loss.backward()
-        for t in flat:
-            t.grad /= k
-        opt.step()
-        losses.append(float(loss))
-    return losses
+    return po.train(params, lambda ps: intended_forward(A, H, ps, slope, heads), n, f, k, epochs, lr)

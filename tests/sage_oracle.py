@@ -12,6 +12,8 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from oracle import pgat_oracle as po
+
 
 def max_aggregate(rowptr, colidx, X):
     """(Z, arg): Z [rows, f] in X's dtype, arg [rows, f] int32 entry indices into colidx (-1 and Z = 0 for empty rows)."""
@@ -75,22 +77,8 @@ def intended_forward(A, H, params):
 
 
 def intended_training(A, nlayers, f, seed, k=1, epochs=50, lr=1e-3):
-    """The loss curve sage.run prints: inputs H[i, :] = i, labels i % f, loss sum_all nll / n, gradients averaged over
-    k ranks, Adam(lr)."""
+    """The loss curve sage.run prints: inputs H[i, :] = i (pgat_oracle.inputs) and pgat_oracle.train's loop."""
     n = A.shape[0]
-    H = np.repeat(np.arange(n, dtype=np.float64)[:, None], f, axis=1)
-    labels = torch.from_numpy(np.arange(n) % f)
+    H, _ = po.inputs(n, f)
     params = [tuple(torch.tensor(t, requires_grad=True) for t in p) for p in init_params(nlayers, f, seed)]
-    flat = [t for p in params for t in p]
-    opt = torch.optim.Adam(flat, lr=lr)
-    losses = []
-    for _ in range(epochs):
-        logits = intended_forward(A, H, params)
-        loss = F.nll_loss(F.log_softmax(logits, 1), labels, reduction="sum") / n
-        opt.zero_grad()
-        loss.backward()
-        for t in flat:
-            t.grad /= k
-        opt.step()
-        losses.append(float(loss.detach()))
-    return losses
+    return po.train(params, lambda ps: intended_forward(A, H, ps), n, f, k, epochs, lr)

@@ -9,68 +9,18 @@ op.PGATAttention and the PGAT command line.
   * PSpMM after attention equals a fresh plan; CUDA-graph capture of the layer on one and two ranks, and its refusal
     before pgcn_plan_prepare; PGAT.py follows the fp64 loss curve of oracle/pgat_oracle.py.
 """
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 import scipy.sparse as sp
 import torch
 
-from conftest import ROOT
-from helpers import GOLDEN, Golden
+from harness import (EPS, assert_follows, check_one_rank_capture, check_two_rank_capture, dev, edges, karate,
+                     linked_plans, one_rank_plan, problem, run_cli, run_ranks, stream, t)
 from oracle import pgat_oracle as po
-from pgcn_b200 import cabi, graphio, plan as planmod
+from pgcn_b200 import cabi, plan as planmod
 from pgcn_b200.op import PGATAttention, PSpMM
 
 pytestmark = pytest.mark.gpu
-EPS = 2.0 ** -24
-
-
-def dev():
-    if not torch.cuda.is_available():
-        pytest.fail("no CUDA device: -m gpu tests must run on a GPU machine")
-    return torch.device("cuda", 0)
-
-
-def stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def hub_graph():
-    """R-MAT (6000 vertices) with a hub row of 3000 entries, rows of one entry (rows 20..29) and empty rows (10..19)."""
-    A = sp.coo_matrix(graphio.synthetic_graph(6000, 120000, seed=31))
-    keep = (A.row < 10) | (A.row >= 30)
-    row = np.concatenate([A.row[keep], np.zeros(3000, np.int64), np.arange(20, 30)])
-    col = np.concatenate([A.col[keep], np.arange(3000) * 2, np.arange(20, 30) + 100])
-    val = np.ones(len(row), np.float32)
-    B = sp.csr_matrix((val, (row, col)), shape=A.shape)
-    B.sum_duplicates()
-    return B.tocoo()
-
-
-def problem(case):
-    if case == "hub":
-        A = hub_graph()
-        return A, np.zeros(A.shape[0], dtype=np.int64), 1
-    if case == "karate":
-        z = np.load(os.path.join(GOLDEN, "pgat_karate_k3.npz"))
-        n = int(z["n"])
-        return sp.coo_matrix((z["val"], (z["row"], z["col"])), shape=(n, n)), z["partvec"].astype(np.int64), 3
-    g = Golden(case)
-    return g.A, g.partvec, g.k
-
-
-def edges(lp):
-    return np.repeat(np.arange(lp.m), np.diff(lp.rowptr.astype(np.int64))), lp.colidx.astype(np.int64)
-
-
-def one_rank_plan(case, f):
-    A, _, _ = problem(case)
-    plan = planmod.build_plan(A, np.zeros(A.shape[0], dtype=np.int64), 0, 1, f, device=dev())
-    plan.bind_values()
-    return A, plan
 
 
 @pytest.mark.parametrize("case", ["gemat11_k1", "karate", "hub"])
@@ -87,7 +37,6 @@ def test_softmax_kernels_within_fp32_bound_and_deterministic(case, slope, scale)
     er = rs.uniform(-scale, scale, lp.m).astype(np.float32)
     dal = rs.uniform(-1, 1, lp.nnz()).astype(np.float32)
     lib = cabi.load()
-    t = lambda x: torch.from_numpy(x).to(dev())
     el_d, er_d, dal_d = t(el), t(er), t(dal)
     runs = []
     for _ in range(2):
@@ -186,25 +135,6 @@ def test_layer_gradients_one_rank(case, f, layout):
     plan.close()
 
 
-def make_plans(lps, f, overlap):
-    plans = [planmod.PgcnPlan(lp, f, device=dev()) for lp in lps]
-    planmod.link_local_plans(plans)
-    for p in plans:
-        p.set_option("overlap", overlap)
-        p.bind_values()
-    return plans
-
-
-def run_ranks(plans, fn, streams):
-    torch.cuda.synchronize()
-    out = [None] * len(plans)
-    for r, s in enumerate(streams):
-        with torch.cuda.stream(s):
-            out[r] = fn(r)
-    torch.cuda.synchronize()
-    return out
-
-
 @pytest.mark.parametrize("overlap", [0, 1])
 @pytest.mark.parametrize("case,f", [("gemat11_k2", 40), ("gemat11_k2", 128), ("gemat11_k3_hp", 256),
                                     ("karate", 16)])
@@ -212,17 +142,17 @@ def test_layer_gradients_multi_rank(case, f, overlap):
     A, pv, k = problem(case)
     n = A.shape[0]
     lps = [planmod.build_local_plan(A, pv, r, k) for r in range(k)]
-    plans = make_plans(lps, f, overlap)
+    plans = linked_plans(lps, f, overlap)
     streams = [torch.cuda.Stream(device=dev()) for _ in plans]
     rs = np.random.RandomState(f + k)
     Zn = rs.uniform(-1, 1, size=(n, f)).astype(np.float32)
     Gn = rs.uniform(-1, 1, size=(n, f)).astype(np.float32)
     eln = rs.uniform(-3, 3, n).astype(np.float32)
     ern = rs.uniform(-3, 3, n).astype(np.float32)
-    t = lambda x, lp: torch.from_numpy(x[lp.owned]).to(dev()).requires_grad_(True)
-    Z = [t(Zn, lp) for lp in lps]
-    el = [t(eln, lp) for lp in lps]
-    er = [t(ern, lp) for lp in lps]
+    own = lambda x, lp: t(x[lp.owned]).requires_grad_(True)
+    Z = [own(Zn, lp) for lp in lps]
+    el = [own(eln, lp) for lp in lps]
+    er = [own(ern, lp) for lp in lps]
     out = run_ranks(plans, lambda r: PGATAttention.apply(plans[r], Z[r], el[r], er[r], 0.2), streams)
     run_ranks(plans, lambda r: out[r].backward(torch.from_numpy(Gn[lps[r].owned]).to(dev())), streams)
     C = sp.csr_matrix(A)
@@ -245,7 +175,7 @@ def test_halo_rows_bit_exact_across_parities(w):
     A, pv, k = problem("gemat11_k3_hp")
     n = A.shape[0]
     lps = [planmod.build_local_plan(A, pv, r, k) for r in range(k)]
-    plans = make_plans(lps, 128, 1)
+    plans = linked_plans(lps, 128, 1)
     streams = [torch.cuda.Stream(device=dev()) for _ in plans]
     lib = cabi.load()
     rs = np.random.RandomState(w)
@@ -303,32 +233,28 @@ def test_one_rank_capture_and_refusal_before_prepare():
     A, plan = one_rank_plan("hub", 128)
     f, n = 128, A.shape[0]
     rs = np.random.RandomState(11)
-    t = lambda *s: torch.from_numpy(rs.uniform(-1, 1, size=s).astype(np.float32)).to(dev())
+    rnd = lambda *s: t(rs.uniform(-1, 1, size=s).astype(np.float32))
     x, g = torch.zeros((n, f), device=dev()), torch.zeros((n, f), device=dev())
     W = torch.zeros((f, f), device=dev(), requires_grad=True)
     a = torch.zeros((2 * f, 1), device=dev(), requires_grad=True)
-    s = torch.cuda.Stream()
-    with pytest.raises(RuntimeError, match="pgcn_plan_prepare"):
-        with torch.cuda.graph(torch.cuda.CUDAGraph(), stream=s):
-            layer_step(plan, f, x, W, a, g)
-    W.grad = a.grad = None
-    plan.prepare(f)
-    plan.prepare(4)
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        out = layer_step(plan, f, x, W, a, g)
-    ins = [(t(n, f), t(n, f), t(f, f) * 0.1, t(2 * f, 1) * 0.1) for _ in range(3)]
-    for i in (0, 1, 2, 1):
-        xi, gi, Wi, ai = ins[i]
+    ins = [(rnd(n, f), rnd(n, f), rnd(f, f) * 0.1, rnd(2 * f, 1) * 0.1) for _ in range(3)]
+
+    def step():
+        return dict(out=layer_step(plan, f, x, W, a, g), dW=W.grad, da=a.grad)
+
+    def load(i):
         with torch.no_grad():
-            x.copy_(xi); g.copy_(gi); W.copy_(Wi); a.copy_(ai)
-        graph.replay()
-        got = [u.detach().clone() for u in (out, W.grad, a.grad)]
+            for u, v in zip((x, g, W, a), ins[i]):
+                u.copy_(v)
+
+    def eager(i):
+        xi, gi, Wi, ai = ins[i]
         We, ae = Wi.clone().requires_grad_(True), ai.clone().requires_grad_(True)
         oe = layer_step(plan, f, xi, We, ae, gi)
         PSpMM.apply(plan, xi)                                  # the creation values in between
-        for name, u, w in zip(("out", "dW", "da"), got, (oe, We.grad, ae.grad)):
-            assert torch.equal(u, w.detach()), "replay %d: %s differs from eager" % (i, name)
+        return dict(out=oe, dW=We.grad, da=ae.grad)
+
+    check_one_rank_capture(plan, step, load, eager, prepare=(f, 4), leaves=(W, a))
     plan.close()
 
 
@@ -336,7 +262,7 @@ def test_two_rank_capture_over_the_peer_transport():
     A, pv, k = problem("gemat11_k2")
     f, n = 128, A.shape[0]
     lps = [planmod.build_local_plan(A, pv, r, k) for r in range(k)]
-    plans = make_plans(lps, f, 1)
+    plans = linked_plans(lps, f, 1)
     for p in plans:
         p.prepare(f)
         p.prepare(4)
@@ -361,51 +287,14 @@ def test_two_rank_capture_over_the_peer_transport():
                 b["W"].copy_(torch.from_numpy(Wn)); b["a"].copy_(torch.from_numpy(an))
         torch.cuda.synchronize()
 
-    cap = [buffers(r) for r in range(k)]
-    graphs, outs = [], []
-    for r in range(k):
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph, stream=streams[r]):
-            b = cap[r]
-            outs.append(layer_step(plans[r], f, b["x"], b["W"], b["a"], b["g"]))
-        graphs.append(graph)
-    lib = cabi.load()
-    for step, i in enumerate((0, 1, 2, 1)):
-        load(cap, i)
-        run_ranks(plans, lambda r: graphs[r].replay(), streams)
-        got = [(outs[r].detach().clone(), cap[r]["W"].grad.clone(), cap[r]["a"].grad.clone()) for r in range(k)]
-        eager = [buffers(r) for r in range(k)]
-        load(eager, i)
-        res = run_ranks(plans, lambda r: layer_step(plans[r], f, eager[r]["x"], eager[r]["W"], eager[r]["a"],
-                                                    eager[r]["g"]), streams)
-        for r in range(k):
-            for name, u, w in zip(("out", "dW", "da"), got[r], (res[r], eager[r]["W"].grad, eager[r]["a"].grad)):
-                assert torch.equal(u, w.detach()), "step %d rank %d: %s replay differs from eager" % (step, r, name)
-        if step == 1:                                  # one more fused call: the later replays see the other parity
-            run_ranks(plans, lambda r: cabi.check(lib.pgcn_forward(plans[r].handle, eager[r]["x"].data_ptr(),
-                                                                   torch.empty_like(eager[r]["x"]).data_ptr(), f,
-                                                                   stream()), plans[r].handle), streams)
+    def step(r, b):
+        return dict(out=layer_step(plans[r], f, b["x"], b["W"], b["a"], b["g"]), dW=b["W"].grad, da=b["a"].grad)
+
+    check_two_rank_capture(plans, streams, buffers, load, step)
     for p in plans:
         p.close()
 
 
 def test_cli_follows_the_fp64_loss_curve(tmp_path):
-    from scipy.io import mmwrite
-    z = np.load(os.path.join(GOLDEN, "pgat_karate_k1.npz"))
-    n = int(z["n"])
-    A = sp.coo_matrix((z["val"], (z["row"], z["col"])), shape=(n, n))
-    a = str(tmp_path / "karate.mtx")
-    mmwrite(a, A)
-    p = str(tmp_path / "karate.mtx.1.rp")
-    graphio.write_partvec(p, np.zeros(n, dtype=np.int64))
-    env = dict(os.environ, SLURM_NPROCS="1", SLURM_PROCID="0", MASTER_ADDR="127.0.0.1", MASTER_PORT="29660")
-    out = subprocess.run([sys.executable, os.path.join(ROOT, "PGAT.py"), "-a", a, "-p", p, "-b", "nccl", "-s", "1",
-                          "-l", "2", "-f", "4", "--seed", "7"], env=env, capture_output=True, text=True, timeout=600)
-    assert out.returncode == 0, out.stderr[-2000:]
-    lines = [l for l in out.stdout.splitlines() if l.startswith("Epoch")]
-    assert [l[:11] for l in lines] == ["Epoch %05d" % i for i in range(50)]
-    assert any(l.startswith("Elapsed time ") for l in out.stdout.splitlines())
-    want = po.intended_training(A, 2, 4, 7, 1.0)
-    # the printed values carry 4 decimals; compare them against the fp64 curve rounded the same way
-    got = [float(l.split("Loss")[1]) for l in lines]
-    np.testing.assert_allclose(got, want, rtol=1e-3, atol=6e-5)
+    lines = run_cli(tmp_path, "PGAT.py", [], 29660)
+    assert_follows(lines, po.intended_training(karate(), 2, 4, 7, 1.0))

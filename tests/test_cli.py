@@ -12,6 +12,7 @@ import pytest
 import torch
 
 from conftest import ROOT
+from harness import TIMEOUT, spawn_ranks
 from helpers import GOLDEN, Golden
 
 
@@ -41,7 +42,8 @@ def test_cli_single_rank_matches_reference_losses(tmp_path):
     a, p, g = _write_inputs(tmp_path, "gemat11_k1")
     env = dict(os.environ, SLURM_NPROCS="1", SLURM_PROCID="0", MASTER_ADDR="127.0.0.1", MASTER_PORT="29650")
     out = subprocess.run([sys.executable, os.path.join(ROOT, "PGCN.py"), "-a", a, "-p", p, "-b", "nccl", "-s", "1",
-                          "-l", "2", "-f", "16", "--seed", "1000"], env=env, capture_output=True, text=True, timeout=600)
+                          "-l", "2", "-f", "16", "--seed", "1000"], env=env, capture_output=True, text=True,
+                         timeout=TIMEOUT)
     assert out.returncode == 0, out.stderr[-2000:]
     ref = json.load(open(os.path.join(GOLDEN, "gemat11_e2e.json")))["k1"]
     losses = [float(l.split("Loss")[1]) for l in out.stdout.splitlines() if l.startswith("Epoch")]
@@ -52,16 +54,12 @@ def test_cli_single_rank_matches_reference_losses(tmp_path):
     assert "'send_volume': 0" in out.stdout
 
 
-def _mg_worker(rank, k, port, a, p, q):
-    try:
-        os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(k))
-        from pgcn_b200 import pgcn
-        buf = io.StringIO()
-        res = pgcn.init_process(rank, k, pgcn.run, 2, 16, a, p, "nccl", ref_quirks=True, seed=1000 + rank, out=buf)
-        q.put((rank, "ok", res, buf.getvalue()))
-    except Exception:
-        import traceback
-        q.put((rank, "ERROR", traceback.format_exc(), ""))
+def _mg_worker(rank, k, port, a, p):
+    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(k))
+    from pgcn_b200 import pgcn
+    buf = io.StringIO()
+    res = pgcn.init_process(rank, k, pgcn.run, 2, 16, a, p, "nccl", ref_quirks=True, seed=1000 + rank, out=buf)
+    return res, buf.getvalue()
 
 
 @pytest.mark.gpu
@@ -73,23 +71,8 @@ def test_cli_multi_rank_matches_reference(tmp_path, k):
     k = 3: statistics exact; the loss is compared loosely (Q3 makes the reference's gradients wrong)."""
     if not torch.cuda.is_available() or torch.cuda.device_count() < k:
         pytest.skip("needs %d GPUs" % k)
-    import torch.multiprocessing as mp
     a, p, g = _write_inputs(tmp_path, "gemat11_k2" if k == 2 else "gemat11_k3_hp")
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    procs = [ctx.Process(target=_mg_worker, args=(r, k, 29660 + k, a, p, q)) for r in range(k)]
-    for pr in procs:
-        pr.start()
-    res = {}
-    for _ in range(k):
-        rank, status, payload, text = q.get(timeout=600)
-        if status != "ok":
-            for pr in procs:
-                pr.kill()
-            pytest.fail("rank %d:\n%s" % (rank, payload))
-        res[rank] = (payload, text)
-    for pr in procs:
-        pr.join(timeout=60)
+    res = spawn_ranks(_mg_worker, k, (29660 + k, a, p))
     ref = json.load(open(os.path.join(GOLDEN, "gemat11_e2e.json")))["k%d" % k]
     out0, text0 = res[0]
     assert out0["total_vol"] == ref["total_vol"] and out0["total_nmsg"] == ref["total_nmsg"]

@@ -20,18 +20,13 @@ import numpy as np
 import pytest
 import torch
 
+from harness import dev, run_ranks, spawn_ranks
 from helpers import GOLDEN, Golden, assert_close_fp32, fp32_tol
 from oracle import pgcn_oracle as orc
 from pgcn_b200 import cabi, graphio, plan as planmod
 from pgcn_b200.op import PSpMM, PSpMMRelu
 
 pytestmark = pytest.mark.gpu
-
-
-def dev():
-    if not torch.cuda.is_available():
-        pytest.fail("no CUDA device: -m gpu tests must run on a GPU machine")
-    return torch.device("cuda", 0)
 
 
 def rand(rs, rows, f):
@@ -154,15 +149,6 @@ def test_refused_capture_enqueues_nothing():
     plan.close()
 
 
-def run_ranks(plans, calls, streams):
-    """Enqueue calls[r]() on streams[r] for every rank (the ranks' kernels wait for each other on the device), sync."""
-    torch.cuda.synchronize()
-    for c, s in zip(calls, streams):
-        with torch.cuda.stream(s):
-            c()
-    torch.cuda.synchronize()
-
-
 @pytest.mark.parametrize("overlap", [1, 0])
 @pytest.mark.parametrize("case", ["gemat11_k2", "gemat11_k3_hp", "karate_k3_hp", "rmat_k4"])
 def test_peer_transport_capture_and_replay(case, overlap):
@@ -216,14 +202,14 @@ def test_peer_transport_capture_and_replay(case, overlap):
         ze = [torch.empty_like(t) for t in xe]
         he = [torch.empty_like(t) for t in xe]
         if extra_forward:                            # one more exchange: the replays after it see the other parities
-            run_ranks(plans, [fused(r, xe[r], ze[r], ge[r], he[r]) for r in range(k)], streams)
+            run_ranks(plans, lambda r: fused(r, xe[r], ze[r], ge[r], he[r])(), streams)
             z1 = [t.clone() for t in ze]
-            run_ranks(plans, [lambda r=r: cabi.check(lib.pgcn_forward(
+            run_ranks(plans, lambda r: cabi.check(lib.pgcn_forward(
                 plans[r].handle, xe[r].data_ptr(), ze[r].data_ptr(), f, torch.cuda.current_stream().cuda_stream),
-                plans[r].handle) for r in range(k)], streams)
+                plans[r].handle), streams)
             assert all(torch.equal(a, b) for a, b in zip(z1, ze))
             return ze, he, 3
-        run_ranks(plans, [fused(r, xe[r], ze[r], ge[r], he[r]) for r in range(k)], streams)
+        run_ranks(plans, lambda r: fused(r, xe[r], ze[r], ge[r], he[r])(), streams)
         return ze, he, 2
 
     calls = 0
@@ -235,7 +221,7 @@ def test_peer_transport_capture_and_replay(case, overlap):
             got[i] = (ze, he)
         else:
             load(i)
-            run_ranks(plans, [g.replay for g in graphs], streams)
+            run_ranks(plans, lambda r: graphs[r].replay(), streams)
             calls += 2
             got[i] = ([t.clone() for t in z], [t.clone() for t in gh])
     for i in (1, 2, 4):                              # the eager result of every replayed input
@@ -311,43 +297,39 @@ def test_minibatch_trainer_with_cuda_graphs(tmp_path):
 
 # ---- >= 2 GPUs: one process per GPU --------------------------------------------------------------------------------
 
-def _worker(rank, k, port, transport, q):
-    try:
-        os.environ["MASTER_ADDR"] = "127.0.0.1"
-        os.environ["MASTER_PORT"] = str(port)
-        import torch.distributed as dist
-        torch.cuda.set_device(rank)
-        dist.init_process_group("nccl", rank=rank, world_size=k, device_id=torch.device("cuda", rank))
-        g = Golden("gemat11_k2")
-        d = torch.device("cuda", rank)
-        p = planmod.build_plan(g.A, g.partvec, rank, k, g.f, device=d)
-        used = p.init_comm(transport=transport)
-        p.prepare(g.f)
-        own = p.lp.owned
-        rs = np.random.RandomState(3)
-        ins = [(torch.from_numpy(rs.uniform(-1, 1, size=(g.n, g.f)).astype(np.float32)[own]).to(d),
-                torch.from_numpy(rs.uniform(-1, 1, size=(g.n, g.f)).astype(np.float32)[own]).to(d)) for _ in range(3)]
-        x = torch.zeros_like(ins[0][0], requires_grad=True)
-        gz = torch.zeros_like(ins[0][1])
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            z = PSpMM.apply(p, x)
-            z.backward(gz)
-        for xi, gi in ins:
-            with torch.no_grad():
-                x.copy_(xi); gz.copy_(gi)
-            graph.replay()
-            zr, hr = z.detach().clone(), x.grad.clone()
-            ze, he = eager_fwd_bwd(PSpMM, p, xi, gi)
-            torch.cuda.synchronize()
-            assert torch.equal(zr, ze) and torch.equal(hr, he)
-        q.put((rank, used))
-        dist.barrier()
-        p.close()
-        dist.destroy_process_group()
-    except Exception as e:
-        import traceback
-        q.put((rank, "ERROR", traceback.format_exc(), str(e)))
+def _worker(rank, k, port, transport):
+    os.environ["MASTER_ADDR"] = "127.0.0.1"
+    os.environ["MASTER_PORT"] = str(port)
+    import torch.distributed as dist
+    torch.cuda.set_device(rank)
+    dist.init_process_group("nccl", rank=rank, world_size=k, device_id=torch.device("cuda", rank))
+    g = Golden("gemat11_k2")
+    d = torch.device("cuda", rank)
+    p = planmod.build_plan(g.A, g.partvec, rank, k, g.f, device=d)
+    used = p.init_comm(transport=transport)
+    p.prepare(g.f)
+    own = p.lp.owned
+    rs = np.random.RandomState(3)
+    ins = [(torch.from_numpy(rs.uniform(-1, 1, size=(g.n, g.f)).astype(np.float32)[own]).to(d),
+            torch.from_numpy(rs.uniform(-1, 1, size=(g.n, g.f)).astype(np.float32)[own]).to(d)) for _ in range(3)]
+    x = torch.zeros_like(ins[0][0], requires_grad=True)
+    gz = torch.zeros_like(ins[0][1])
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        z = PSpMM.apply(p, x)
+        z.backward(gz)
+    for xi, gi in ins:
+        with torch.no_grad():
+            x.copy_(xi); gz.copy_(gi)
+        graph.replay()
+        zr, hr = z.detach().clone(), x.grad.clone()
+        ze, he = eager_fwd_bwd(PSpMM, p, xi, gi)
+        torch.cuda.synchronize()
+        assert torch.equal(zr, ze) and torch.equal(hr, he)
+    dist.barrier()
+    p.close()
+    dist.destroy_process_group()
+    return used
 
 
 @pytest.mark.multigpu
@@ -355,18 +337,4 @@ def _worker(rank, k, port, transport, q):
 def test_two_gpus_capture_and_replay(transport, port):
     if not torch.cuda.is_available() or torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs")
-    import torch.multiprocessing as mp
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    procs = [ctx.Process(target=_worker, args=(r, 2, port, transport, q)) for r in range(2)]
-    for pr in procs:
-        pr.start()
-    for _ in range(2):
-        item = q.get(timeout=600)
-        if item[1] == "ERROR":
-            for pr in procs:
-                pr.kill()
-            pytest.fail("rank %d failed:\n%s" % (item[0], item[2]))
-        assert item[1] == transport
-    for pr in procs:
-        pr.join(timeout=120)
+    assert spawn_ranks(_worker, 2, (port, transport)) == {0: transport, 1: transport}

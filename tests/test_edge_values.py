@@ -13,32 +13,11 @@ import pytest
 import scipy.sparse as sp
 import torch
 
-from helpers import Golden
-from pgcn_b200 import cabi, graphio, plan as planmod
+from harness import check_one_rank_capture, check_two_rank_capture, dev, linked_plans, problem, run_ranks, stream
+from pgcn_b200 import cabi, plan as planmod
 from pgcn_b200.op import PSpMM, PSpMMWeighted
 
 pytestmark = pytest.mark.gpu
-
-
-def dev():
-    if not torch.cuda.is_available():
-        pytest.fail("no CUDA device: -m gpu tests must run on a GPU machine")
-    return torch.device("cuda", 0)
-
-
-def stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def problem(case):
-    """(A, partvec, k) of a golden case or a small R-MAT graph ("rmat": one rank, "rmat_k2": two)."""
-    if case.startswith("rmat"):
-        n = 6000
-        A = graphio.synthetic_graph(n, 120000, seed=31)
-        k = 2 if case == "rmat_k2" else 1
-        return A, (graphio.random_partvec(n, k, seed=5) if k > 1 else np.zeros(n, dtype=np.int64)), k
-    g = Golden(case)
-    return g.A, g.partvec, g.k
 
 
 def with_values(lp, v):
@@ -57,26 +36,6 @@ def with_values(lp, v):
 def new_values(lp, seed):
     rs = np.random.RandomState(seed)
     return (rs.uniform(0.25, 2.0, lp.nnz()) * rs.choice([-1.0, 1.0], lp.nnz())).astype(np.float32)
-
-
-def make_plans(lps, f, overlap):
-    plans = [planmod.PgcnPlan(lp, f, device=dev()) for lp in lps]
-    if len(plans) > 1:
-        planmod.link_local_plans(plans)
-    for p in plans:
-        p.set_option("overlap", overlap)
-    return plans
-
-
-def run_ranks(plans, fn, streams):
-    """fn(r) for every rank on its own stream (the ranks' kernels wait for each other on the device), then sync."""
-    torch.cuda.synchronize()
-    out = [None] * len(plans)
-    for r, s in enumerate(streams):
-        with torch.cuda.stream(s):
-            out[r] = fn(r)
-    torch.cuda.synchronize()
-    return out
 
 
 def fused_outputs(plans, xs, gs, f, streams):
@@ -116,8 +75,8 @@ def setup_case(case, f, overlap):
 def test_set_values_is_bit_exact(case, overlap, f):
     lps, H, G, xs, gs = setup_case(case, f, overlap)
     v1 = [new_values(lp, 100 + r) for r, lp in enumerate(lps)]
-    pa = make_plans(lps, f, overlap)
-    pb = make_plans([with_values(lp, v) for lp, v in zip(lps, v1)], f, overlap)
+    pa = linked_plans(lps, f, overlap, bind=False)
+    pb = linked_plans([with_values(lp, v) for lp, v in zip(lps, v1)], f, overlap, bind=False)
     streams = [torch.cuda.Stream(device=dev()) for _ in lps]
     orig = fused_outputs(pa, xs, gs, f, streams)
     for r, p in enumerate(pa):
@@ -152,7 +111,7 @@ def sddmm_truth(lp, gZ, Hcat):
 @pytest.mark.parametrize("f", [16, 40, 128, 256, 384, 512])
 def test_sddmm_within_fp32_bound_and_deterministic(case, overlap, f):
     lps, H, G, xs, gs = setup_case(case, f, overlap)
-    plans = make_plans(lps, f, overlap)
+    plans = linked_plans(lps, f, overlap, bind=False)
     streams = [torch.cuda.Stream(device=dev()) for _ in lps]
     lib = cabi.load()
 
@@ -298,9 +257,7 @@ def test_multi_rank_weighted_layers_gradients(case, f, overlap):
     A, pv, k = problem(case)
     n = A.shape[0]
     lps = [planmod.build_local_plan(A, pv, r, k) for r in range(k)]
-    plans = make_plans(lps, f, overlap)
-    for p in plans:
-        p.bind_values()
+    plans = linked_plans(lps, f, overlap)
     streams = [torch.cuda.Stream(device=dev()) for _ in plans]
     rs = np.random.RandomState(f + k)
     Hn = rs.uniform(-1, 1, size=(n, f)).astype(np.float32)
@@ -365,25 +322,25 @@ def test_one_rank_capture_of_weighted_layers():
     v1 = torch.zeros(plan.lp.nnz(), device=dev(), requires_grad=True)
     v2 = torch.zeros(plan.lp.nnz(), device=dev(), requires_grad=True)
 
-    def step(x, v1, v2, g):
+    def step():
         z = PSpMMWeighted.apply(plan, v2, PSpMMWeighted.apply(plan, v1, x))
         z.backward(g)
-        return z
+        return dict(Z=z, dH=x.grad, dv1=v1.grad, dv2=v2.grad)
 
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        z = step(x, v1, v2, g)
-    for i in (0, 1, 2, 1):
-        xi, gi, a, b = ins[i]
+    def load(i):
         with torch.no_grad():
-            x.copy_(xi); g.copy_(gi); v1.copy_(a); v2.copy_(b)
-        graph.replay()
-        got = [t.detach().clone() for t in (z, x.grad, v1.grad, v2.grad)]
-        xe, ae, be = (t.clone().requires_grad_(True) for t in (xi, a, b))
-        ze = step(xe, ae, be, gi)
+            for u, w in zip((x, g, v1, v2), ins[i]):
+                u.copy_(w)
+
+    def eager(i):
+        xi, gi, a, b = ins[i]
+        xe, ae, be = (u.clone().requires_grad_(True) for u in (xi, a, b))
+        ze = PSpMMWeighted.apply(plan, be, PSpMMWeighted.apply(plan, ae, xe))
+        ze.backward(gi)
         PSpMM.apply(plan, xi)                                      # the creation values in between
-        for name, u, w in zip(("Z", "dH", "dv1", "dv2"), got, (ze, xe.grad, ae.grad, be.grad)):
-            assert torch.equal(u, w.detach()), "replay %d: %s differs from eager" % (i, name)
+        return dict(Z=ze, dH=xe.grad, dv1=ae.grad, dv2=be.grad)
+
+    check_one_rank_capture(plan, step, load, eager)
     plan.close()
 
 
@@ -391,7 +348,7 @@ def test_two_rank_capture_over_the_peer_transport():
     A, pv, k = problem("gemat11_k2")
     f = 128
     lps = [planmod.build_local_plan(A, pv, r, k) for r in range(k)]
-    plans = make_plans(lps, f, 1)
+    plans = linked_plans(lps, f, 1, bind=False)
     for p in plans:
         p.prepare(f)
         p.bind_values()
@@ -412,7 +369,7 @@ def test_two_rank_capture_over_the_peer_transport():
                     g1=torch.zeros((m, f), device=dev()), g0=torch.zeros((m, f), device=dev()),
                     d1=torch.zeros(nnz, device=dev()), d2=torch.zeros(nnz, device=dev()))
 
-    def calls(r, b):
+    def step(r, b):
         p = plans[r]
         hd, st = p.handle, stream()
         chk = lambda rc: cabi.check(rc, hd)
@@ -425,6 +382,7 @@ def test_two_rank_capture_over_the_peer_transport():
         chk(lib.pgcn_plan_set_values(hd, b["v1"].data_ptr(), st))
         chk(lib.pgcn_backward(hd, b["g1"].data_ptr(), b["g0"].data_ptr(), f, st))
         chk(lib.pgcn_sddmm(hd, b["g1"].data_ptr(), b["x"].data_ptr(), b["h1"].data_ptr(), b["d1"].data_ptr(), f, st))
+        return {o: b[o] for o in ("z2", "g0", "d1", "d2")}
 
     def load(bufs, i):
         H, G, a, c = ins[i]
@@ -433,28 +391,7 @@ def test_two_rank_capture_over_the_peer_transport():
             bufs[r]["v1"].copy_(torch.from_numpy(a[r])); bufs[r]["v2"].copy_(torch.from_numpy(c[r]))
         torch.cuda.synchronize()
 
-    cap = [buffers(r) for r in range(k)]
-    graphs = []
-    for r in range(k):
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph, stream=streams[r]):
-            calls(r, cap[r])
-        graphs.append(graph)
-    outs = ("z2", "g0", "d1", "d2")
-    for step, i in enumerate((0, 1, 2, 1)):
-        load(cap, i)
-        run_ranks(plans, lambda r: graphs[r].replay(), streams)
-        got = [{o: cap[r][o].clone() for o in outs} for r in range(k)]
-        eager = [buffers(r) for r in range(k)]
-        load(eager, i)
-        run_ranks(plans, lambda r: calls(r, eager[r]), streams)
-        for r in range(k):
-            for o in outs:
-                assert torch.equal(got[r][o], eager[r][o]), "step %d rank %d: %s replay differs from eager" % (step, r, o)
-        if step == 1:                                  # one more fused call: the later replays see the other parity
-            run_ranks(plans, lambda r: cabi.check(lib.pgcn_forward(plans[r].handle, eager[r]["x"].data_ptr(),
-                                                                   eager[r]["z1"].data_ptr(), f, stream()),
-                                                  plans[r].handle), streams)
+    check_two_rank_capture(plans, streams, buffers, load, step)
     assert plans[0].get_option("epoch") % 2 == 1
     for p in plans:
         p.close()

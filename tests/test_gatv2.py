@@ -10,57 +10,20 @@
   * autograd in both layouts and with XL is XR; CUDA-graph capture on one and two ranks; refusals;
   * PGAT.py --v2 follows the fp64 loss curve, and PGAT.py without --v2 prints what it printed before.
 """
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 import scipy.sparse as sp
 import torch
 
 import gatv2_oracle as go
-from conftest import ROOT
-from helpers import GOLDEN, Golden
-from pgcn_b200 import cabi, graphio, plan as planmod
+import harness
+from harness import (EPS, assert_follows, check_one_rank_capture, check_two_rank_capture, dev, edges, karate,
+                     linked_plans, problem, run_cli, run_ranks, shifted, stream, t)
+from pgcn_b200 import cabi, plan as planmod
 from pgcn_b200.op import PGATv2Attention
 
 pytestmark = pytest.mark.gpu
-EPS = 2.0 ** -24
 PGCN_ERR_INVALID, PGCN_ERR_STATE = -1, -5
-
-
-def dev():
-    if not torch.cuda.is_available():
-        pytest.fail("no CUDA device: -m gpu tests must run on a GPU machine")
-    return torch.device("cuda", 0)
-
-
-def stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def t(x):
-    return torch.from_numpy(np.ascontiguousarray(x)).to(dev())
-
-
-def shifted(x):
-    """A copy of x whose data starts 4 bytes into its buffer."""
-    buf = torch.empty(x.numel() + 1, dtype=x.dtype, device=x.device)
-    v = buf[1:].view(x.shape)
-    v.copy_(x)
-    return v
-
-
-def hub_graph():
-    """R-MAT (6000 vertices) with a hub row of 3000 entries, rows of one entry (rows 20..29) and empty rows (10..19)."""
-    A = sp.coo_matrix(graphio.synthetic_graph(6000, 120000, seed=31))
-    keep = (A.row < 10) | (A.row >= 30)
-    row = np.concatenate([A.row[keep], np.zeros(3000, np.int64), np.arange(20, 30)])
-    col = np.concatenate([A.col[keep], np.arange(3000) * 2, np.arange(20, 30) + 100])
-    B = sp.csr_matrix((np.ones(len(row), np.float32), (row, col)), shape=A.shape)
-    B.sum_duplicates()
-    return B.tocoo()
 
 
 def dup_graph():
@@ -73,26 +36,14 @@ def dup_graph():
     return sp.coo_matrix((np.ones(len(row), np.float32), (row, col)), shape=(400, 400))
 
 
-def problem(case):
-    if case == "hub":
-        A = hub_graph()
-        return A, np.zeros(A.shape[0], dtype=np.int64), 1
-    if case == "dup":
-        A = dup_graph()
-        return A, np.zeros(A.shape[0], dtype=np.int64), 1
-    g = Golden(case)
-    return g.A, g.partvec, g.k
-
-
 def one_rank_plan(case, f):
-    A, _, _ = problem(case)
+    """The harness's one-rank plan, or one of dup_graph() (a case of this file only)."""
+    if case != "dup":
+        return harness.one_rank_plan(case, f)
+    A = dup_graph()
     plan = planmod.build_plan(A, np.zeros(A.shape[0], dtype=np.int64), 0, 1, f, device=dev())
     plan.bind_values()
     return A, plan
-
-
-def edges(lp):
-    return np.repeat(np.arange(lp.m), np.diff(lp.rowptr.astype(np.int64))), lp.colidx.astype(np.int64)
 
 
 def gatv2_run(plan, K, xl, xr, att, gZ, slope):
@@ -238,25 +189,6 @@ def test_exact_identities(f, K):
     plan.close()
 
 
-def make_plans(lps, f, overlap):
-    plans = [planmod.PgcnPlan(lp, f, device=dev()) for lp in lps]
-    planmod.link_local_plans(plans)
-    for p in plans:
-        p.set_option("overlap", overlap)
-        p.bind_values()
-    return plans
-
-
-def run_ranks(plans, fn, streams):
-    torch.cuda.synchronize()
-    out = [None] * len(plans)
-    for r, s in enumerate(streams):
-        with torch.cuda.stream(s):
-            out[r] = fn(r)
-    torch.cuda.synchronize()
-    return out
-
-
 def global_edges(A):
     C = sp.csr_matrix(A)
     C.sum_duplicates()
@@ -271,7 +203,7 @@ def test_multi_rank(case, f, K, overlap):
     A, pv, k = problem(case)
     n = A.shape[0]
     lps = [planmod.build_local_plan(A, pv, r, k) for r in range(k)]
-    plans = make_plans(lps, f, overlap)
+    plans = linked_plans(lps, f, overlap)
     streams = [torch.cuda.Stream(device=dev()) for _ in plans]
     rs = np.random.RandomState(f + k + K)
     xl, xr, att, gZ = inputs(rs, n, f, K)
@@ -409,26 +341,21 @@ def test_one_rank_capture_and_refusals():
     Wl = torch.zeros((f, f), device=dev(), requires_grad=True)
     Wr = torch.zeros((f, f), device=dev(), requires_grad=True)
     att = torch.zeros((K, f // K), device=dev(), requires_grad=True)
-    s = torch.cuda.Stream()
-    with pytest.raises(RuntimeError, match="pgcn_plan_prepare"):
-        with torch.cuda.graph(torch.cuda.CUDAGraph(), stream=s):
-            step(plan, x, Wl, Wr, att, g)
-    Wl.grad = Wr.grad = att.grad = None
-    plan.prepare(f)
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        out = step(plan, x, Wl, Wr, att, g)
     ins = [(rnd(n, f), rnd(n, f), rnd(f, f) * 0.1, rnd(f, f) * 0.1, rnd(K, f // K)) for _ in range(3)]
-    for i in (0, 1, 2, 1):
-        xi, gi, Wli, Wri, ai = ins[i]
+
+    def load(i):
         with torch.no_grad():
-            x.copy_(xi); g.copy_(gi); Wl.copy_(Wli); Wr.copy_(Wri); att.copy_(ai)
-        graph.replay()
-        got = [u.detach().clone() for u in (out, Wl.grad, Wr.grad, att.grad)]
+            for u, v in zip((x, g, Wl, Wr, att), ins[i]):
+                u.copy_(v)
+
+    def eager(i):
+        xi, gi, Wli, Wri, ai = ins[i]
         e = [u.clone().requires_grad_(True) for u in (Wli, Wri, ai)]
         oe = step(plan, xi, e[0], e[1], e[2], gi)
-        for name, u, w in zip(("out", "dWl", "dWr", "datt"), got, (oe, e[0].grad, e[1].grad, e[2].grad)):
-            assert torch.equal(u, w.detach()), "replay %d: %s differs from eager" % (i, name)
+        return dict(out=oe, dWl=e[0].grad, dWr=e[1].grad, datt=e[2].grad)
+
+    check_one_rank_capture(plan, lambda: dict(out=step(plan, x, Wl, Wr, att, g), dWl=Wl.grad, dWr=Wr.grad,
+                                              datt=att.grad), load, eager, prepare=(f,), leaves=(Wl, Wr, att))
     plan.close()
 
 
@@ -436,7 +363,7 @@ def test_two_rank_capture():
     A, pv, k = problem("gemat11_k2")
     f, n, K = 128, A.shape[0], 8
     lps = [planmod.build_local_plan(A, pv, r, k) for r in range(k)]
-    plans = make_plans(lps, f, 1)
+    plans = linked_plans(lps, f, 1)
     for p in plans:
         p.prepare(f)
     streams = [torch.cuda.Stream(device=dev()) for _ in plans]
@@ -461,61 +388,21 @@ def test_two_rank_capture():
                 b["att"].copy_(torch.from_numpy(att))
         torch.cuda.synchronize()
 
-    run = lambda r, b: step(plans[r], b["x"], b["Wl"], b["Wr"], b["att"], b["g"])
-    cap = [buffers(r) for r in range(k)]
-    graphs, outs = [], []
-    for r in range(k):
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph, stream=streams[r]):
-            outs.append(run(r, cap[r]))
-        graphs.append(graph)
-    lib = cabi.load()
-    for it, i in enumerate((0, 1, 2, 1)):
-        load(cap, i)
-        run_ranks(plans, lambda r: graphs[r].replay(), streams)
-        got = [[outs[r].detach().clone()] + [cap[r][w].grad.clone() for w in ("Wl", "Wr", "att")] for r in range(k)]
-        eager = [buffers(r) for r in range(k)]
-        load(eager, i)
-        res = run_ranks(plans, lambda r: run(r, eager[r]), streams)
-        for r in range(k):
-            want = [res[r]] + [eager[r][w].grad for w in ("Wl", "Wr", "att")]
-            for name, u, w in zip(("out", "dWl", "dWr", "datt"), got[r], want):
-                assert torch.equal(u, w.detach()), "step %d rank %d: %s replay differs from eager" % (it, r, name)
-        if it == 1:                                    # one more fused call: the later replays see the other parity
-            run_ranks(plans, lambda r: cabi.check(lib.pgcn_forward(plans[r].handle, eager[r]["x"].data_ptr(),
-                                                                   torch.empty_like(eager[r]["x"]).data_ptr(), f,
-                                                                   stream()), plans[r].handle), streams)
+    def run(r, b):
+        out = step(plans[r], b["x"], b["Wl"], b["Wr"], b["att"], b["g"])
+        return dict(out=out, dWl=b["Wl"].grad, dWr=b["Wr"].grad, datt=b["att"].grad)
+
+    check_two_rank_capture(plans, streams, buffers, load, run)
     for p in plans:
         p.close()
 
 
-def run_cli(tmp_path, extra, port):
-    from scipy.io import mmwrite
-    z = np.load(os.path.join(GOLDEN, "pgat_karate_k1.npz"))
-    n = int(z["n"])
-    A = sp.coo_matrix((z["val"], (z["row"], z["col"])), shape=(n, n))
-    a = str(tmp_path / "karate.mtx")
-    mmwrite(a, A)
-    p = str(tmp_path / "karate.mtx.1.rp")
-    graphio.write_partvec(p, np.zeros(n, dtype=np.int64))
-    env = dict(os.environ, SLURM_NPROCS="1", SLURM_PROCID="0", MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-    out = subprocess.run([sys.executable, os.path.join(ROOT, "PGAT.py"), "-a", a, "-p", p, "-b", "nccl", "-s", "1",
-                          "-l", "2", "-f", "4", "--seed", "7"] + extra, env=env, capture_output=True, text=True,
-                         timeout=600)
-    assert out.returncode == 0, out.stderr[-2000:]
-    return A, [l for l in out.stdout.splitlines() if l.startswith("Epoch")]
-
-
 def test_cli_v2_follows_the_fp64_loss_curve(tmp_path):
-    A, lines = run_cli(tmp_path, ["--v2", "--heads", "2"], 29681)
-    assert [l[:11] for l in lines] == ["Epoch %05d" % i for i in range(50)]
-    want = go.intended_training(A, 2, 4, 7, 1.0, heads=2)
-    got = [float(l.split("Loss")[1]) for l in lines]
-    np.testing.assert_allclose(got, want, rtol=1e-3, atol=6e-5)
+    lines = run_cli(tmp_path, "PGAT.py", ["--v2", "--heads", "2"], 29681)
+    assert_follows(lines, go.intended_training(karate(), 2, 4, 7, 1.0, heads=2))
 
 
 def test_cli_without_v2_is_unchanged(tmp_path):
     import pgat_heads_oracle as ho
-    A, lines = run_cli(tmp_path, ["--heads", "2"], 29682)
-    want = ho.intended_training(A, 2, 4, 7, 1.0, heads=2)
-    np.testing.assert_allclose([float(l.split("Loss")[1]) for l in lines], want, rtol=1e-3, atol=6e-5)
+    lines = run_cli(tmp_path, "PGAT.py", ["--heads", "2"], 29682)
+    assert_follows(lines, ho.intended_training(karate(), 2, 4, 7, 1.0, heads=2))

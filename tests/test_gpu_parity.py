@@ -15,6 +15,7 @@ import scipy.sparse as sp
 import torch
 
 from conftest import golden_cases
+from harness import dev, t
 from helpers import Golden, assert_close_fp32, fp32_tol
 from oracle import build_oracle, pgcn_oracle as orc
 from pgcn_b200 import graphio, plan as planmod
@@ -22,17 +23,7 @@ from pgcn_b200 import graphio, plan as planmod
 pytestmark = pytest.mark.gpu
 
 
-def dev():
-    if not torch.cuda.is_available():
-        pytest.fail("no CUDA device: -m gpu tests must run on a GPU machine")
-    return torch.device("cuda", 0)
-
-
-def t(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).to(dev())
-
-
-def make_plans(A, partvec, k, f_max):
+def build_plans(A, partvec, k, f_max):
     from pgcn_b200 import op  # noqa: F401  (import checks the extension loads)
     return [planmod.build_plan(A, partvec, r, k, f_max, device=dev()) for r in range(k)]
 
@@ -83,7 +74,7 @@ def backward_all(plans, G):
 @pytest.mark.parametrize("case", golden_cases())
 def test_golden_forward_backward(case):
     g = Golden(case)
-    plans = make_plans(g.A, g.partvec, g.k, g.f)
+    plans = build_plans(g.A, g.partvec, g.k, g.f)
     Z = forward_all(plans, g.H)
     Gd = backward_all(plans, g.G)
     Z64 = orc.truth_forward(g.A, g.H)
@@ -129,7 +120,7 @@ def test_feature_widths_vs_oracle(f):
     H = rng.uniform(-1, 1, size=(n, f)).astype(np.float32)
     G = rng.uniform(-1, 1, size=(n, f)).astype(np.float32)
     pv = graphio.random_partvec(n, 2, seed=5)
-    plans = make_plans(A, pv, 2, f)
+    plans = build_plans(A, pv, 2, f)
     Z = forward_all(plans, H)
     Gd = backward_all(plans, G)
     Z64 = orc.truth_forward(A, H); G64 = orc.truth_backward(A, G)
@@ -156,7 +147,7 @@ def test_schedule_options_do_not_change_results(opts):
     n, f = 4000, 128
     A = skewed_graph(n, 120000, seed=11)
     H = np.random.RandomState(1).uniform(-1, 1, size=(n, f)).astype(np.float32)
-    plans = make_plans(A, np.zeros(n, dtype=np.int64), 1, f)
+    plans = build_plans(A, np.zeros(n, dtype=np.int64), 1, f)
     Z64 = orc.truth_forward(A, H)
     tol = fp32_tol(A, H, int(orc.row_degree(A).max()))
     opts = dict(opts, kernel=4)                  # the register-pipeline kernel (the ring kernel has its own test)
@@ -194,7 +185,7 @@ def test_ring_kernel_matches_truth_and_register_kernel(f, opts):
     tolZ = fp32_tol(A, H, int(orc.row_degree(A).max())); tolG = fp32_tol(A.T, G, int(orc.row_degree(A.T).max()))
     for k in (1, 2):
         pv = np.zeros(n, dtype=np.int64) if k == 1 else graphio.random_partvec(n, 2, seed=5)
-        plans = make_plans(A, pv, k, f)
+        plans = build_plans(A, pv, k, f)
         z1 = forward_all(plans, H, **opts)
         z2 = forward_all(plans, H, **opts)
         gd = backward_all(plans, G)
@@ -215,7 +206,7 @@ def test_empty_rank_and_tiny_graphs():
     A = sp.coo_matrix((np.arange(1, 9, dtype=np.float64), (row, col)), shape=(6, 6))
     pv = np.array([0, 1, 0, 1, 0, 1])
     H = np.arange(24, dtype=np.float32).reshape(6, 4)
-    plans = make_plans(A, pv, 3, 4)                      # rank 2 owns nothing
+    plans = build_plans(A, pv, 3, 4)                      # rank 2 owns nothing
     Z = forward_all(plans, H)
     Gd = backward_all(plans, H)
     Z64 = orc.truth_forward(A, H); G64 = orc.truth_backward(A, H)
@@ -231,7 +222,7 @@ def test_autograd_op_single_rank_matches_torch_sparse():
     from pgcn_b200.op import PSpMM
     n, f = 2500, 48
     A = skewed_graph(n, 40000, seed=3)
-    p = make_plans(A, np.zeros(n, dtype=np.int64), 1, f)[0]
+    p = build_plans(A, np.zeros(n, dtype=np.int64), 1, f)[0]
     H = torch.randn(n, f, device=dev(), requires_grad=True)
     Z = PSpMM.apply(p, H)
     gz = torch.randn(n, f, device=dev())
@@ -296,7 +287,7 @@ def test_overlap_halves_equal_single_pass(case):
     """The own-columns / halo-columns kernels of the overlapped forward (what runs on > 1 GPU) on one GPU."""
     from pgcn_b200 import op
     g = Golden(case)
-    plans = make_plans(g.A, g.partvec, g.k, g.f)
+    plans = build_plans(g.A, g.partvec, g.k, g.f)
     Z = forward_all(plans, g.H)
     Z64 = orc.truth_forward(g.A, g.H)
     tol = fp32_tol(g.A, g.H, int(orc.row_degree(g.A).max()))
@@ -316,7 +307,7 @@ def test_autotune_keeps_results():
     n, f = 6000, 128
     A = skewed_graph(n, 150000, seed=13)
     H = np.random.RandomState(4).uniform(-1, 1, size=(n, f)).astype(np.float32)
-    p = make_plans(A, np.zeros(n, dtype=np.int64), 1, f)[0]
+    p = build_plans(A, np.zeros(n, dtype=np.int64), 1, f)[0]
     z0 = forward_all([p], H)[0]
     chosen = p.autotune(f)                       # f = 128: the ring kernel's block size is what gets tuned
     assert chosen in (256, 512, 1024) and p.get_option("ring_edges_per_block") == chosen

@@ -17,18 +17,12 @@ import numpy as np
 import pytest
 import torch
 
+from harness import ROOT, dev
 from helpers import Golden, assert_close_fp32, fp32_tol
 from oracle import pgcn_oracle as orc
 from pgcn_b200 import cabi, graphio, plan as planmod
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def dev():
-    if not torch.cuda.is_available():
-        pytest.fail("no CUDA device: -m gpu tests must run on a GPU machine")
-    return torch.device("cuda", 0)
 
 
 def run_all(plans, fn_name, inputs, f):

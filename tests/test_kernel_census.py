@@ -31,9 +31,9 @@ import torch
 
 import sage_oracle as so
 from conftest import ROOT
+from harness import EPS, dev, edges, shifted, stream, t
 from pgcn_b200 import cabi, graphio, plan as planmod
 
-EPS = 2.0 ** -24
 F_MAX = 512
 SLOPE = 0.2
 MANIFEST = os.path.join(ROOT, "tests", "kernel_instances.txt")
@@ -270,28 +270,6 @@ def test_manifest_matches_the_library():
 
 # ---- GPU fixtures ----------------------------------------------------------------------------------------------------
 
-def dev():
-    if not torch.cuda.is_available():
-        pytest.fail("no CUDA device: -m gpu tests must run on a GPU machine")
-    return torch.device("cuda", 0)
-
-
-def stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def t(x):
-    return torch.from_numpy(np.ascontiguousarray(x)).to(dev())
-
-
-def shifted(x):
-    """A copy of x whose data starts 4 bytes into its buffer."""
-    buf = torch.empty(x.numel() + 1, dtype=x.dtype, device=x.device)
-    v = buf[1:].view(x.shape)
-    v.copy_(x)
-    return v
-
-
 def nan_like(x, shift=False):
     y = torch.full_like(x, float("nan")) if x.dtype.is_floating_point else torch.full_like(x, -7)
     return shifted(y) if shift else y
@@ -391,10 +369,6 @@ def reset(P):
 
 
 # ---- fp64 references -------------------------------------------------------------------------------------------------
-
-def edges(lp):
-    return np.repeat(np.arange(lp.m), np.diff(lp.rowptr.astype(np.int64))), lp.colidx.astype(np.int64)
-
 
 def local_csr(lp):
     return sp.csr_matrix((lp.vals.astype(np.float64), lp.colidx, lp.rowptr), shape=(lp.m, lp.m + lp.h))

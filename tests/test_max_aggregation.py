@@ -14,8 +14,6 @@
   * PSAGE.py follows the fp64 loss curve, and the layer on 3 ranks follows the one-rank curve.
 """
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -23,47 +21,15 @@ import scipy.sparse as sp
 import torch
 
 import sage_oracle as so
-from conftest import ROOT
-from helpers import GOLDEN, Golden, fp32_tol
-from pgcn_b200 import cabi, graphio, plan as planmod
+from harness import (assert_follows, bits, check_one_rank_capture, check_two_rank_capture, dev, karate,
+                     linked_plans, problem, run_cli, run_ranks, shifted, spawn_ranks, stream, t)
+from helpers import fp32_tol
+from pgcn_b200 import cabi, plan as planmod
 from pgcn_b200.op import PSpMMMax, aggregate_max, aggregate_max_backward
 
 pytestmark = pytest.mark.gpu
 WIDTHS = [1, 3, 4, 8, 64, 128, 132, 256]
 SCHEDULES = {"default": {}, "segments": {"edges_per_block": 16, "long_row": 32}}
-
-
-def dev():
-    if not torch.cuda.is_available():
-        pytest.fail("no CUDA device: -m gpu tests must run on a GPU machine")
-    return torch.device("cuda", 0)
-
-
-def stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def t(x):
-    return torch.from_numpy(np.ascontiguousarray(x)).to(dev())
-
-
-def shifted(x):
-    """A copy of x whose data starts 4 bytes into its buffer."""
-    buf = torch.empty(x.numel() + 1, dtype=x.dtype, device=x.device)
-    v = buf[1:].view(x.shape)
-    v.copy_(x)
-    return v
-
-
-def hub_graph():
-    """R-MAT (6000 vertices) with a hub row of 3000 entries, rows of one entry (rows 20..29) and empty rows (10..19)."""
-    A = sp.coo_matrix(graphio.synthetic_graph(6000, 120000, seed=31))
-    keep = (A.row < 10) | (A.row >= 30)
-    row = np.concatenate([A.row[keep], np.zeros(3000, np.int64), np.arange(20, 30)])
-    col = np.concatenate([A.col[keep], np.arange(3000) * 2, np.arange(20, 30) + 100])
-    B = sp.csr_matrix((np.ones(len(row), np.float32), (row, col)), shape=A.shape)
-    B.sum_duplicates()
-    return B.tocoo()
 
 
 def with_duplicates(lp):
@@ -87,18 +53,6 @@ def with_duplicates(lp):
     out.t_colidx = r[tor].astype(np.int32)
     out.t_vals = np.ones(len(c), np.float32)
     return out
-
-
-def problem(case):
-    if case == "hub":
-        A = hub_graph()
-        return A, np.zeros(A.shape[0], dtype=np.int64), 1
-    if case == "karate":
-        z = np.load(os.path.join(GOLDEN, "pgat_karate_k3.npz"))
-        n = int(z["n"])
-        return sp.coo_matrix((z["val"], (z["row"], z["col"])), shape=(n, n)), z["partvec"].astype(np.int64), 3
-    g = Golden(case)
-    return g.A, g.partvec, g.k
 
 
 def one_rank_plan(case, f, opts=None, bind=True):
@@ -128,10 +82,6 @@ def run_max_backward(plan, arg, g, f):
     cabi.check(cabi.load().pgcn_backward_max(plan.handle, arg.data_ptr(), g.data_ptr(), G.data_ptr(), f, stream()),
                plan.handle)
     return G
-
-
-def bits(x):
-    return x.detach().cpu().numpy().view(np.uint32) if x.dtype == torch.float32 else x.detach().cpu().numpy()
 
 
 def backward_tol(lp, gZ):
@@ -223,25 +173,6 @@ def test_unbound_plan_is_refused():
     plan.close()
 
 
-def make_plans(lps, f, overlap):
-    plans = [planmod.PgcnPlan(lp, f, device=dev()) for lp in lps]
-    planmod.link_local_plans(plans)
-    for p in plans:
-        p.set_option("overlap", overlap)
-        p.bind_values()
-    return plans
-
-
-def run_ranks(plans, fn, streams):
-    torch.cuda.synchronize()
-    out = [None] * len(plans)
-    for r, s in enumerate(streams):
-        with torch.cuda.stream(s):
-            out[r] = fn(r)
-    torch.cuda.synchronize()
-    return out
-
-
 def tie_free(n, f, seed):
     return (np.random.RandomState(seed).permutation(n * f).reshape(n, f).astype(np.float32) - n * f / 2) / 64.0
 
@@ -268,7 +199,7 @@ def test_multi_rank_equals_one_rank(case, f, overlap):
     G64 = so.max_backward(lp1.colidx, ao, gn, n)
     tol = backward_tol(lp1, gn)
     lps = [planmod.build_local_plan(A, pv, r, k) for r in range(k)]
-    plans = make_plans(lps, f, overlap)
+    plans = linked_plans(lps, f, overlap)
     streams = [torch.cuda.Stream(device=dev()) for _ in plans]
     Hr = [t(Hn[lp.owned]) for lp in lps]
     gr = [t(gn[lp.owned]) for lp in lps]
@@ -312,7 +243,7 @@ def test_autograd_three_ranks():
     G64 = so.max_backward(one.lp.colidx, ao, gn, n)
     tol = backward_tol(one.lp, gn)
     lps = [planmod.build_local_plan(A, pv, r, k) for r in range(k)]
-    plans = make_plans(lps, f, 1)
+    plans = linked_plans(lps, f, 1)
     streams = [torch.cuda.Stream(device=dev()) for _ in plans]
     H = [t(Hn[lp.owned]).requires_grad_(True) for lp in lps]
     Z = run_ranks(plans, lambda r: PSpMMMax.apply(plans[r], H[r]), streams)
@@ -328,24 +259,18 @@ def test_one_rank_capture_and_refusal_before_prepare():
     plan = one_rank_plan("hub", f, SCHEDULES["segments"])
     m = plan.lp.m
     x, g = torch.zeros((m, f), device=dev()), torch.zeros((m, f), device=dev())
-    s = torch.cuda.Stream()
-    with pytest.raises(RuntimeError, match="pgcn_plan_prepare"):
-        with torch.cuda.graph(torch.cuda.CUDAGraph(), stream=s):
-            aggregate_max(plan, x)
-    plan.prepare(f)
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        Z, arg = aggregate_max(plan, x)
-        G = aggregate_max_backward(plan, arg, g)
     rs = np.random.RandomState(2)
     ins = [(t(rs.standard_normal((m, f)).astype(np.float32)), t(rs.uniform(-1, 1, (m, f)).astype(np.float32)))
            for _ in range(3)]
-    for i in (0, 1, 2, 1):
+
+    def step(x, g):
+        Z, arg = aggregate_max(plan, x)
+        return dict(Z=Z, arg=arg, G=aggregate_max_backward(plan, arg, g))
+
+    def load(i):
         x.copy_(ins[i][0]); g.copy_(ins[i][1])
-        graph.replay()
-        Ze, ae = aggregate_max(plan, ins[i][0])
-        Ge = aggregate_max_backward(plan, ae, ins[i][1])
-        assert np.array_equal(bits(Z), bits(Ze)) and torch.equal(arg, ae) and np.array_equal(bits(G), bits(Ge)), i
+
+    check_one_rank_capture(plan, lambda: step(x, g), load, lambda i: step(*ins[i]), prepare=(f,))
     plan.close()
 
 
@@ -353,125 +278,68 @@ def test_two_rank_capture_over_the_peer_transport():
     A, pv, k = problem("gemat11_k2")
     f, n = 128, A.shape[0]
     lps = [planmod.build_local_plan(A, pv, r, k) for r in range(k)]
-    plans = make_plans(lps, f, 1)
+    plans = linked_plans(lps, f, 1)
     for p in plans:
         p.prepare(f)
     streams = [torch.cuda.Stream(device=dev()) for _ in plans]
     rs = np.random.RandomState(6)
     ins = [(tie_free(n, f, i), rs.uniform(-1, 1, (n, f)).astype(np.float32)) for i in range(3)]
-    cap = [(torch.zeros((lp.m, f), device=dev()), torch.zeros((lp.m, f), device=dev())) for lp in lps]
 
-    def step(r, x, g):
-        Z, arg = aggregate_max(plans[r], x)
-        return Z, arg, aggregate_max_backward(plans[r], arg, g)
+    def buffers(r):
+        return dict(x=torch.zeros((lps[r].m, f), device=dev()), g=torch.zeros((lps[r].m, f), device=dev()))
 
-    graphs, outs = [], []
-    for r in range(k):
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph, stream=streams[r]):
-            outs.append(step(r, *cap[r]))
-        graphs.append(graph)
-    lib = cabi.load()
-    for it, i in enumerate((0, 1, 2, 1)):
+    def load(bufs, i):
         Hn, gn = ins[i]
         for r, lp in enumerate(lps):
-            cap[r][0].copy_(t(Hn[lp.owned])); cap[r][1].copy_(t(gn[lp.owned]))
+            bufs[r]["x"].copy_(t(Hn[lp.owned])); bufs[r]["g"].copy_(t(gn[lp.owned]))
         torch.cuda.synchronize()
-        run_ranks(plans, lambda r: graphs[r].replay(), streams)
-        got = [[u.clone() for u in outs[r]] for r in range(k)]
-        eager = run_ranks(plans, lambda r: step(r, t(Hn[lps[r].owned]), t(gn[lps[r].owned])), streams)
-        for r in range(k):
-            for name, u, w in zip(("Z", "arg", "G"), got[r], eager[r]):
-                assert np.array_equal(bits(u), bits(w)), "step %d rank %d: %s replay differs from eager" % (it, r, name)
-        if it == 1:                                    # one more fused call: the later replays see the other parity
-            run_ranks(plans, lambda r: cabi.check(lib.pgcn_forward(plans[r].handle, cap[r][0].data_ptr(),
-                                                                   torch.empty_like(cap[r][0]).data_ptr(), f,
-                                                                   stream()), plans[r].handle), streams)
+
+    def step(r, b):
+        Z, arg = aggregate_max(plans[r], b["x"])
+        return dict(Z=Z, arg=arg, G=aggregate_max_backward(plans[r], arg, b["g"]))
+
+    check_two_rank_capture(plans, streams, buffers, load, step)
     for p in plans:
         p.close()
 
 
-def _nccl_worker(rank, k, port, transport, q):
-    try:
-        os.environ["MASTER_ADDR"] = "127.0.0.1"
-        os.environ["MASTER_PORT"] = str(port)
-        import torch.distributed as dist
-        torch.cuda.set_device(rank)
-        dist.init_process_group("nccl", rank=rank, world_size=k, device_id=torch.device("cuda", rank))
-        A, pv, _ = problem("gemat11_k2")
-        n, f = A.shape[0], 128
-        p = planmod.build_plan(A, pv, rank, k, f, device=torch.device("cuda", rank))
-        used = p.init_comm(transport=transport)
-        p.bind_values()
-        own = p.lp.owned
-        Hd = torch.from_numpy(tie_free(n, f, 1)[own]).cuda().requires_grad_(True)
-        Z = PSpMMMax.apply(p, Hd)
-        Z.backward(torch.from_numpy(np.random.RandomState(2).uniform(-1, 1, (n, f)).astype(np.float32)[own]).cuda())
-        torch.cuda.synchronize()
-        q.put((rank, used, Z.detach().cpu().numpy(), Hd.grad.cpu().numpy()))
-        dist.barrier()
-        p.close()
-        dist.destroy_process_group()
-    except Exception as e:
-        import traceback
-        q.put((rank, "ERROR", traceback.format_exc(), str(e)))
-
-
-def _nccl_run(k, transport, port):
-    import torch.multiprocessing as mp
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    procs = [ctx.Process(target=_nccl_worker, args=(r, k, port, transport, q)) for r in range(k)]
-    for p in procs:
-        p.start()
-    out = {}
-    for _ in range(k):
-        item = q.get(timeout=600)
-        if item[1] == "ERROR":
-            for p in procs:
-                p.kill()
-            pytest.fail("rank %d failed:\n%s" % (item[0], item[2]))
-        out[item[0]] = item[1:]
-    for p in procs:
-        p.join(timeout=120)
-    return out
+def _nccl_worker(rank, k, port, transport):
+    os.environ["MASTER_ADDR"] = "127.0.0.1"
+    os.environ["MASTER_PORT"] = str(port)
+    import torch.distributed as dist
+    torch.cuda.set_device(rank)
+    dist.init_process_group("nccl", rank=rank, world_size=k, device_id=torch.device("cuda", rank))
+    A, pv, _ = problem("gemat11_k2")
+    n, f = A.shape[0], 128
+    p = planmod.build_plan(A, pv, rank, k, f, device=torch.device("cuda", rank))
+    used = p.init_comm(transport=transport)
+    p.bind_values()
+    own = p.lp.owned
+    Hd = torch.from_numpy(tie_free(n, f, 1)[own]).cuda().requires_grad_(True)
+    Z = PSpMMMax.apply(p, Hd)
+    Z.backward(torch.from_numpy(np.random.RandomState(2).uniform(-1, 1, (n, f)).astype(np.float32)[own]).cuda())
+    torch.cuda.synchronize()
+    dist.barrier()
+    p.close()
+    dist.destroy_process_group()
+    return used, Z.detach().cpu().numpy(), Hd.grad.cpu().numpy()
 
 
 @pytest.mark.multigpu
 def test_two_gpus_nccl_gives_the_peer_transport_bits():
     if not torch.cuda.is_available() or torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs")
-    a = _nccl_run(2, "nccl", 29861)
-    b = _nccl_run(2, "p2p", 29862)
+    a = spawn_ranks(_nccl_worker, 2, (29861, "nccl"))
+    b = spawn_ranks(_nccl_worker, 2, (29862, "p2p"))
     for r in range(2):
         assert a[r][0] == "nccl" and b[r][0] == "p2p"
         assert np.array_equal(a[r][1].view(np.uint32), b[r][1].view(np.uint32))
         assert np.array_equal(a[r][2].view(np.uint32), b[r][2].view(np.uint32))
 
 
-def karate():
-    z = np.load(os.path.join(GOLDEN, "pgat_karate_k1.npz"))
-    n = int(z["n"])
-    return sp.coo_matrix((z["val"], (z["row"], z["col"])), shape=(n, n))
-
-
 def test_cli_follows_the_fp64_loss_curve(tmp_path):
-    from scipy.io import mmwrite
-    A = karate()
-    n = A.shape[0]
-    a = str(tmp_path / "karate.mtx")
-    mmwrite(a, A)
-    p = str(tmp_path / "karate.mtx.1.rp")
-    graphio.write_partvec(p, np.zeros(n, dtype=np.int64))
-    env = dict(os.environ, SLURM_NPROCS="1", SLURM_PROCID="0", MASTER_ADDR="127.0.0.1", MASTER_PORT="29681")
-    out = subprocess.run([sys.executable, os.path.join(ROOT, "PSAGE.py"), "-a", a, "-p", p, "-b", "nccl", "-s", "1",
-                          "-l", "2", "-f", "4", "--seed", "7"], env=env, capture_output=True, text=True, timeout=600)
-    assert out.returncode == 0, out.stderr[-2000:]
-    lines = [l for l in out.stdout.splitlines() if l.startswith("Epoch")]
-    assert [l[:11] for l in lines] == ["Epoch %05d" % i for i in range(50)]
-    want = so.intended_training(A, 2, 4, 7)
-    got = [float(l.split("Loss")[1]) for l in lines]
-    np.testing.assert_allclose(got, want, rtol=1e-3, atol=6e-5)
+    lines = run_cli(tmp_path, "PSAGE.py", [], 29681)
+    assert_follows(lines, so.intended_training(karate(), 2, 4, 7))
 
 
 def test_layer_on_three_ranks_follows_the_one_rank_curve():
@@ -516,7 +384,7 @@ def test_layer_on_three_ranks_follows_the_one_rank_curve():
     one[0].bind_values()
     curve1 = train(one, lp1)
     lps = [planmod.build_local_plan(A, pv, r, k) for r in range(k)]
-    plans = make_plans(lps, f, 1)
+    plans = linked_plans(lps, f, 1)
     curve3 = train(plans, lps)
     np.testing.assert_allclose(curve1, so.intended_training(A, L, f, 7), rtol=1e-3, atol=6e-5)
     np.testing.assert_allclose(curve3, so.intended_training(A, L, f, 7, k=3), rtol=1e-3, atol=6e-5)

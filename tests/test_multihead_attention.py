@@ -11,79 +11,18 @@ pgcn_forward_heads, pgcn_backward_heads, pgcn_sddmm_heads, op.PGATMultiHeadAtten
     with overlap 0 and 1; the plan's resident values are untouched; CUDA-graph capture on one and two ranks;
   * the command line follows the fp64 loss curve with --heads 2, and --heads 1 prints what no flag prints.
 """
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 import scipy.sparse as sp
 import torch
 
 import pgat_heads_oracle as ho
-from conftest import ROOT
-from helpers import GOLDEN, Golden
-from pgcn_b200 import cabi, graphio, plan as planmod
+from harness import (EPS, assert_follows, check_one_rank_capture, check_two_rank_capture, dev, edges, karate,
+                     linked_plans, one_rank_plan, problem, run_cli, run_ranks, shifted, stream, t)
+from pgcn_b200 import cabi, plan as planmod
 from pgcn_b200.op import PGATAttention, PGATMultiHeadAttention, PSpMM
 
 pytestmark = pytest.mark.gpu
-EPS = 2.0 ** -24
-
-
-def dev():
-    if not torch.cuda.is_available():
-        pytest.fail("no CUDA device: -m gpu tests must run on a GPU machine")
-    return torch.device("cuda", 0)
-
-
-def stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def hub_graph():
-    """R-MAT (6000 vertices) with a hub row of 3000 entries, rows of one entry (rows 20..29) and empty rows (10..19)."""
-    A = sp.coo_matrix(graphio.synthetic_graph(6000, 120000, seed=31))
-    keep = (A.row < 10) | (A.row >= 30)
-    row = np.concatenate([A.row[keep], np.zeros(3000, np.int64), np.arange(20, 30)])
-    col = np.concatenate([A.col[keep], np.arange(3000) * 2, np.arange(20, 30) + 100])
-    B = sp.csr_matrix((np.ones(len(row), np.float32), (row, col)), shape=A.shape)
-    B.sum_duplicates()
-    return B.tocoo()
-
-
-def problem(case):
-    if case == "hub":
-        A = hub_graph()
-        return A, np.zeros(A.shape[0], dtype=np.int64), 1
-    if case == "karate":
-        z = np.load(os.path.join(GOLDEN, "pgat_karate_k3.npz"))
-        n = int(z["n"])
-        return sp.coo_matrix((z["val"], (z["row"], z["col"])), shape=(n, n)), z["partvec"].astype(np.int64), 3
-    g = Golden(case)
-    return g.A, g.partvec, g.k
-
-
-def edges(lp):
-    return np.repeat(np.arange(lp.m), np.diff(lp.rowptr.astype(np.int64))), lp.colidx.astype(np.int64)
-
-
-def one_rank_plan(case, f):
-    A, _, _ = problem(case)
-    plan = planmod.build_plan(A, np.zeros(A.shape[0], dtype=np.int64), 0, 1, f, device=dev())
-    plan.bind_values()
-    return A, plan
-
-
-def t(x):
-    return torch.from_numpy(np.ascontiguousarray(x)).to(dev())
-
-
-def shifted(x):
-    """A copy of x whose data starts 4 bytes into its buffer."""
-    buf = torch.empty(x.numel() + 1, dtype=x.dtype, device=x.device)
-    v = buf[1:].view(x.shape)
-    v.copy_(x)
-    return v
 
 
 def softmax_run(lib, plan, K, el, er, dal, slope):
@@ -300,25 +239,6 @@ def test_layer_gradients_one_rank(f, K, layout):
     plan.close()
 
 
-def make_plans(lps, f, overlap):
-    plans = [planmod.PgcnPlan(lp, f, device=dev()) for lp in lps]
-    planmod.link_local_plans(plans)
-    for p in plans:
-        p.set_option("overlap", overlap)
-        p.bind_values()
-    return plans
-
-
-def run_ranks(plans, fn, streams):
-    torch.cuda.synchronize()
-    out = [None] * len(plans)
-    for r, s in enumerate(streams):
-        with torch.cuda.stream(s):
-            out[r] = fn(r)
-    torch.cuda.synchronize()
-    return out
-
-
 @pytest.mark.parametrize("overlap", [0, 1])
 @pytest.mark.parametrize("case,f,K", [("gemat11_k2", 40, 2), ("gemat11_k2", 128, 8), ("gemat11_k3_hp", 256, 4),
                                       ("karate", 16, 4)])
@@ -326,7 +246,7 @@ def test_layer_gradients_multi_rank(case, f, K, overlap):
     A, pv, k = problem(case)
     n = A.shape[0]
     lps = [planmod.build_local_plan(A, pv, r, k) for r in range(k)]
-    plans = make_plans(lps, f, overlap)
+    plans = linked_plans(lps, f, overlap)
     streams = [torch.cuda.Stream(device=dev()) for _ in plans]
     rs = np.random.RandomState(f + k + K)
     Zn = rs.uniform(-1, 1, size=(n, f)).astype(np.float32)
@@ -379,6 +299,12 @@ def test_resident_values_untouched():
     plan.close()
 
 
+def step(plan, x, W, a, g, K):
+    out = layer(plan, x, W, a, K)
+    out.backward(g)
+    return dict(out=out, dW=W.grad, da=a.grad)
+
+
 def test_one_rank_capture_and_refusal_before_prepare():
     A, plan = one_rank_plan("hub", 128)
     f, n, K = 128, A.shape[0], 4
@@ -387,29 +313,18 @@ def test_one_rank_capture_and_refusal_before_prepare():
     x, g = torch.zeros((n, f), device=dev()), torch.zeros((n, f), device=dev())
     W = torch.zeros((f, f), device=dev(), requires_grad=True)
     a = torch.zeros((2 * f // K, K), device=dev(), requires_grad=True)
-    s = torch.cuda.Stream()
-    with pytest.raises(RuntimeError, match="pgcn_plan_prepare"):
-        with torch.cuda.graph(torch.cuda.CUDAGraph(), stream=s):
-            layer(plan, x, W, a, K).backward(g)
-    W.grad = a.grad = None
-    plan.prepare(f)
-    plan.prepare(4 * K)
-    graph = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(graph):
-        out = layer(plan, x, W, a, K)
-        out.backward(g)
     ins = [(rnd(n, f), rnd(n, f), rnd(f, f) * 0.1, rnd(2 * f // K, K) * 0.1) for _ in range(3)]
-    for i in (0, 1, 2, 1):
-        xi, gi, Wi, ai = ins[i]
+
+    def load(i):
         with torch.no_grad():
-            x.copy_(xi); g.copy_(gi); W.copy_(Wi); a.copy_(ai)
-        graph.replay()
-        got = [u.detach().clone() for u in (out, W.grad, a.grad)]
-        We, ae = Wi.clone().requires_grad_(True), ai.clone().requires_grad_(True)
-        oe = layer(plan, xi, We, ae, K)
-        oe.backward(gi)
-        for name, u, w in zip(("out", "dW", "da"), got, (oe, We.grad, ae.grad)):
-            assert torch.equal(u, w.detach()), "replay %d: %s differs from eager" % (i, name)
+            for u, v in zip((x, g, W, a), ins[i]):
+                u.copy_(v)
+
+    def eager(i):
+        xi, gi, Wi, ai = ins[i]
+        return step(plan, xi, Wi.clone().requires_grad_(True), ai.clone().requires_grad_(True), gi, K)
+
+    check_one_rank_capture(plan, lambda: step(plan, x, W, a, g, K), load, eager, prepare=(f, 4 * K), leaves=(W, a))
     plan.close()
 
 
@@ -417,7 +332,7 @@ def test_two_rank_capture_over_the_peer_transport():
     A, pv, k = problem("gemat11_k2")
     f, n, K = 128, A.shape[0], 8
     lps = [planmod.build_local_plan(A, pv, r, k) for r in range(k)]
-    plans = make_plans(lps, f, 1)
+    plans = linked_plans(lps, f, 1)
     for p in plans:
         p.prepare(f)
         p.prepare(4 * K)
@@ -443,63 +358,18 @@ def test_two_rank_capture_over_the_peer_transport():
                 b["W"].copy_(torch.from_numpy(Wn)); b["a"].copy_(torch.from_numpy(an))
         torch.cuda.synchronize()
 
-    def step(r, b):
-        o = layer(plans[r], b["x"], b["W"], b["a"], K)
-        o.backward(b["g"])
-        return o
-
-    cap = [buffers(r) for r in range(k)]
-    graphs, outs = [], []
-    for r in range(k):
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph, stream=streams[r]):
-            outs.append(step(r, cap[r]))
-        graphs.append(graph)
-    lib = cabi.load()
-    for it, i in enumerate((0, 1, 2, 1)):
-        load(cap, i)
-        run_ranks(plans, lambda r: graphs[r].replay(), streams)
-        got = [(outs[r].detach().clone(), cap[r]["W"].grad.clone(), cap[r]["a"].grad.clone()) for r in range(k)]
-        eager = [buffers(r) for r in range(k)]
-        load(eager, i)
-        res = run_ranks(plans, lambda r: step(r, eager[r]), streams)
-        for r in range(k):
-            for name, u, w in zip(("out", "dW", "da"), got[r], (res[r], eager[r]["W"].grad, eager[r]["a"].grad)):
-                assert torch.equal(u, w.detach()), "step %d rank %d: %s replay differs from eager" % (it, r, name)
-        if it == 1:                                    # one more fused call: the later replays see the other parity
-            run_ranks(plans, lambda r: cabi.check(lib.pgcn_forward(plans[r].handle, eager[r]["x"].data_ptr(),
-                                                                   torch.empty_like(eager[r]["x"]).data_ptr(), f,
-                                                                   stream()), plans[r].handle), streams)
+    check_two_rank_capture(plans, streams, buffers, load,
+                           lambda r, b: step(plans[r], b["x"], b["W"], b["a"], b["g"], K))
     for p in plans:
         p.close()
 
 
-def run_cli(tmp_path, extra, port):
-    from scipy.io import mmwrite
-    z = np.load(os.path.join(GOLDEN, "pgat_karate_k1.npz"))
-    n = int(z["n"])
-    A = sp.coo_matrix((z["val"], (z["row"], z["col"])), shape=(n, n))
-    a = str(tmp_path / "karate.mtx")
-    mmwrite(a, A)
-    p = str(tmp_path / "karate.mtx.1.rp")
-    graphio.write_partvec(p, np.zeros(n, dtype=np.int64))
-    env = dict(os.environ, SLURM_NPROCS="1", SLURM_PROCID="0", MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-    out = subprocess.run([sys.executable, os.path.join(ROOT, "PGAT.py"), "-a", a, "-p", p, "-b", "nccl", "-s", "1",
-                          "-l", "2", "-f", "4", "--seed", "7"] + extra, env=env, capture_output=True, text=True,
-                         timeout=600)
-    assert out.returncode == 0, out.stderr[-2000:]
-    return A, [l for l in out.stdout.splitlines() if l.startswith("Epoch")]
-
-
 def test_cli_heads_follows_the_fp64_loss_curve(tmp_path):
-    A, lines = run_cli(tmp_path, ["--heads", "2"], 29671)
-    assert [l[:11] for l in lines] == ["Epoch %05d" % i for i in range(50)]
-    want = ho.intended_training(A, 2, 4, 7, 1.0, heads=2)
-    got = [float(l.split("Loss")[1]) for l in lines]
-    np.testing.assert_allclose(got, want, rtol=1e-3, atol=6e-5)
+    lines = run_cli(tmp_path, "PGAT.py", ["--heads", "2"], 29671)
+    assert_follows(lines, ho.intended_training(karate(), 2, 4, 7, 1.0, heads=2))
 
 
 def test_cli_heads_one_prints_what_no_flag_prints(tmp_path):
-    _, plain = run_cli(tmp_path, [], 29672)
-    _, one = run_cli(tmp_path, ["--heads", "1"], 29673)
+    plain = run_cli(tmp_path, "PGAT.py", [], 29672)
+    one = run_cli(tmp_path, "PGAT.py", ["--heads", "1"], 29673)
     assert len(plain) == 50 and one == plain

@@ -21,6 +21,7 @@ import scipy.sparse as sp
 import torch
 import torch.nn.functional as F
 
+from harness import EPS, bits, dev, hub_graph, stream
 from helpers import assert_close_fp32, fp32_tol
 from oracle import pgcn_oracle as orc
 from pgcn_b200 import cabi, graphio, op, plan as planmod
@@ -28,19 +29,8 @@ from pgcn_b200.op import PGATAttention, PSpMM, PSpMMRelu, PSpMMWeighted
 from test_gpu_parity import skewed_graph
 
 pytestmark = pytest.mark.gpu
-EPS = 2.0 ** -24
 SENTINEL = 0x7FBADBAD                    # a NaN payload no kernel produces: any write to a guard float changes it
 N, NNZ, F_MAX = 3000, 60000, 640
-
-
-def dev():
-    if not torch.cuda.is_available():
-        pytest.fail("no CUDA device: -m gpu tests must run on a GPU machine")
-    return torch.device("cuda", 0)
-
-
-def stream():
-    return torch.cuda.current_stream().cuda_stream
 
 
 def ptr(x):
@@ -87,16 +77,12 @@ def check_guards():
         assert bool((b[:lo] == SENTINEL).all()) and bool((b[hi:] == SENTINEL).all()), "write outside the operand"
 
 
-def bits(x):
-    return x.detach().contiguous().view(torch.int32).cpu().numpy()
-
-
 def assert_bits(got, want, what):
     g, w = bits(got), bits(want)
     assert g.shape == w.shape and np.array_equal(g, w), "%s: %d elements differ in their bits" % (what, int((g != w).sum()))
 
 
-def make_plans(A, k, f_max=F_MAX, link=True, seed=5):
+def random_plans(A, k, f_max=F_MAX, link=True, seed=5):
     pv = graphio.random_partvec(A.shape[0], k, seed=seed)
     plans = [planmod.build_plan(A, pv, r, k, f_max, device=dev()) for r in range(k)]
     if k > 1 and link:
@@ -156,7 +142,7 @@ def test_spmm_pack_unpack_unaligned(f, shift):
     bound of fp64, exact copies for the pack. Hub rows are split (edges_per_block 16), so the fixup writes into the
     unaligned Z; empty rows are zero-filled there."""
     A = skewed_graph(N, NNZ, seed=7)
-    plans = make_plans(A, 2, link=False)
+    plans = random_plans(A, 2, link=False)
     rs = np.random.RandomState(f)
     H = rs.uniform(-1, 1, size=(N, f)).astype(np.float32)
     G = rs.uniform(-1, 1, size=(N, f)).astype(np.float32)
@@ -229,7 +215,7 @@ def test_fused_forward_backward_unaligned(k, f, s):
     ranks have to agree), the input, the output or both misaligned: bit-identical to aligned copies on the register
     kernel, within the fp32 bound of fp64."""
     A = skewed_graph(N, NNZ, seed=9)
-    plans = make_plans(A, k)
+    plans = random_plans(A, k)
     rs = np.random.RandomState(10 * k + f)
     H = rs.uniform(-1, 1, size=(N, f)).astype(np.float32)
     G = rs.uniform(-1, 1, size=(N, f)).astype(np.float32)
@@ -286,7 +272,7 @@ def test_keep_halo_and_halo_rows_unaligned(k, w, shift):
     and with H_own and Z): the halo rows are exact copies of their owners' rows, Z is bit-identical to the aligned
     call (register kernel when H_own / Z are misaligned)."""
     A = skewed_graph(N, NNZ, seed=13)
-    plans = make_plans(A, k)
+    plans = random_plans(A, k)
     for p in plans:
         p.bind_values()
     X = np.random.RandomState(w + k).uniform(-1, 1, size=(N, w)).astype(np.float32)
@@ -344,7 +330,7 @@ def test_sddmm_softmax_set_values_unaligned(k, f, shift):
     identical), pgcn_edge_softmax(_backward) (bit-identical to the aligned call, every argument misaligned on its own
     and all at once), pgcn_plan_set_values from an unaligned array (the aggregation that follows is bit-identical)."""
     A = skewed_graph(N, NNZ, seed=15)
-    plans = make_plans(A, k, link=False)
+    plans = random_plans(A, k, link=False)
     rs = np.random.RandomState(f + shift)
     H = rs.uniform(-1, 1, size=(N, f)).astype(np.float32)
     for p in plans:
@@ -414,7 +400,7 @@ def test_autograd_ops_take_unaligned_views_uncopied(f, shift):
     """PSpMM, PSpMMRelu, PSpMMWeighted and PGATAttention (local layout) fed unaligned views: _check_feat passes them
     through uncopied, and outputs and gradients are bit-identical to aligned copies on the register kernel."""
     A = skewed_graph(N, NNZ, seed=19)
-    p = make_plans(A, 1)[0]
+    p = random_plans(A, 1)[0]
     p.bind_values()
     rs = np.random.RandomState(f * shift)
     X = torch.from_numpy(rs.uniform(-1, 1, size=(N, f)).astype(np.float32)).to(dev())
@@ -462,7 +448,7 @@ def test_capture_with_unaligned_buffers(f, shift):
     buffers: the capture is not refused, and replays on new inputs are bit-identical to eager calls on the same
     unaligned buffers."""
     A = skewed_graph(N, NNZ, seed=23)
-    p = make_plans(A, 1)[0]
+    p = random_plans(A, 1)[0]
     p.prepare(f)
     rs = np.random.RandomState(f + shift)
     xs = [rs.uniform(-1, 1, size=(N, f)).astype(np.float32) for _ in range(3)]
@@ -510,7 +496,7 @@ def special_graph():
     (A, dead columns, pad rows).
 
     The pad rows are the rows behind local column 0 on one rank (global row 0) and on each rank of the 2-way
-    partition make_plans uses (its first owned row). Padding entries of the piece records, and the register kernel's
+    partition random_plans uses (its first owned row). Padding entries of the piece records, and the register kernel's
     lanes past a block's end, hold column 0 with value 0. So a kernel that multiplied them in would read exactly these
     rows. They are dead columns, and their rows of A are emptied too, so that nothing references them in the transposed
     product either."""
@@ -581,8 +567,8 @@ def test_nonfinite_features(cfg):
     A, dead_cols, pads = special_graph()
     n = A.shape[0]
     rs = np.random.RandomState(f)
-    plans2 = make_plans(A, 2, link=False)
-    p1 = make_plans(A, 1)[0]
+    plans2 = random_plans(A, 2, link=False)
+    p1 = random_plans(A, 1)[0]
     everyone = [p1] + plans2
     set_opts(everyone, edges_per_block=16, ring_edges_per_block=64, **opts)
     # local column 0 of every plan, where padding entries point, is one of the pad rows
@@ -637,7 +623,7 @@ def test_zero_edge_values_times_inf_give_nan(f):
     rows that reach it through a non-zero edge are +-Inf."""
     A, _, _ = special_graph()
     n = A.shape[0]
-    p = make_plans(A, 1)[0]
+    p = random_plans(A, 1)[0]
     p.bind_values()
     lp = p.lp
     rs = np.random.RandomState(f)
@@ -666,7 +652,7 @@ def test_sddmm_nonfinite(f):
     f = 40, ring kernel at f = 128), with the class of the fp64 dot product."""
     A, _, _ = special_graph()
     n = A.shape[0]
-    p = make_plans(A, 1)[0]
+    p = random_plans(A, 1)[0]
     lp = p.lp
     rs = np.random.RandomState(f + 1)
     # one feature per row: a dot product with a single infinite term stays infinite
@@ -696,9 +682,8 @@ def softmax64(rows, m, s):
 def test_edge_softmax_nonfinite_scores():
     """+-Inf and NaN in el and er: the NaN / zero / finite pattern of alpha, dpre and d_el equals that of an fp64 softmax
     with torch's semantics (checked against torch.softmax on the special rows); warp rows and a CTA hub row."""
-    from test_attention import hub_graph
     A = hub_graph()
-    p = make_plans(A, 1)[0]
+    p = random_plans(A, 1)[0]
     p.bind_values()
     lp = p.lp
     m = lp.m
@@ -763,7 +748,7 @@ def test_fused_relu_keeps_nan(k, f):
     by the fixup. At the layer level PSpMMRelu(A, linear(H)) has the NaN pattern of relu(PSpMM(A, linear(H)))."""
     A, _, _ = special_graph()
     n = A.shape[0]
-    plans = make_plans(A, k)
+    plans = random_plans(A, k)
     rs = np.random.RandomState(k * f)
     X0 = rs.uniform(-1, 1, size=(n, f)).astype(np.float32)
     hrows, _ = special_rows(A, [], planmod.build_local_plan(A, graphio.random_partvec(n, 2, seed=5), 0, 2).halo, rs)
@@ -806,7 +791,7 @@ def test_subnormal_products(cfg):
     name, f, opts = cfg
     A, _, _ = special_graph()
     n = A.shape[0]
-    p = make_plans(A, 1)[0]
+    p = random_plans(A, 1)[0]
     set_opts([p], edges_per_block=16, ring_edges_per_block=64, **opts)
     lp = p.lp
     rs = np.random.RandomState(f)

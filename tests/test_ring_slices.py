@@ -8,7 +8,7 @@ import torch
 from helpers import assert_close_fp32, fp32_tol
 from oracle import pgcn_oracle as orc
 from pgcn_b200 import graphio
-from test_gpu_parity import backward_all, forward_all, make_plans, skewed_graph
+from test_gpu_parity import backward_all, build_plans, forward_all, skewed_graph
 
 pytestmark = pytest.mark.gpu
 
@@ -33,7 +33,7 @@ def test_sliced_ring_matches_truth_and_full_width(f, opts):
     tolZ = fp32_tol(A, H, int(orc.row_degree(A).max())); tolG = fp32_tol(A.T, G, int(orc.row_degree(A.T).max()))
     for k in (1, 2):
         pv = np.zeros(n, dtype=np.int64) if k == 1 else graphio.random_partvec(n, 2, seed=5)
-        plans = make_plans(A, pv, k, f)
+        plans = build_plans(A, pv, k, f)
         zs = forward_all(plans, H, ring_tile_floats=64, **opts)
         gs = backward_all(plans, G)
         zs2 = forward_all(plans, H)
@@ -55,7 +55,7 @@ def test_tile_option_and_autotune():
     n, f = 6000, 256
     A = skewed_graph(n, 150000, seed=13)
     H = np.random.RandomState(4).uniform(-1, 1, size=(n, f)).astype(np.float32)
-    p = make_plans(A, np.zeros(n, dtype=np.int64), 1, f)[0]
+    p = build_plans(A, np.zeros(n, dtype=np.int64), 1, f)[0]
     assert p.get_option("ring_tile_floats") == 0
     with pytest.raises(RuntimeError):
         p.set_option("ring_tile_floats", 96)

@@ -7,7 +7,7 @@ import pytest
 import torch
 
 from pgcn_b200 import graphio
-from test_gpu_parity import backward_all, forward_all, make_plans, skewed_graph
+from test_gpu_parity import backward_all, build_plans, forward_all, skewed_graph
 
 pytestmark = pytest.mark.gpu
 
@@ -27,7 +27,7 @@ def test_warp_copies_match_lane_copies_and_full_width(f, k, sched):
     H = rng.uniform(-1, 1, size=(n, f)).astype(np.float32)
     G = rng.uniform(-1, 1, size=(n, f)).astype(np.float32)
     pv = np.zeros(n, dtype=np.int64) if k == 1 else graphio.random_partvec(n, 2, seed=7)
-    plans = make_plans(A, pv, k, f)
+    plans = build_plans(A, pv, k, f)
     # kernel 5 (1-D bulk, one copy per lane) has the 16- and 32-slot rings; kernel 7 also has the two 64-slot rings
     ref = {}
     for tile in (64, 128):
