@@ -409,6 +409,9 @@ int pgcn_forward_host(pgcn_plan* plan, const float* H_host, float* Z_host, int32
  * enqueued so far. Pinned host buffers are needed for the copies to overlap. Replaces nothing in the reference
  * (it has no host-resident path, GPU/PGCN.py:186-196 keeps H on the device): it is the C-trainer-facing form of
  * the PSpMM.forward boundary (GPU/PGCN.py:123-127).
+ * On a multi-rank plan the call advances the exchange epoch on the plan's own stream, which is not ordered with the
+ * caller's streams: every earlier call of the plan must have completed before it (synchronise the caller's stream),
+ * and no other call of the plan may be enqueued between it and pgcn_forward_host_wait.
  */
 int pgcn_forward_host_async(pgcn_plan* plan, const float* H_host, float* Z_host, int32_t f);
 int pgcn_forward_host_wait(pgcn_plan* plan);
