@@ -1,6 +1,7 @@
 """Build the native pieces in-tree (so the .so files travel to the GPU box with the snapshot).
 
-  lib/libpgcn_b200.so   csrc/pgcn_b200.cu (+ spmm_kernels.cuh, spmm_ring.cuh, sddmm.cuh, attention.cuh, spmm_max.cuh, gatv2.cuh)   nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo
+  lib/libpgcn_b200.so     csrc/pgcn_b200.cu (+ spmm_kernels.cuh, spmm_ring.cuh, sddmm.cuh, attention.cuh, spmm_max.cuh, gatv2.cuh)   nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo
+  lib/libpgcn_dropout.so  csrc/edge_dropout.cu (+ philox.cuh)                                                                        the same flags
   (the CPU oracle under oracle/ is built by oracle/build_oracle.py — test infrastructure only)
 
 nvcc cross-compiles without a GPU; `python -m <pkg>.build` or `__graft_entry__.build()` runs this.
@@ -24,6 +25,11 @@ DEPS = SOURCES + [os.path.join(CSRC, "spmm_kernels.cuh"), os.path.join(CSRC, "sp
                   os.path.join(CSRC, "sddmm.cuh"), os.path.join(CSRC, "attention.cuh"), os.path.join(CSRC, "spmm_max.cuh"),
                   os.path.join(CSRC, "gatv2.cuh"),
                   os.path.join(ROOT, "include", "pgcn_b200.h"), os.path.abspath(__file__)]
+# the edge-dropout library has its own sources and dependency list: editing one library never rebuilds the other
+DROPOUT_LIB = os.path.join(LIBDIR, "libpgcn_dropout.so")
+DROPOUT_SOURCES = [os.path.join(CSRC, "edge_dropout.cu")]
+DROPOUT_DEPS = DROPOUT_SOURCES + [os.path.join(CSRC, "philox.cuh"), os.path.join(ROOT, "include", "pgcn_dropout.h"),
+                                  os.path.abspath(__file__)]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -39,32 +45,52 @@ def _nvcc():
     return None
 
 
-def is_stale():
-    if not os.path.exists(LIB):
+def _stale(lib, deps):
+    if not os.path.exists(lib):
         return True
-    t = os.path.getmtime(LIB)
-    return any(os.path.getmtime(d) > t for d in DEPS if os.path.exists(d))
+    t = os.path.getmtime(lib)
+    return any(os.path.getmtime(d) > t for d in deps if os.path.exists(d))
+
+
+def is_stale():
+    return _stale(LIB, DEPS)
+
+
+def dropout_is_stale():
+    return _stale(DROPOUT_LIB, DROPOUT_DEPS)
+
+
+def _compile(lib, sources, defs, verbose):
+    nvcc = _nvcc()
+    if nvcc is None:
+        raise RuntimeError("nvcc not found: cannot build %s (no prebuilt library either)" % os.path.basename(lib))
+    os.makedirs(LIBDIR, exist_ok=True)
+    tmp = lib + ".tmp.%d" % os.getpid()
+    cmd = [nvcc] + NVCC_FLAGS + defs + (["-Xptxas", "-v"] if verbose else []) + ["-o", tmp] + sources + ["-ldl"]
+    res = subprocess.run(cmd, capture_output=True, text=True)
+    if res.returncode != 0:
+        raise RuntimeError("nvcc failed:\n" + " ".join(cmd) + "\n" + res.stdout + res.stderr)
+    if verbose:
+        sys.stderr.write(res.stderr)
+    os.replace(tmp, lib)
+    return lib
 
 
 def build(force=False, verbose=False):
     """Compile libpgcn_b200.so for sm_90a if missing or older than its sources. Returns its path."""
     if not force and not is_stale():
         return LIB
-    nvcc = _nvcc()
-    if nvcc is None:
-        raise RuntimeError("nvcc not found: cannot build libpgcn_b200.so (no prebuilt library either)")
-    os.makedirs(LIBDIR, exist_ok=True)
-    tmp = LIB + ".tmp.%d" % os.getpid()
-    defs = os.environ.get("PGCN_B200_DEFS", "").split() if _VARIANT else []
-    cmd = [nvcc] + NVCC_FLAGS + defs + (["-Xptxas", "-v"] if verbose else []) + ["-o", tmp] + SOURCES + ["-ldl"]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    if res.returncode != 0:
-        raise RuntimeError("nvcc failed:\n" + " ".join(cmd) + "\n" + res.stdout + res.stderr)
-    if verbose:
-        sys.stderr.write(res.stderr)
-    os.replace(tmp, LIB)
-    return LIB
+    return _compile(LIB, SOURCES, os.environ.get("PGCN_B200_DEFS", "").split() if _VARIANT else [], verbose)
+
+
+def build_dropout(force=False, verbose=False):
+    """Compile libpgcn_dropout.so for sm_90a if missing or older than its sources. Returns its path."""
+    if not force and not dropout_is_stale():
+        return DROPOUT_LIB
+    return _compile(DROPOUT_LIB, DROPOUT_SOURCES, [], verbose)
 
 
 if __name__ == "__main__":
-    print(build(force="--force" in sys.argv, verbose="-v" in sys.argv))
+    force, verbose = "--force" in sys.argv, "-v" in sys.argv
+    print(build(force=force, verbose=verbose))
+    print(build_dropout(force=force, verbose=verbose))

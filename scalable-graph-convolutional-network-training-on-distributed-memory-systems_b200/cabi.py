@@ -1,7 +1,7 @@
-"""ctypes binding of include/pgcn_b200.h — the C-ABI drop-in boundary (SURVEY.md §8b).
+"""ctypes binding of include/pgcn_b200.h — the C-ABI drop-in boundary (SURVEY.md §8b) — and of include/pgcn_dropout.h.
 
-Nothing here computes: it loads lib/libpgcn_b200.so, declares every exported symbol and turns
-negative status codes into RuntimeError. If the library is missing there is no fallback: the
+Nothing here computes: it loads lib/libpgcn_b200.so (load) and lib/libpgcn_dropout.so (load_dropout), declares every
+exported symbol and turns negative status codes into RuntimeError. If the library is missing there is no fallback: the
 product path fails loudly (the CPU oracle under oracle/ is test infrastructure only).
 """
 import ctypes as C
@@ -26,6 +26,9 @@ SYMBOLS = [
     "pgcn_sddmm_heads", "pgcn_forward_max", "pgcn_backward_max", "pgcn_forward_gatv2", "pgcn_backward_gatv2",
 ]
 
+# every symbol declared in include/pgcn_dropout.h
+DROPOUT_SYMBOLS = ["pgcn_dropout_version", "pgcn_dropout_last_error", "pgcn_edge_dropout"]
+
 
 class PgcnBytes(C.Structure):
     _fields_ = [(n, C.c_int64) for n in (
@@ -36,10 +39,29 @@ class PgcnBytes(C.Structure):
 
 
 _lib = None
+_dropout = None
 
 
 def lib_path():
     return _build.LIB
+
+
+def dropout_lib_path():
+    return _build.DROPOUT_LIB
+
+
+def _built(path, stale, build, build_if_missing):
+    """path, rebuilt first when stale and nvcc is available; a missing library raises."""
+    if build_if_missing and stale():
+        try:
+            build()
+        except RuntimeError:
+            if not os.path.exists(path):
+                raise
+    if not os.path.exists(path):
+        raise RuntimeError("%s is missing (%s): build it with __graft_entry__.build(); there is no CPU fallback for "
+                           "the PGCN hot path" % (os.path.basename(path), path))
+    return path
 
 
 def load(build_if_missing=True):
@@ -47,16 +69,7 @@ def load(build_if_missing=True):
     global _lib
     if _lib is not None:
         return _lib
-    path = _build.LIB
-    if build_if_missing and _build.is_stale():
-        try:
-            _build.build()
-        except RuntimeError:
-            if not os.path.exists(path):
-                raise
-    if not os.path.exists(path):
-        raise RuntimeError("libpgcn_b200.so is missing (%s): build it with __graft_entry__.build(); "
-                           "there is no CPU fallback for the PGCN hot path" % path)
+    path = _built(_build.LIB, _build.is_stale, _build.build, build_if_missing)
     lib = C.CDLL(path, mode=C.RTLD_GLOBAL)
     vp, i32, i64 = C.c_void_p, C.c_int32, C.c_int64
     lib.pgcn_version.restype = C.c_char_p
@@ -154,4 +167,29 @@ def check(rc, plan=None):
     if rc < 0:
         msg = load().pgcn_last_error(plan)
         raise RuntimeError("pgcn_b200 error %d: %s" % (rc, (msg or b"").decode("utf-8", "replace")))
+    return rc
+
+
+def load_dropout(build_if_missing=True):
+    """Load libpgcn_dropout.so (building it first when stale and nvcc is available)."""
+    global _dropout
+    if _dropout is not None:
+        return _dropout
+    lib = C.CDLL(_built(_build.DROPOUT_LIB, _build.dropout_is_stale, _build.build_dropout, build_if_missing))
+    lib.pgcn_dropout_version.restype = C.c_char_p
+    lib.pgcn_dropout_version.argtypes = []
+    lib.pgcn_dropout_last_error.restype = C.c_char_p
+    lib.pgcn_dropout_last_error.argtypes = []
+    lib.pgcn_edge_dropout.restype = C.c_int
+    lib.pgcn_edge_dropout.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_uint32, C.c_float, C.c_void_p, C.c_void_p,
+                                      C.c_void_p, C.c_void_p]
+    _dropout = lib
+    return lib
+
+
+def check_dropout(rc):
+    """Raise RuntimeError carrying pgcn_dropout_last_error when a libpgcn_dropout call returned a negative status."""
+    if rc < 0:
+        msg = load_dropout().pgcn_dropout_last_error()
+        raise RuntimeError("pgcn_dropout error %d: %s" % (rc, (msg or b"").decode("utf-8", "replace")))
     return rc

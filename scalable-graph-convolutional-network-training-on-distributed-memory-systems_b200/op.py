@@ -226,11 +226,115 @@ class PSpMMWeighted(torch.autograd.Function):
         return None, dvals, dH
 
 
+# ---- edge dropout (libpgcn_dropout.so) -------------------------------------------------------------------------------
+
+def dropout_constants(p):
+    """(threshold, scale) of drop probability p in [0, 1): threshold = floor(p 2^32) in fp64, an entry is kept when its
+    Philox word is >= threshold; scale = float32(1 / (1 - p)), the fp64 quotient rounded once."""
+    import math
+    import numpy as np
+    p = float(p)
+    if not 0.0 <= p < 1.0:
+        raise ValueError("dropout probability p=%r must lie in [0, 1)" % p)
+    return int(math.floor(p * 4294967296.0)), float(np.float32(1.0 / (1.0 - p)))
+
+
+class EdgeDropout:
+    """Dropout on per-edge arrays in forward-CSR order whose mask is a pure function of the global edge (include/
+    pgcn_dropout.h): entry (global row gi, global column gj), head h, keep iff word h & 3 of Philox4x32-10(counter =
+    (gi, gj, c, h >> 2), key) >= floor(p 2^32); kept values are scaled by float32(1 / (1 - p)), dropped ones multiplied
+    by 0. Any partition of a graph, and one GPU or k, draw the same mask.
+
+        EdgeDropout(p, key, device)     p in [0, 1), key a 64-bit integer
+
+    `state` is the device int64 [key, c]. Every use on an operator (edge_dropout, PGATAttention,
+    PGATMultiHeadAttention) adds 1 to c on the device, in stream order, and uses the new value, so the first use draws
+    with c = 1 and a captured CUDA graph draws a new mask on every replay; the backward reuses its own forward's c. With
+    p == 0 the operators make no dropout launch at all."""
+
+    def __init__(self, p, key, device=None):
+        self.p = float(p)
+        self.threshold, self.scale = dropout_constants(self.p)
+        key = int(key)
+        if not 0 <= key < 2 ** 64:
+            raise ValueError("key=%d must lie in [0, 2^64)" % key)
+        self.state = torch.tensor([key - 2 ** 64 if key >= 2 ** 63 else key, 0], dtype=torch.int64,
+                                  device=torch.device("cuda", torch.cuda.current_device()) if device is None else device)
+
+    def draw(self):
+        """Advance the call counter (on the device, current stream) and return a snapshot [key, c] of the new state."""
+        self.state[1:].add_(1)
+        return self.state.clone()
+
+
+def _active(drop):
+    return drop if drop is not None and drop.p > 0 else None
+
+
+def _mask(pairs, snap, drop, x, y):
+    """y = the mask of `drop` at the state `snap` applied to x ([nnz] or [nnz, K], contiguous); y may be x."""
+    K = x.shape[1] if x.dim() == 2 else 1
+    with torch.cuda.device(x.device):
+        cabi.check_dropout(cabi.load_dropout().pgcn_edge_dropout(pairs.data_ptr(), pairs.shape[0], K, drop.threshold,
+                                                                 drop.scale, snap.data_ptr(), x.data_ptr(),
+                                                                 y.data_ptr(), _stream_ptr()))
+    return y
+
+
+def _dropout_pairs(A, drop):
+    """A.edge_pairs() when `drop` is active, else None. Operators call it before anything else, so that a capture that
+    needs the pairs before they exist is refused before it enqueues any work."""
+    if drop is None:
+        return None
+    if drop.state.device != A.device:
+        raise ValueError("the EdgeDropout state lives on %s, the plan on %s" % (drop.state.device, A.device))
+    return A.edge_pairs()
+
+
+class EdgeDropoutFunction(torch.autograd.Function):
+    """y = mask(x) for x [nnz] or [nnz, K] (K in 1, 2, 4, 8) in A's forward-CSR order; the gradient is the same map
+    with the same counter. Use edge_dropout()."""
+
+    @staticmethod
+    def forward(ctx, A, x, drop):
+        pairs = _dropout_pairs(A, drop)
+        snap = drop.draw()
+        y = _mask(pairs, snap, drop, x, torch.empty_like(x))
+        ctx.plan, ctx.drop = A, drop
+        ctx.save_for_backward(snap)
+        return y
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        (snap,) = ctx.saved_tensors
+        g = grad_output.contiguous()
+        return None, _mask(ctx.plan.edge_pairs(), snap, ctx.drop, g, torch.empty_like(g)), None
+
+
+def edge_dropout(A, x, drop):
+    """Edge dropout of a per-edge array: x is fp32 CUDA [nnz] or [nnz, K] (K in 1, 2, 4, 8) in A's local forward-CSR
+    order (A.edge_index()), drop an EdgeDropout or None. Differentiable. With drop None or p == 0 it returns x itself.
+    DropEdge-style value dropout: PSpMMWeighted.apply(A, edge_dropout(A, vals, drop), H)."""
+    if _active(drop) is None:
+        return x
+    _dropout_pairs(A, drop)
+    _check_f32(x, "x")
+    nnz = A.lp.nnz()
+    if x.dim() not in (1, 2) or x.shape[0] != nnz or (x.dim() == 2 and x.shape[1] not in HEADS):
+        raise ValueError("x must be [%d] or [%d, K] with K in 1, 2, 4, 8, got %s" % (nnz, nnz, tuple(x.shape)))
+    if x.device != A.device:
+        raise ValueError("x lives on %s, the plan on %s" % (x.device, A.device))
+    return EdgeDropoutFunction.apply(A, x.contiguous(), drop)
+
+
+HEADS = (1, 2, 4, 8)
+
+
 class PGATAttention(torch.autograd.Function):
     """Single-head sparse graph attention over the plan's stored pattern (GPU/PGAT.py:139-148 without the dense n x n
     score matrix):
 
-        PGATAttention.apply(A, Z, el, er, negative_slope)
+        PGATAttention.apply(A, Z, el, er, negative_slope, dropout=None)
         s_e = LeakyReLU(el[row(e)] + er[col(e)]),  alpha = softmax of s over each row's stored entries,  out = A(alpha) Z
 
     Z is [rows, f], el and er are [rows] fp32 CUDA tensors (rows = m in the "local" layout, n in the "global" one, whose
@@ -240,38 +344,48 @@ class PGATAttention(torch.autograd.Function):
     with the exchange; dalpha = SDDMM(gOut, [Z_own; Z_halo]); the softmax backward kernel gives dpre and d_el; and
     d_er = A(dpre)^T 1, the column sums of dpre with the halo partials summed at their owners (pgcn_backward on an
     m x 4 matrix of ones). Everything is deterministic. Gradients to W and a flow through torch, since el and er are
-    computed outside. The plan must be bound (PgcnPlan.bind_values); a later PSpMM on it restores the creation values."""
+    computed outside. The plan must be bound (PgcnPlan.bind_values); a later PSpMM on it restores the creation values.
+
+    dropout (an EdgeDropout with p > 0) applies attention dropout between the softmax and the aggregation: alpha_d =
+    mask(alpha) aggregates Z, and the backward takes dZ with alpha_d, dalpha = mask(dalpha_d) and the softmax backward
+    with the undropped alpha. alpha_d is kept for the backward (4 B per entry). None or p == 0: no dropout launch."""
 
     @staticmethod
-    def forward(ctx, A, Z, el, er, negative_slope=0.2):
+    def forward(ctx, A, Z, el, er, negative_slope=0.2, dropout=None):
+        drop = _active(dropout)
+        pairs = _dropout_pairs(A, drop)
         Z_own = _own(A, Z, "Z")
         el_own = _own_scores(A, el, "el")
         er_own = _own_scores(A, er, "er")
         _require_bound(A, "PGATAttention sets the plan's edge values")
+        snap = drop.draw() if drop else None
         lp, dev, slope = A.lp, Z_own.device, float(negative_slope)
         er_halo = _score_halo(A, er_own)
         alpha = torch.empty((lp.nnz(),), dtype=torch.float32, device=dev)
         _call(A, dev, "pgcn_edge_softmax", el_own.data_ptr(), er_own.data_ptr(), er_halo.data_ptr(), slope,
               alpha.data_ptr())
-        A.use_values(alpha)
+        alpha_d = _mask(pairs, snap, drop, alpha, torch.empty_like(alpha)) if drop else alpha
+        A.use_values(alpha_d)
         out, Z_halo = _aggregate(A, Z_own, keep_halo=True)
-        ctx.plan, ctx.slope = A, slope
-        ctx.save_for_backward(alpha, Z_own, Z_halo, el_own, er_own, er_halo)
+        ctx.plan, ctx.slope, ctx.drop = A, slope, drop
+        ctx.save_for_backward(alpha, Z_own, Z_halo, el_own, er_own, er_halo, alpha_d if drop else None, snap)
         return _to_layout(A, out)
 
     @staticmethod
     def backward(ctx, grad_output):
-        A, slope = ctx.plan, ctx.slope
-        alpha, Z_own, Z_halo, el_own, er_own, er_halo = ctx.saved_tensors
+        A, slope, drop = ctx.plan, ctx.slope, ctx.drop
+        alpha, Z_own, Z_halo, el_own, er_own, er_halo, alpha_d, snap = ctx.saved_tensors
         g = _own(A, grad_output, "grad_output")
         lp, f, dev = A.lp, g.shape[1], g.device
         dZ = d_el = d_er = None
         if ctx.needs_input_grad[1]:
-            A.use_values(alpha)
+            A.use_values(alpha_d if drop else alpha)
             dZ = _to_layout(A, _aggregate_t(A, g))
         if ctx.needs_input_grad[2] or ctx.needs_input_grad[3]:
             dalpha = torch.empty_like(alpha)
             _call(A, dev, "pgcn_sddmm", g.data_ptr(), Z_own.data_ptr(), _ptr(Z_halo), dalpha.data_ptr(), f)
+            if drop:
+                _mask(A.edge_pairs(), snap, drop, dalpha, dalpha)
             dpre = torch.empty_like(alpha)
             gel = torch.empty((lp.m,), dtype=torch.float32, device=dev)
             _call(A, dev, "pgcn_edge_softmax_backward", el_own.data_ptr(), er_own.data_ptr(), er_halo.data_ptr(),
@@ -281,17 +395,14 @@ class PGATAttention(torch.autograd.Function):
                 A.use_values(dpre)
                 ones = torch.ones((lp.m, 4), dtype=torch.float32, device=dev)
                 d_er = _to_layout(A, _aggregate_t(A, ones)[:, 0].contiguous())
-        return None, dZ, d_el, d_er, None
-
-
-HEADS = (1, 2, 4, 8)
+        return None, dZ, d_el, d_er, None, None
 
 
 class PGATMultiHeadAttention(torch.autograd.Function):
     """Multi-head sparse graph attention over the plan's stored pattern: K = el.shape[1] heads (1, 2, 4 or 8) of width
     d = f / K, concatenated.
 
-        PGATMultiHeadAttention.apply(A, Z, el, er, negative_slope)
+        PGATMultiHeadAttention.apply(A, Z, el, er, negative_slope, dropout=None)
         s_eh = LeakyReLU(el[row(e), h] + er[col(e), h]),  alpha_.h = softmax of s_.h over each row's stored entries,
         out[:, h d:(h+1) d] = A(alpha[:, h]) Z[:, h d:(h+1) d]
 
@@ -302,10 +413,15 @@ class PGATMultiHeadAttention(torch.autograd.Function):
     restore. Backward: dZ = A(alpha)^T gOut per head (pgcn_backward_heads), dalpha from pgcn_sddmm_heads, dpre and d_el
     from the softmax backward, d_er[:, h] = A(dpre[:, h])^T 1 (pgcn_backward_heads on an m x 4K matrix of ones, column
     4h), so the plan's f_max must be at least max(f, 4K). Deterministic. The exchange is the unsplit one (no per-source
-    overlap). The plan must be bound (PgcnPlan.bind_values)."""
+    overlap). The plan must be bound (PgcnPlan.bind_values).
+
+    dropout (an EdgeDropout with p > 0): attention dropout on every head, as PGATAttention; alpha_d = mask(alpha)
+    ([nnz, K]) is the alpha argument of the aggregation and is kept for the backward (4K B per entry)."""
 
     @staticmethod
-    def forward(ctx, A, Z, el, er, negative_slope=0.2):
+    def forward(ctx, A, Z, el, er, negative_slope=0.2, dropout=None):
+        drop = _active(dropout)
+        pairs = _dropout_pairs(A, drop)
         if el.dim() != 2:
             raise ValueError("el must be [%d, heads], got %s" % (_rows(A), tuple(el.shape)))
         K = el.shape[1]
@@ -321,33 +437,38 @@ class PGATMultiHeadAttention(torch.autograd.Function):
         el_own = _own_scores(A, el, "el", K)
         er_own = _own_scores(A, er, "er", K)
         _require_bound(A, "PGATMultiHeadAttention reads the plan's value maps")
+        snap = drop.draw() if drop else None
         lp, dev, slope = A.lp, Z_own.device, float(negative_slope)
         er_halo = _score_halo(A, er_own)
         alpha = torch.empty((lp.nnz(), K), dtype=torch.float32, device=dev)
         _call(A, dev, "pgcn_edge_softmax_heads", K, el_own.data_ptr(), er_own.data_ptr(), er_halo.data_ptr(), slope,
               alpha.data_ptr())
+        alpha_d = _mask(pairs, snap, drop, alpha, torch.empty_like(alpha)) if drop else alpha
         out = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
         Z_halo = torch.empty((lp.h, f), dtype=torch.float32, device=dev) if lp.k > 1 and lp.h > 0 else None
-        _call(A, dev, "pgcn_forward_heads", K, alpha.data_ptr(), Z_own.data_ptr(), out.data_ptr(), _ptr(Z_halo), f,
+        _call(A, dev, "pgcn_forward_heads", K, alpha_d.data_ptr(), Z_own.data_ptr(), out.data_ptr(), _ptr(Z_halo), f,
               exchange=False)
-        ctx.plan, ctx.slope, ctx.heads = A, slope, K
-        ctx.save_for_backward(alpha, Z_own, Z_halo, el_own, er_own, er_halo)
+        ctx.plan, ctx.slope, ctx.heads, ctx.drop = A, slope, K, drop
+        ctx.save_for_backward(alpha, Z_own, Z_halo, el_own, er_own, er_halo, alpha_d if drop else None, snap)
         return _to_layout(A, out)
 
     @staticmethod
     def backward(ctx, grad_output):
-        A, slope, K = ctx.plan, ctx.slope, ctx.heads
-        alpha, Z_own, Z_halo, el_own, er_own, er_halo = ctx.saved_tensors
+        A, slope, K, drop = ctx.plan, ctx.slope, ctx.heads, ctx.drop
+        alpha, Z_own, Z_halo, el_own, er_own, er_halo, alpha_d, snap = ctx.saved_tensors
         g = _own(A, grad_output, "grad_output")
         lp, f, dev = A.lp, g.shape[1], g.device
         dZ = d_el = d_er = None
         if ctx.needs_input_grad[1]:
             G = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
-            _call(A, dev, "pgcn_backward_heads", K, alpha.data_ptr(), g.data_ptr(), G.data_ptr(), f, exchange=True)
+            _call(A, dev, "pgcn_backward_heads", K, (alpha_d if drop else alpha).data_ptr(), g.data_ptr(), G.data_ptr(),
+                  f, exchange=True)
             dZ = _to_layout(A, G)
         if ctx.needs_input_grad[2] or ctx.needs_input_grad[3]:
             dalpha = torch.empty_like(alpha)
             _call(A, dev, "pgcn_sddmm_heads", K, g.data_ptr(), Z_own.data_ptr(), _ptr(Z_halo), dalpha.data_ptr(), f)
+            if drop:
+                _mask(A.edge_pairs(), snap, drop, dalpha, dalpha)
             dpre = torch.empty_like(alpha)
             gel = torch.empty((lp.m, K), dtype=torch.float32, device=dev)
             _call(A, dev, "pgcn_edge_softmax_backward_heads", K, el_own.data_ptr(), er_own.data_ptr(), er_halo.data_ptr(),
@@ -359,7 +480,7 @@ class PGATMultiHeadAttention(torch.autograd.Function):
                 _call(A, dev, "pgcn_backward_heads", K, dpre.data_ptr(), ones.data_ptr(), D.data_ptr(), 4 * K,
                       exchange=True)
                 d_er = _to_layout(A, D[:, 0::4].contiguous())
-        return None, dZ, d_el, d_er, None
+        return None, dZ, d_el, d_er, None, None
 
 
 class PGATv2Attention(torch.autograd.Function):

@@ -20,6 +20,12 @@ layer stays f -> f. K = 1 is the single-head layer above, with the same paramete
 and a (2d x K) attention matrix, both xavier_normal with the relu gain in that order; el[:, h] = Z_h a[:d, h] and
 er[:, h] = Z_h a[d:, h] for head h's slice Z_h of Z (op.PGATMultiHeadAttention).
 
+--attn-dropout P (0 <= P < 1, default 0): attention dropout with probability P between the softmax and the aggregation
+of every layer while training (op.EdgeDropout, the GAT paper's recipe uses 0.6). The mask is a function of the global
+edge, so any partition trains the same model. Layer l draws with key seed * 2^16 + l (seed 0 when --seed is absent) and
+call counter epoch + 1; nothing is drawn from torch's generator, so the parameters are those of a run without the flag.
+Not taken with --v2.
+
 --v2: GATv2 layers instead (dynamic attention, op.PGATv2Attention), with --heads K as above. Per layer lin_l and lin_r
 (Linear(f, f, bias=False)) and att (K x d), drawn in that order, each xavier_normal with the relu gain; the layer is
 PyG GATv2Conv(share_weights=False, concat=True, bias=False, add_self_loops=False) over the stored pattern.
@@ -29,20 +35,22 @@ import sys
 import torch
 import torch.nn as nn
 
-from .op import HEADS, PGATAttention, PGATMultiHeadAttention, PGATv2Attention
+from .op import HEADS, EdgeDropout, PGATAttention, PGATMultiHeadAttention, PGATv2Attention
 from .pgcn import launch, parse_args, train
 
 
 class PGAT(nn.Module):
-    """GPU/PGAT.py:124-148 with the plan handle in place of the dense matrix and a sparse edge softmax."""
+    """GPU/PGAT.py:124-148 with the plan handle in place of the dense matrix and a sparse edge softmax. attn_dropout (an
+    op.EdgeDropout or None) drops attention coefficients while the module is training; eval mode runs without it."""
 
-    def __init__(self, A, in_features, out_features, negative_slope=0.2, heads=1):
+    def __init__(self, A, in_features, out_features, negative_slope=0.2, heads=1, attn_dropout=None):
         super().__init__()
         self.in_features = in_features
         self.out_features = out_features
         self.A = A
         self.negative_slope = negative_slope
         self.heads = heads
+        self.attn_dropout = attn_dropout
         self.linear = nn.Linear(in_features, out_features, bias=False)
         d = out_features // heads
         self.attention = nn.Parameter(torch.empty(size=(2 * out_features, 1) if heads == 1 else (2 * d, heads)))
@@ -56,15 +64,16 @@ class PGAT(nn.Module):
     def forward(self, H):
         Z = self.linear(H)
         f = self.out_features
+        drop = self.attn_dropout if self.training else None
         if self.heads > 1:
             d = f // self.heads
             Zh = Z.view(Z.shape[0], self.heads, d)
             el = torch.einsum("nhd,dh->nh", Zh, self.attention[:d])
             er = torch.einsum("nhd,dh->nh", Zh, self.attention[d:])
-            return PGATMultiHeadAttention.apply(self.A, Z, el, er, self.negative_slope)
+            return PGATMultiHeadAttention.apply(self.A, Z, el, er, self.negative_slope, drop)
         el = torch.matmul(Z, self.attention[:f, :]).squeeze(1)
         er = torch.matmul(Z, self.attention[f:, :]).squeeze(1)
-        return PGATAttention.apply(self.A, Z, el, er, self.negative_slope)
+        return PGATAttention.apply(self.A, Z, el, er, self.negative_slope, drop)
 
 
 class PGATv2(nn.Module):
@@ -89,18 +98,29 @@ class PGATv2(nn.Module):
         return PGATv2Attention.apply(self.A, self.lin_l(H), self.lin_r(H), self.att, self.negative_slope)
 
 
+def dropout_key(seed, layer):
+    """The attention-dropout key of layer `layer` (0-based) under --seed `seed` (None: 0)."""
+    return ((seed or 0) * 2 ** 16 + layer) % 2 ** 64
+
+
 def run(rank, size, nlayers, nfeatures, path_A, path_partvec, backend, transport="auto", out=sys.stdout, seed=None,
-        negative_slope=1.0, epochs=50, heads=1, v2=False):
-    layer = PGATv2 if v2 else PGAT
+        negative_slope=1.0, epochs=50, heads=1, v2=False, attn_dropout=0.0):
     # the multi-head backward gets d_er from an aggregation of width 4 K (PGATMultiHeadAttention)
     f_max = nfeatures if heads == 1 or v2 else max(nfeatures, 4 * heads)
-    return train(rank, size, nlayers, nfeatures, path_A, path_partvec, backend, "PGAT",
-                 lambda plan: layer(plan, nfeatures, nfeatures, negative_slope, heads), f_max, True,
+    if v2:
+        make = lambda plan: PGATv2(plan, nfeatures, nfeatures, negative_slope, heads)
+    else:
+        index = iter(range(nlayers))      # train builds the layers in order
+
+        def make(plan):
+            drop = EdgeDropout(attn_dropout, dropout_key(seed, next(index)), plan.device) if attn_dropout > 0 else None
+            return PGAT(plan, nfeatures, nfeatures, negative_slope, heads, drop)
+    return train(rank, size, nlayers, nfeatures, path_A, path_partvec, backend, "PGAT", make, f_max, True,
                  transport=transport, out=out, seed=seed, epochs=epochs)
 
 
 USAGE = ("usage: PGAT.py -a <A.mtx> -p <partvec> -b nccl -s <nparts> -l <nlayers> -f <nfeatures> "
-         "[--seed N] [--negative-slope S] [--heads 1|2|4|8, dividing nfeatures] [--v2]")
+         "[--seed N] [--negative-slope S] [--heads 1|2|4|8, dividing nfeatures] [--attn-dropout P, 0 <= P < 1] [--v2]")
 
 
 def _heads(arg):
@@ -112,11 +132,14 @@ def _heads(arg):
 
 def _valid(size, nlayers, nfeatures, kw):
     heads = kw.get("heads", 1)
-    return heads in HEADS and nfeatures % heads == 0
+    p = kw.get("attn_dropout", 0.0)
+    return (heads in HEADS and nfeatures % heads == 0 and 0.0 <= p < 1.0
+            and not ("attn_dropout" in kw and kw.get("v2")))
 
 
 def main(argv):
-    options = {"--negative-slope": ("negative_slope", float), "--heads": ("heads", _heads), "--v2": ("v2", None)}
+    options = {"--negative-slope": ("negative_slope", float), "--heads": ("heads", _heads), "--v2": ("v2", None),
+               "--attn-dropout": ("attn_dropout", float)}
     launch(run, *parse_args(argv, USAGE, options, _valid))
 
 

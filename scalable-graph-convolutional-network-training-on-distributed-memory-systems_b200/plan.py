@@ -237,6 +237,7 @@ class PgcnPlan:
         cabi.check(rc, None)
         self._owned_t = None
         self._edge_index = None
+        self._edge_pairs = None
         # edge values (bind_values / set_values): which values the records hold, as far as this process knows
         self._bound = False
         self._resident = "creation"      # "creation", a key of the tensor set last, or None: unknown
@@ -362,6 +363,25 @@ class PgcnPlan:
             self._edge_index = (torch.from_numpy(rows).to(self.device),
                                 torch.from_numpy(lp.colidx.astype(np.int64)).to(self.device))
         return self._edge_index
+
+    def edge_pairs(self):
+        """(global row, global column) of every forward entry, a CUDA int32 [nnz, 2] tensor in lp.colidx's order (the
+        order of edge_index() and of the values set_values takes). Edge dropout (op.EdgeDropout) draws its mask from
+        these pairs, so that every partition of the graph draws the same mask. Built on first use by a host-to-device
+        copy, which a CUDA graph cannot capture: call it once before capturing a step that uses it."""
+        import torch
+        if self._edge_pairs is None:
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError("PgcnPlan.edge_pairs is built by a host-to-device copy, which a CUDA-graph capture "
+                                   "cannot hold: call plan.edge_pairs() once before the capture")
+            lp = self.lp
+            if lp.n > np.iinfo(np.int32).max:
+                raise ValueError("n=%d: edge_pairs holds global ids as int32" % lp.n)
+            rows = np.repeat(lp.owned, np.diff(lp.rowptr.astype(np.int64)))
+            cols = np.concatenate([lp.owned, lp.halo])[lp.colidx]
+            pairs = np.stack([rows, cols], 1).astype(np.int32)
+            self._edge_pairs = torch.from_numpy(pairs).to(self.device)
+        return self._edge_pairs
 
     def algorithmic_bytes(self, f):
         b = cabi.PgcnBytes()
