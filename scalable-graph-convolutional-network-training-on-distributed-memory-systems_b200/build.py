@@ -2,6 +2,7 @@
 
   lib/libpgcn_b200.so     csrc/pgcn_b200.cu (+ spmm_kernels.cuh, spmm_ring.cuh, sddmm.cuh, attention.cuh, spmm_max.cuh, gatv2.cuh)   nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo
   lib/libpgcn_dropout.so  csrc/edge_dropout.cu (+ philox.cuh)                                                                        the same flags
+  lib/libpgcn_gated.so    csrc/gated.cu                                                                                              the same flags
   (the CPU oracle under oracle/ is built by oracle/build_oracle.py — test infrastructure only)
 
 nvcc cross-compiles without a GPU; `python -m <pkg>.build` or `__graft_entry__.build()` runs this.
@@ -24,12 +25,17 @@ SOURCES = [os.path.join(CSRC, "pgcn_b200.cu")]
 DEPS = SOURCES + [os.path.join(CSRC, "spmm_kernels.cuh"), os.path.join(CSRC, "spmm_ring.cuh"),
                   os.path.join(CSRC, "sddmm.cuh"), os.path.join(CSRC, "attention.cuh"), os.path.join(CSRC, "spmm_max.cuh"),
                   os.path.join(CSRC, "gatv2.cuh"),
-                  os.path.join(ROOT, "include", "pgcn_b200.h"), os.path.abspath(__file__)]
+                  os.path.join(ROOT, "include", "pgcn_b200.h"), os.path.join(ROOT, "include", "pgcn_b200_halo.h"),
+                  os.path.abspath(__file__)]
 # the edge-dropout library has its own sources and dependency list: editing one library never rebuilds the other
 DROPOUT_LIB = os.path.join(LIBDIR, "libpgcn_dropout.so")
 DROPOUT_SOURCES = [os.path.join(CSRC, "edge_dropout.cu")]
 DROPOUT_DEPS = DROPOUT_SOURCES + [os.path.join(CSRC, "philox.cuh"), os.path.join(ROOT, "include", "pgcn_dropout.h"),
                                   os.path.abspath(__file__)]
+# so has the gated-aggregation library
+GATED_LIB = os.path.join(LIBDIR, "libpgcn_gated.so")
+GATED_SOURCES = [os.path.join(CSRC, "gated.cu")]
+GATED_DEPS = GATED_SOURCES + [os.path.join(ROOT, "include", "pgcn_gated.h"), os.path.abspath(__file__)]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -58,6 +64,10 @@ def is_stale():
 
 def dropout_is_stale():
     return _stale(DROPOUT_LIB, DROPOUT_DEPS)
+
+
+def gated_is_stale():
+    return _stale(GATED_LIB, GATED_DEPS)
 
 
 def _compile(lib, sources, defs, verbose):
@@ -90,7 +100,15 @@ def build_dropout(force=False, verbose=False):
     return _compile(DROPOUT_LIB, DROPOUT_SOURCES, [], verbose)
 
 
+def build_gated(force=False, verbose=False):
+    """Compile libpgcn_gated.so for sm_90a if missing or older than its sources. Returns its path."""
+    if not force and not gated_is_stale():
+        return GATED_LIB
+    return _compile(GATED_LIB, GATED_SOURCES, [], verbose)
+
+
 if __name__ == "__main__":
     force, verbose = "--force" in sys.argv, "-v" in sys.argv
     print(build(force=force, verbose=verbose))
     print(build_dropout(force=force, verbose=verbose))
+    print(build_gated(force=force, verbose=verbose))

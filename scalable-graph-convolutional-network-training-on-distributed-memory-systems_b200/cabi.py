@@ -1,7 +1,8 @@
-"""ctypes binding of include/pgcn_b200.h — the C-ABI drop-in boundary (SURVEY.md §8b) — and of include/pgcn_dropout.h.
+"""ctypes binding of include/pgcn_b200.h — the C-ABI drop-in boundary (SURVEY.md §8b) — and of include/pgcn_b200_halo.h,
+include/pgcn_dropout.h and include/pgcn_gated.h.
 
-Nothing here computes: it loads lib/libpgcn_b200.so (load) and lib/libpgcn_dropout.so (load_dropout), declares every
-exported symbol and turns negative status codes into RuntimeError. If the library is missing there is no fallback: the
+Nothing here computes: it loads lib/libpgcn_b200.so (load), lib/libpgcn_dropout.so (load_dropout) and
+lib/libpgcn_gated.so (load_gated), declares every exported symbol and turns negative status codes into RuntimeError. If the library is missing there is no fallback: the
 product path fails loudly (the CPU oracle under oracle/ is test infrastructure only).
 """
 import ctypes as C
@@ -26,8 +27,15 @@ SYMBOLS = [
     "pgcn_sddmm_heads", "pgcn_forward_max", "pgcn_backward_max", "pgcn_forward_gatv2", "pgcn_backward_gatv2",
 ]
 
+# every symbol declared in include/pgcn_b200_halo.h (exported by libpgcn_b200.so as well)
+HALO_SYMBOLS = ["pgcn_halo_rows_add"]
+
 # every symbol declared in include/pgcn_dropout.h
 DROPOUT_SYMBOLS = ["pgcn_dropout_version", "pgcn_dropout_last_error", "pgcn_edge_dropout"]
+
+# every symbol declared in include/pgcn_gated.h
+GATED_SYMBOLS = ["pgcn_gated_version", "pgcn_gated_last_error", "pgcn_gated_chunk", "pgcn_gated_forward",
+                 "pgcn_gated_backward_rows", "pgcn_gated_backward_cols"]
 
 
 class PgcnBytes(C.Structure):
@@ -38,8 +46,15 @@ class PgcnBytes(C.Structure):
         return {n: int(getattr(self, n)) for n, _ in self._fields_}
 
 
+class PgcnGatedWalk(C.Structure):
+    """pgcn_gated_walk: a CSR's entries and its work table, device pointers."""
+    _fields_ = [("idx", C.c_void_p), ("items", C.c_void_p), ("splits", C.c_void_p), ("rows", C.c_int32),
+                ("nitems", C.c_int32), ("nsplits", C.c_int32), ("nslots", C.c_int32)]
+
+
 _lib = None
 _dropout = None
+_gated = None
 
 
 def lib_path():
@@ -48,6 +63,10 @@ def lib_path():
 
 def dropout_lib_path():
     return _build.DROPOUT_LIB
+
+
+def gated_lib_path():
+    return _build.GATED_LIB
 
 
 def _built(path, stale, build, build_if_missing):
@@ -158,6 +177,8 @@ def load(build_if_missing=True):
     lib.pgcn_forward_gatv2.argtypes = [vp, i32, vp, vp, vp, C.c_float, vp, vp, vp, i32, vp]
     lib.pgcn_backward_gatv2.restype = C.c_int
     lib.pgcn_backward_gatv2.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, C.c_float, vp, vp, vp, vp, i32, vp]
+    lib.pgcn_halo_rows_add.restype = C.c_int
+    lib.pgcn_halo_rows_add.argtypes = [vp, vp, vp, i32, vp]
     _lib = lib
     return lib
 
@@ -192,4 +213,35 @@ def check_dropout(rc):
     if rc < 0:
         msg = load_dropout().pgcn_dropout_last_error()
         raise RuntimeError("pgcn_dropout error %d: %s" % (rc, (msg or b"").decode("utf-8", "replace")))
+    return rc
+
+
+def load_gated(build_if_missing=True):
+    """Load libpgcn_gated.so (building it first when stale and nvcc is available)."""
+    global _gated
+    if _gated is not None:
+        return _gated
+    lib = C.CDLL(_built(_build.GATED_LIB, _build.gated_is_stale, _build.build_gated, build_if_missing))
+    vp, i32, walk = C.c_void_p, C.c_int32, C.POINTER(PgcnGatedWalk)
+    lib.pgcn_gated_version.restype = C.c_char_p
+    lib.pgcn_gated_version.argtypes = []
+    lib.pgcn_gated_last_error.restype = C.c_char_p
+    lib.pgcn_gated_last_error.argtypes = []
+    lib.pgcn_gated_chunk.restype = i32
+    lib.pgcn_gated_chunk.argtypes = []
+    lib.pgcn_gated_forward.restype = C.c_int
+    lib.pgcn_gated_forward.argtypes = [walk, i32, i32, vp, vp, vp, vp, vp, i32, vp]
+    lib.pgcn_gated_backward_rows.restype = C.c_int
+    lib.pgcn_gated_backward_rows.argtypes = [walk, i32, i32, vp, vp, vp, vp, vp, vp, i32, vp]
+    lib.pgcn_gated_backward_cols.restype = C.c_int
+    lib.pgcn_gated_backward_cols.argtypes = [walk, i32, i32, vp, vp, vp, vp, vp, vp, i32, vp]
+    _gated = lib
+    return lib
+
+
+def check_gated(rc):
+    """Raise RuntimeError carrying pgcn_gated_last_error when a libpgcn_gated call returned a negative status."""
+    if rc < 0:
+        msg = load_gated().pgcn_gated_last_error()
+        raise RuntimeError("pgcn_gated error %d: %s" % (rc, (msg or b"").decode("utf-8", "replace")))
     return rc

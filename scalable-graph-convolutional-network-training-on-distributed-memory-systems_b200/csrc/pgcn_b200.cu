@@ -6,6 +6,7 @@
 // exchange (NCCL grouped send/recv resolved at run time from the process's libnccl, and the
 // peer-memory path that stores rows directly into the neighbour GPU's slab over NVLink).
 #include "../../include/pgcn_b200.h"
+#include "../../include/pgcn_b200_halo.h"
 #include "spmm_kernels.cuh"
 #include "spmm_ring.cuh"
 #include "sddmm.cuh"
@@ -2427,6 +2428,23 @@ int pgcn_halo_rows(pgcn_plan* p, const float* X_own, float* X_halo_out, int32_t 
     cudaStream_t st = (cudaStream_t)stream;
     return unsplit_forward(p, X_own, w, st, [&](float* halo, const float* halo_odd) {
         return copy_halo(p, halo, halo_odd, X_halo_out, w, st);
+    });
+}
+
+// The reverse of pgcn_halo_rows: the unsplit backward exchange with X_halo copied into the reverse send slab.
+int pgcn_halo_rows_add(pgcn_plan* p, const float* X_halo, float* G_own, int32_t w, void* stream)
+{
+    int rc = check_f(p, w);
+    if (rc) return rc;
+    if (!p->bound) return fail(p, PGCN_ERR_STATE, "pgcn_halo_rows_add: call pgcn_plan_bind_values first");
+    if (p->k == 1) return 0;
+    if (p->m > 0 && !G_own) return fail(p, PGCN_ERR_INVALID, "null G_own");
+    if (p->h > 0 && !X_halo) return fail(p, PGCN_ERR_INVALID, "h=%d but X_halo is null", p->h);
+    cudaStream_t st = (cudaStream_t)stream;
+    return unsplit_backward(p, G_own, w, st, [&]() -> int {
+        if (p->h > 0)
+            CU(p, cudaMemcpyAsync(p->d_hsend_slab, X_halo, (size_t)p->h * w * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        return 0;
     });
 }
 

@@ -17,6 +17,8 @@ All arithmetic happens in libpgcn_b200.so on the current CUDA stream; there is n
 Every operator takes its inputs through _own / _own_scores, returns its outputs through _to_layout and makes each C
 call through _call, so an operator is its validation and its sequence of C calls.
 """
+import ctypes as C
+
 import torch
 
 from . import cabi
@@ -593,6 +595,107 @@ class PSpMMMax(torch.autograd.Function):
         A = ctx.plan
         (arg,) = ctx.saved_tensors
         return None, _to_layout(A, aggregate_max_backward(A, arg, _own(A, grad_output, "grad_output")))
+
+
+# ---- gated aggregation (libpgcn_gated.so) ----------------------------------------------------------------------------
+
+def _gated(dev, name, *args):
+    """libpgcn_gated.<name>(*args, stream) on `dev`'s current stream, its status checked."""
+    with torch.cuda.device(dev):
+        cabi.check_gated(getattr(cabi.load_gated(), name)(*args, _stream_ptr()))
+
+
+def _gated_operands(plan, K_own, Q_own, V_own, what):
+    """The walks, then K_own, Q_own, V_own checked ([m, f] each, 2f <= f_max, a bound plan). The walks come first, so
+    that a capture that needs them before they exist is refused before any work is enqueued."""
+    walks = plan.gated_walks()
+    f = K_own.shape[-1]
+    if 2 * f > plan.f_max:
+        raise ValueError("f=%d: %s exchanges [Q | V] rows of 2f = %d floats, the plan's f_max is %d: build the plan "
+                         "with f_max >= 2f" % (f, what, 2 * f, plan.f_max))
+    K_own = _check_feat(plan, K_own, plan.m, "K")
+    Q_own = _check_feat(plan, Q_own, plan.m, "Q")
+    V_own = _check_feat(plan, V_own, plan.m, "V")
+    if Q_own.shape[1] != f or V_own.shape[1] != f:
+        raise ValueError("K, Q and V must have the same width, got %d, %d and %d" % (f, Q_own.shape[1], V_own.shape[1]))
+    _require_bound(plan, "%s exchanges [Q | V] through pgcn_halo_rows" % what)
+    return walks, K_own, Q_own, V_own
+
+
+def aggregate_gated(plan, K_own, Q_own, V_own):
+    """(Z_own, QV_own, QV_halo): Z_own[i] = sum over row i's stored entries (i, j) of sigmoid(K[i] + Q[j]) * V[j],
+    element-wise, over [own | halo] columns (pgcn_gated_forward); K_own, Q_own, V_own, Z_own are [m, f]. QV_own is the
+    [m, 2f] concatenation [Q | V] and QV_halo [h, 2f] its halo rows from one exchange (pgcn_halo_rows), which
+    aggregate_gated_backward takes. Needs a bound plan with f_max >= 2f."""
+    (fwd, _), K_own, Q_own, V_own = _gated_operands(plan, K_own, Q_own, V_own, "aggregate_gated")
+    lp, f, dev = plan.lp, K_own.shape[1], K_own.device
+    QV = torch.cat([Q_own, V_own], 1)
+    QV_halo = torch.empty((lp.h, 2 * f), dtype=torch.float32, device=dev)
+    _call(plan, dev, "pgcn_halo_rows", QV.data_ptr(), QV_halo.data_ptr(), 2 * f, exchange=False)
+    Z = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+    work = torch.empty((fwd.nslots, f), dtype=torch.float32, device=dev)
+    _gated(dev, "pgcn_gated_forward", C.byref(fwd.c), lp.m, lp.h, K_own.data_ptr(), QV.data_ptr(), QV_halo.data_ptr(),
+           Z.data_ptr(), work.data_ptr(), f)
+    return Z, QV, QV_halo
+
+
+def aggregate_gated_backward(plan, K_own, QV_own, QV_halo, gZ_own):
+    """(dK, dQ, dV), each [m, f]: the gradients of aggregate_gated's Z_own for the output gradient gZ_own [m, f], from
+    its QV_own and QV_halo. dK comes from the row walk (pgcn_gated_backward_rows); dQ and dV from the column walk over
+    the transposed entries (pgcn_gated_backward_cols), whose halo rows go back to their owners and are added there
+    (pgcn_halo_rows_add)."""
+    f = K_own.shape[-1]
+    if QV_own.dim() != 2 or QV_own.shape[1] != 2 * f:
+        raise ValueError("QV_own must be [%d, %d], got %s" % (plan.m, 2 * f, tuple(QV_own.shape)))
+    (fwd, tr), K_own, gZ_own, _ = _gated_operands(plan, K_own, gZ_own, gZ_own, "aggregate_gated_backward")
+    lp, dev = plan.lp, K_own.device
+    QV_own = QV_own.contiguous()
+    if QV_own.shape[0] != lp.m or tuple(QV_halo.shape) != (lp.h, 2 * f):
+        raise ValueError("QV_own / QV_halo must be [%d, %d] / [%d, %d], got %s / %s" % (
+            lp.m, 2 * f, lp.h, 2 * f, tuple(QV_own.shape), tuple(QV_halo.shape)))
+    QV_halo = QV_halo.contiguous()
+    dK = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+    work = torch.empty((fwd.nslots, f), dtype=torch.float32, device=dev)
+    _gated(dev, "pgcn_gated_backward_rows", C.byref(fwd.c), lp.m, lp.h, K_own.data_ptr(), QV_own.data_ptr(),
+           QV_halo.data_ptr(), gZ_own.data_ptr(), dK.data_ptr(), work.data_ptr(), f)
+    dQV = torch.empty((lp.m + lp.h, 2 * f), dtype=torch.float32, device=dev)
+    work = torch.empty((tr.nslots, 2 * f), dtype=torch.float32, device=dev)
+    _gated(dev, "pgcn_gated_backward_cols", C.byref(tr.c), lp.m, lp.h, K_own.data_ptr(), QV_own.data_ptr(),
+           QV_halo.data_ptr(), gZ_own.data_ptr(), dQV.data_ptr(), work.data_ptr(), f)
+    _call(plan, dev, "pgcn_halo_rows_add", dQV[lp.m:].data_ptr(), dQV.data_ptr(), 2 * f, exchange=True)
+    return dK, dQV[:lp.m, :f], dQV[:lp.m, f:]
+
+
+class PSpMMGated(torch.autograd.Function):
+    """Sigmoid-gated aggregation over the plan's stored pattern, the message of PyG's ResGatedGraphConv (GatedGCN's
+    without the edge features and the normalisation):
+
+        PSpMMGated.apply(A, K, Q, V)
+        out[i] = sum over the stored entries (i, j) of  sigmoid(K[i] + Q[j]) * V[j]        (element-wise, f features)
+
+    K, Q and V are [rows, f] fp32 CUDA tensors, out is [rows, f] (rows = m in the "local" layout, n in the "global"
+    one, as PSpMM). The values of A are not read; every stored entry contributes, duplicates included. One exchange
+    per layer carries [Q | V] (2f floats per row), so the plan's f_max must be at least 2f; the backward returns the
+    halo rows' partial dQ and dV to their owners in one reverse exchange. Nothing is stored per entry: the backward
+    recomputes the gates from K, Q and V. Gradients go to K, Q and V. Deterministic. The exchange is the unsplit one
+    (no per-source overlap). The plan must be bound (PgcnPlan.bind_values); the first call builds its index tables
+    (PgcnPlan.gated_walks)."""
+
+    @staticmethod
+    def forward(ctx, A, K, Q, V):
+        A.gated_walks()
+        K_own = _own(A, K, "K")
+        Z, QV, QV_halo = aggregate_gated(A, K_own, _own(A, Q, "Q"), _own(A, V, "V"))
+        ctx.plan = A
+        ctx.save_for_backward(K_own, QV, QV_halo)
+        return _to_layout(A, Z)
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        A = ctx.plan
+        K_own, QV, QV_halo = ctx.saved_tensors
+        dK, dQ, dV = aggregate_gated_backward(A, K_own, QV, QV_halo, _own(A, grad_output, "grad_output"))
+        return None, _to_layout(A, dK), _to_layout(A, dQ), _to_layout(A, dV)
 
 
 # ---- the pieces, individually callable (NCCL transport), mirroring communicate_fgm ----------------

@@ -238,6 +238,7 @@ class PgcnPlan:
         self._owned_t = None
         self._edge_index = None
         self._edge_pairs = None
+        self._gated_walks = None
         # edge values (bind_values / set_values): which values the records hold, as far as this process knows
         self._bound = False
         self._resident = "creation"      # "creation", a key of the tensor set last, or None: unknown
@@ -383,6 +384,22 @@ class PgcnPlan:
             self._edge_pairs = torch.from_numpy(pairs).to(self.device)
         return self._edge_pairs
 
+    def gated_walks(self):
+        """(fwd, tr): the GatedWalk of the local forward CSR and of its transpose, the device index arrays and work tables
+        of the gated aggregation (op.PSpMMGated, include/pgcn_gated.h). About 8 B per entry (both index arrays) and 16 B
+        per row and per column (the work items), about 170 MB on C2. Built on first use by host-to-device copies, which a
+        CUDA graph cannot capture: call it, or the operator once eagerly, before capturing a step that uses it."""
+        import torch
+        if self._gated_walks is None:
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError("PgcnPlan.gated_walks is built by host-to-device copies, which a CUDA-graph capture "
+                                   "cannot hold: call plan.gated_walks() once before the capture")
+            chunk = cabi.load_gated().pgcn_gated_chunk()
+            lp = self.lp
+            self._gated_walks = (GatedWalk(lp.rowptr, lp.colidx, chunk, self.device),
+                                 GatedWalk(lp.t_rowptr, lp.t_colidx, chunk, self.device))
+        return self._gated_walks
+
     def algorithmic_bytes(self, f):
         b = cabi.PgcnBytes()
         cabi.check(self._lib.pgcn_algorithmic_bytes(self.handle, int(f), C.byref(b)), self._h)
@@ -461,6 +478,45 @@ class PgcnPlan:
         self.stats["recv_volume"] += int(in_rows)
         self.stats["send_nmsg"] += lp.k - 1
         self.stats["recv_nmsg"] += lp.k - 1
+
+
+def gated_work_table(rowptr, chunk):
+    """(items, splits, nslots) of a CSR's row pointer for the gated kernels: items int32 [nitems, 4] of (row, e0, e1,
+    slot), first one per chunk of `chunk` entries of every row longer than `chunk` (slots 0, 1, ... in row and chunk
+    order), then one per other row, empty rows included (slot -1); splits int32 [nsplits, 3] of (row, first slot,
+    chunks) per split row. The split rows' chunks come first so that the longest work starts first."""
+    rowptr = np.asarray(rowptr, dtype=np.int64)
+    deg = np.diff(rowptr)
+    long_rows = np.flatnonzero(deg > chunk)
+    nch = -(-deg[long_rows] // chunk)
+    first = np.cumsum(nch) - nch
+    nslots = int(nch.sum())
+    crow = np.repeat(long_rows, nch)
+    slot = np.arange(nslots, dtype=np.int64)
+    e0 = rowptr[crow] + (slot - np.repeat(first, nch)) * chunk
+    e1 = np.minimum(e0 + chunk, rowptr[crow + 1])
+    short = np.flatnonzero(deg <= chunk)
+    items = np.concatenate([np.stack([crow, e0, e1, slot], 1),
+                            np.stack([short, rowptr[short], rowptr[short + 1], np.full(len(short), -1)], 1)])
+    splits = np.stack([long_rows, first, nch], 1)
+    if rowptr[-1] > np.iinfo(np.int32).max:
+        raise ValueError("nnz=%d: the gated work table holds entry offsets as int32" % rowptr[-1])
+    return items.astype(np.int32).reshape(-1, 4), splits.astype(np.int32).reshape(-1, 3), nslots
+
+
+class GatedWalk:
+    """One walk of the gated kernels on the device: a CSR's entries `idx` and its work table (gated_work_table), with
+    `c`, the pgcn_gated_walk that points at them. `nslots` rows of work memory take the split rows' partial sums."""
+
+    def __init__(self, rowptr, idx, chunk, device):
+        import torch
+        items, splits, self.nslots = gated_work_table(rowptr, chunk)
+        self.rows = len(rowptr) - 1
+        self.idx = torch.from_numpy(np.ascontiguousarray(idx, dtype=np.int32)).to(device)
+        self.items = torch.from_numpy(items).to(device)
+        self.splits = torch.from_numpy(splits).to(device)
+        self.c = cabi.PgcnGatedWalk(self.idx.data_ptr(), self.items.data_ptr(), self.splits.data_ptr(), self.rows,
+                                    len(items), len(splits), self.nslots)
 
 
 def _values_key(vals):
