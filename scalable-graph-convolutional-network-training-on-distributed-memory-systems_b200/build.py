@@ -3,6 +3,7 @@
   lib/libpgcn_b200.so     csrc/pgcn_b200.cu (+ spmm_kernels.cuh, spmm_ring.cuh, sddmm.cuh, attention.cuh, spmm_max.cuh, gatv2.cuh)   nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo
   lib/libpgcn_dropout.so  csrc/edge_dropout.cu (+ philox.cuh)                                                                        the same flags
   lib/libpgcn_gated.so    csrc/gated.cu                                                                                              the same flags
+  lib/libpgcn_transformer.so csrc/transformer.cu (+ philox.cuh, pgcn_gated.h for the walk struct)                                     the same flags
   (the CPU oracle under oracle/ is built by oracle/build_oracle.py — test infrastructure only)
 
 nvcc cross-compiles without a GPU; `python -m <pkg>.build` or `__graft_entry__.build()` runs this.
@@ -36,6 +37,12 @@ DROPOUT_DEPS = DROPOUT_SOURCES + [os.path.join(CSRC, "philox.cuh"), os.path.join
 GATED_LIB = os.path.join(LIBDIR, "libpgcn_gated.so")
 GATED_SOURCES = [os.path.join(CSRC, "gated.cu")]
 GATED_DEPS = GATED_SOURCES + [os.path.join(ROOT, "include", "pgcn_gated.h"), os.path.abspath(__file__)]
+# and the transformer-attention library, which takes the gated library's walk struct and the dropout's Philox
+TRANSFORMER_LIB = os.path.join(LIBDIR, "libpgcn_transformer.so")
+TRANSFORMER_SOURCES = [os.path.join(CSRC, "transformer.cu")]
+TRANSFORMER_DEPS = TRANSFORMER_SOURCES + [os.path.join(CSRC, "philox.cuh"),
+                                          os.path.join(ROOT, "include", "pgcn_transformer.h"),
+                                          os.path.join(ROOT, "include", "pgcn_gated.h"), os.path.abspath(__file__)]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -68,6 +75,10 @@ def dropout_is_stale():
 
 def gated_is_stale():
     return _stale(GATED_LIB, GATED_DEPS)
+
+
+def transformer_is_stale():
+    return _stale(TRANSFORMER_LIB, TRANSFORMER_DEPS)
 
 
 def _compile(lib, sources, defs, verbose):
@@ -107,8 +118,16 @@ def build_gated(force=False, verbose=False):
     return _compile(GATED_LIB, GATED_SOURCES, [], verbose)
 
 
+def build_transformer(force=False, verbose=False):
+    """Compile libpgcn_transformer.so for sm_90a if missing or older than its sources. Returns its path."""
+    if not force and not transformer_is_stale():
+        return TRANSFORMER_LIB
+    return _compile(TRANSFORMER_LIB, TRANSFORMER_SOURCES, [], verbose)
+
+
 if __name__ == "__main__":
     force, verbose = "--force" in sys.argv, "-v" in sys.argv
     print(build(force=force, verbose=verbose))
     print(build_dropout(force=force, verbose=verbose))
     print(build_gated(force=force, verbose=verbose))
+    print(build_transformer(force=force, verbose=verbose))

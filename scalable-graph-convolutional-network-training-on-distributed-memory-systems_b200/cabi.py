@@ -1,8 +1,8 @@
 """ctypes binding of include/pgcn_b200.h — the C-ABI drop-in boundary (SURVEY.md §8b) — and of include/pgcn_b200_halo.h,
-include/pgcn_dropout.h and include/pgcn_gated.h.
+include/pgcn_dropout.h, include/pgcn_gated.h and include/pgcn_transformer.h.
 
 Nothing here computes: it loads lib/libpgcn_b200.so (load), lib/libpgcn_dropout.so (load_dropout) and
-lib/libpgcn_gated.so (load_gated), declares every exported symbol and turns negative status codes into RuntimeError. If the library is missing there is no fallback: the
+lib/libpgcn_gated.so (load_gated) and lib/libpgcn_transformer.so (load_transformer), declares every exported symbol and turns negative status codes into RuntimeError. If the library is missing there is no fallback: the
 product path fails loudly (the CPU oracle under oracle/ is test infrastructure only).
 """
 import ctypes as C
@@ -37,6 +37,10 @@ DROPOUT_SYMBOLS = ["pgcn_dropout_version", "pgcn_dropout_last_error", "pgcn_edge
 GATED_SYMBOLS = ["pgcn_gated_version", "pgcn_gated_last_error", "pgcn_gated_chunk", "pgcn_gated_forward",
                  "pgcn_gated_backward_rows", "pgcn_gated_backward_cols"]
 
+# every symbol declared in include/pgcn_transformer.h
+TRANSFORMER_SYMBOLS = ["pgcn_transformer_version", "pgcn_transformer_last_error", "pgcn_transformer_forward",
+                       "pgcn_transformer_backward_rows", "pgcn_transformer_backward_cols"]
+
 
 class PgcnBytes(C.Structure):
     _fields_ = [(n, C.c_int64) for n in (
@@ -55,6 +59,7 @@ class PgcnGatedWalk(C.Structure):
 _lib = None
 _dropout = None
 _gated = None
+_transformer = None
 
 
 def lib_path():
@@ -67,6 +72,10 @@ def dropout_lib_path():
 
 def gated_lib_path():
     return _build.GATED_LIB
+
+
+def transformer_lib_path():
+    return _build.TRANSFORMER_LIB
 
 
 def _built(path, stale, build, build_if_missing):
@@ -244,4 +253,37 @@ def check_gated(rc):
     if rc < 0:
         msg = load_gated().pgcn_gated_last_error()
         raise RuntimeError("pgcn_gated error %d: %s" % (rc, (msg or b"").decode("utf-8", "replace")))
+    return rc
+
+
+def load_transformer(build_if_missing=True):
+    """Load libpgcn_transformer.so (building it first when stale and nvcc is available)."""
+    global _transformer
+    if _transformer is not None:
+        return _transformer
+    lib = C.CDLL(_built(_build.TRANSFORMER_LIB, _build.transformer_is_stale, _build.build_transformer,
+                        build_if_missing))
+    vp, i32, u32, f32, walk = C.c_void_p, C.c_int32, C.c_uint32, C.c_float, C.POINTER(PgcnGatedWalk)
+    lib.pgcn_transformer_version.restype = C.c_char_p
+    lib.pgcn_transformer_version.argtypes = []
+    lib.pgcn_transformer_last_error.restype = C.c_char_p
+    lib.pgcn_transformer_last_error.argtypes = []
+    # (walk, m, h, heads, Q_own, KV_own, KV_halo, scale, gid, drop, threshold, keep_scale, ...)
+    head = [walk, i32, i32, i32, vp, vp, vp, f32, vp, vp, u32, f32]
+    lib.pgcn_transformer_forward.restype = C.c_int
+    lib.pgcn_transformer_forward.argtypes = head + [vp, vp, vp, i32, vp]
+    lib.pgcn_transformer_backward_rows.restype = C.c_int
+    lib.pgcn_transformer_backward_rows.argtypes = head + [vp, vp, vp, vp, vp, vp, i32, vp]
+    lib.pgcn_transformer_backward_cols.restype = C.c_int
+    lib.pgcn_transformer_backward_cols.argtypes = head + [vp, vp, vp, vp, vp, i32, vp]
+    _transformer = lib
+    return lib
+
+
+def check_transformer(rc):
+    """Raise RuntimeError carrying pgcn_transformer_last_error when a libpgcn_transformer call returned a negative
+    status."""
+    if rc < 0:
+        msg = load_transformer().pgcn_transformer_last_error()
+        raise RuntimeError("pgcn_transformer error %d: %s" % (rc, (msg or b"").decode("utf-8", "replace")))
     return rc

@@ -698,6 +698,162 @@ class PSpMMGated(torch.autograd.Function):
         return None, _to_layout(A, dK), _to_layout(A, dQ), _to_layout(A, dV)
 
 
+# ---- graph transformer attention (libpgcn_transformer.so) -----------------------------------------------------------
+
+TRANSFORMER_MAX_F = 256
+
+
+def transformer_scale(f, heads):
+    """The default score scale, float32(1 / sqrt(f / heads)): 1 / sqrt of the head width."""
+    import math
+    import numpy as np
+    return float(np.float32(1.0 / math.sqrt(f / heads)))
+
+
+def _transformer(dev, name, *args):
+    """libpgcn_transformer.<name>(*args, stream) on `dev`'s current stream, its status checked."""
+    with torch.cuda.device(dev):
+        cabi.check_transformer(getattr(cabi.load_transformer(), name)(*args, _stream_ptr()))
+
+
+def _transformer_operands(plan, Q_own, K_own, V_own, heads, drop, what):
+    """The walks and the global ids, then heads, width and Q_own, K_own, V_own checked ([m, f] each, f <= 256 and
+    2f <= f_max, a bound plan). The walks and ids come first, so that a capture that needs them before they exist is
+    refused before any work is enqueued."""
+    walks = plan.gated_walks()
+    gid = plan.global_ids()
+    if drop is not None and drop.state.device != plan.device:
+        raise ValueError("the EdgeDropout state lives on %s, the plan on %s" % (drop.state.device, plan.device))
+    f = Q_own.shape[-1]
+    if heads not in HEADS:
+        raise ValueError("heads=%r: the transformer kernels take 1, 2, 4 or 8 heads" % (heads,))
+    if f % heads:
+        raise ValueError("f=%d is not a multiple of heads=%d" % (f, heads))
+    if f > TRANSFORMER_MAX_F:
+        raise ValueError("f=%d: the transformer kernels hold a row in registers, f <= %d" % (f, TRANSFORMER_MAX_F))
+    if 2 * f > plan.f_max:
+        raise ValueError("f=%d: %s exchanges [K | V] rows of 2f = %d floats, the plan's f_max is %d: build the plan "
+                         "with f_max >= 2f" % (f, what, 2 * f, plan.f_max))
+    Q_own = _check_feat(plan, Q_own, plan.m, "Q")
+    K_own = _check_feat(plan, K_own, plan.m, "K")
+    V_own = _check_feat(plan, V_own, plan.m, "V")
+    if K_own.shape[1] != f or V_own.shape[1] != f:
+        raise ValueError("Q, K and V must have the same width, got %d, %d and %d" % (f, K_own.shape[1], V_own.shape[1]))
+    _require_bound(plan, "%s exchanges [K | V] through pgcn_halo_rows" % what)
+    return walks, gid, Q_own, K_own, V_own
+
+
+def _drop_args(drop, snap):
+    """(drop, threshold, keep_scale) of the kernels: the snapshot's pointer, or NULL, 0, 1 without dropout."""
+    return (None, 0, 1.0) if drop is None else (snap.data_ptr(), drop.threshold, drop.scale)
+
+
+def aggregate_transformer(plan, Q_own, K_own, V_own, heads, scale=None, drop=None):
+    """(Z_own, L, KV_own, KV_halo, snap): scaled dot-product attention over the plan's stored pattern with `heads` heads
+    of width C = f / heads (pgcn_transformer_forward): s_eh = scale <Q[i, h], K[j, h]>, alpha = softmax of s over each
+    row's stored entries per head, Z_own[i, h] = sum_e alpha_eh M_eh V[j, h]. Q_own, K_own, V_own, Z_own are [m, f],
+    L [m, heads] the rows' log-sum-exp. KV_own is [K | V] ([m, 2f]) and KV_halo [h, 2f] its halo rows from one exchange
+    (pgcn_halo_rows). scale None: float32(1 / sqrt(C)). drop (an EdgeDropout) with p > 0 draws a new counter (its
+    snapshot `snap`, else None) and applies the mask M; aggregate_transformer_backward takes the same snapshot. Needs a
+    bound plan with f_max >= 2f."""
+    drop = _active(drop)
+    (fwd, _), gid, Q_own, K_own, V_own = _transformer_operands(plan, Q_own, K_own, V_own, heads, drop,
+                                                               "aggregate_transformer")
+    lp, f, dev = plan.lp, Q_own.shape[1], Q_own.device
+    scale = transformer_scale(f, heads) if scale is None else float(scale)
+    snap = drop.draw() if drop else None
+    KV = torch.cat([K_own, V_own], 1)
+    KV_halo = torch.empty((lp.h, 2 * f), dtype=torch.float32, device=dev)
+    _call(plan, dev, "pgcn_halo_rows", KV.data_ptr(), KV_halo.data_ptr(), 2 * f, exchange=False)
+    Z = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+    L = torch.empty((lp.m, heads), dtype=torch.float32, device=dev)
+    work = torch.empty((fwd.nslots, f + 2 * heads), dtype=torch.float32, device=dev)
+    _transformer(dev, "pgcn_transformer_forward", C.byref(fwd.c), lp.m, lp.h, heads, Q_own.data_ptr(), KV.data_ptr(),
+                 KV_halo.data_ptr(), scale, gid.data_ptr(), *_drop_args(drop, snap), Z.data_ptr(), L.data_ptr(),
+                 work.data_ptr(), f)
+    return Z, L, KV, KV_halo, snap
+
+
+def aggregate_transformer_backward(plan, Q_own, KV_own, KV_halo, Z_own, L, gZ_own, heads, scale=None, drop=None,
+                                   snap=None):
+    """(dQ, dK, dV), each [m, f]: the gradients of aggregate_transformer's Z_own for the output gradient gZ_own [m, f],
+    from its KV_own, KV_halo, Z_own and L and, with dropout, the same `drop` and its forward's `snap`. dQ and the rows'
+    D = <gZ, Z> come from the row walk (pgcn_transformer_backward_rows); dK and dV from the column walk over the
+    transposed entries (pgcn_transformer_backward_cols), whose halo rows go back to their owners and are added there
+    (pgcn_halo_rows_add)."""
+    drop = _active(drop)
+    f = Q_own.shape[-1]
+    if drop is not None and snap is None:
+        raise ValueError("aggregate_transformer_backward with dropout needs the forward's snapshot")
+    (fwd, tr), gid, Q_own, gZ_own, Z_own = _transformer_operands(plan, Q_own, gZ_own, Z_own, heads, drop,
+                                                                 "aggregate_transformer_backward")
+    lp, dev = plan.lp, Q_own.device
+    KV_own, KV_halo, L = KV_own.contiguous(), KV_halo.contiguous(), L.contiguous()
+    if tuple(KV_own.shape) != (lp.m, 2 * f) or tuple(KV_halo.shape) != (lp.h, 2 * f):
+        raise ValueError("KV_own / KV_halo must be [%d, %d] / [%d, %d], got %s / %s" % (
+            lp.m, 2 * f, lp.h, 2 * f, tuple(KV_own.shape), tuple(KV_halo.shape)))
+    if tuple(L.shape) != (lp.m, heads):
+        raise ValueError("L must be [%d, %d], got %s" % (lp.m, heads, tuple(L.shape)))
+    scale = transformer_scale(f, heads) if scale is None else float(scale)
+    dargs = _drop_args(drop, snap)
+    dQ = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+    D = torch.empty((lp.m, heads), dtype=torch.float32, device=dev)
+    work = torch.empty((fwd.nslots, f), dtype=torch.float32, device=dev)
+    _transformer(dev, "pgcn_transformer_backward_rows", C.byref(fwd.c), lp.m, lp.h, heads, Q_own.data_ptr(),
+                 KV_own.data_ptr(), KV_halo.data_ptr(), scale, gid.data_ptr(), *dargs, gZ_own.data_ptr(),
+                 Z_own.data_ptr(), L.data_ptr(), dQ.data_ptr(), D.data_ptr(), work.data_ptr(), f)
+    dKV = torch.empty((lp.m + lp.h, 2 * f), dtype=torch.float32, device=dev)
+    work = torch.empty((tr.nslots, 2 * f), dtype=torch.float32, device=dev)
+    _transformer(dev, "pgcn_transformer_backward_cols", C.byref(tr.c), lp.m, lp.h, heads, Q_own.data_ptr(),
+                 KV_own.data_ptr(), KV_halo.data_ptr(), scale, gid.data_ptr(), *dargs, gZ_own.data_ptr(), L.data_ptr(),
+                 D.data_ptr(), dKV.data_ptr(), work.data_ptr(), f)
+    _call(plan, dev, "pgcn_halo_rows_add", dKV[lp.m:].data_ptr(), dKV.data_ptr(), 2 * f, exchange=True)
+    return dQ, dKV[:lp.m, :f], dKV[:lp.m, f:]
+
+
+class PTransformerAttention(torch.autograd.Function):
+    """Scaled dot-product attention over the plan's stored pattern, the attention of PyG's TransformerConv (concat=True,
+    without edge features), with K heads of width C = f / K concatenated:
+
+        PTransformerAttention.apply(A, Q, K, V, heads, scale=None, dropout=None)
+        s_eh = scale <Q[i, h], K[j, h]>,  alpha_.h = softmax of s_.h over row i's stored entries,
+        out[i, h] = sum over the stored entries e = (i, j) of  alpha_eh V[j, h]
+
+    Q, K and V are [rows, f] fp32 CUDA tensors (f <= 256, heads 1, 2, 4 or 8 dividing f), out is [rows, f] (rows = m in
+    the "local" layout, n in the "global" one, as PSpMM). scale None: float32(1 / sqrt(C)). The values of A are not
+    read; every stored entry contributes, duplicates included; a row without entries gives 0. One exchange per layer
+    carries [K | V] (2f floats per row), so the plan's f_max must be at least 2f; the backward returns the halo rows'
+    partial dK and dV to their owners in one reverse exchange. Only the rows' log-sum-exp ([rows, K]) is kept besides
+    the operands: the backward recomputes the probabilities. Gradients go to Q, K and V. Deterministic. The exchanges
+    are the unsplit ones (no per-source overlap). The plan must be bound (PgcnPlan.bind_values); the first call builds
+    its index tables (PgcnPlan.gated_walks, PgcnPlan.global_ids).
+
+    dropout (an op.EdgeDropout with p > 0): attention dropout on every head, the mask of op.edge_dropout drawn inline
+    from the global (row, column) of each entry, so every partition draws the same mask. Each forward advances the
+    dropout's counter on the device and the backward reuses that forward's snapshot, so CUDA-graph replays draw new
+    masks. None or p == 0: no mask is drawn."""
+
+    @staticmethod
+    def forward(ctx, A, Q, K, V, heads, scale=None, dropout=None):
+        drop = _active(dropout)
+        A.gated_walks()
+        A.global_ids()
+        Q_own = _own(A, Q, "Q")
+        Z, L, KV, KV_halo, snap = aggregate_transformer(A, Q_own, _own(A, K, "K"), _own(A, V, "V"), heads, scale, drop)
+        ctx.plan, ctx.heads, ctx.drop = A, heads, drop
+        ctx.scale = transformer_scale(Q_own.shape[1], heads) if scale is None else float(scale)
+        ctx.save_for_backward(Q_own, KV, KV_halo, Z, L, snap)
+        return _to_layout(A, Z)
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        A = ctx.plan
+        Q_own, KV, KV_halo, Z, L, snap = ctx.saved_tensors
+        dQ, dK, dV = aggregate_transformer_backward(A, Q_own, KV, KV_halo, Z, L, _own(A, grad_output, "grad_output"),
+                                                    ctx.heads, ctx.scale, ctx.drop, snap)
+        return None, _to_layout(A, dQ), _to_layout(A, dK), _to_layout(A, dV), None, None, None
+
+
 # ---- the pieces, individually callable (NCCL transport), mirroring communicate_fgm ----------------
 
 def spmm_local(plan, H_own, H_halo=None, transpose=False):

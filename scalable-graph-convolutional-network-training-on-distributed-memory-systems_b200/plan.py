@@ -239,6 +239,7 @@ class PgcnPlan:
         self._edge_index = None
         self._edge_pairs = None
         self._gated_walks = None
+        self._global_ids = None
         # edge values (bind_values / set_values): which values the records hold, as far as this process knows
         self._bound = False
         self._resident = "creation"      # "creation", a key of the tensor set last, or None: unknown
@@ -386,7 +387,8 @@ class PgcnPlan:
 
     def gated_walks(self):
         """(fwd, tr): the GatedWalk of the local forward CSR and of its transpose, the device index arrays and work tables
-        of the gated aggregation (op.PSpMMGated, include/pgcn_gated.h). About 8 B per entry (both index arrays) and 16 B
+        of the gated aggregation (op.PSpMMGated, include/pgcn_gated.h) and of the transformer attention
+        (op.PTransformerAttention, include/pgcn_transformer.h), which walk the same tables. About 8 B per entry (both index arrays) and 16 B
         per row and per column (the work items), about 170 MB on C2. Built on first use by host-to-device copies, which a
         CUDA graph cannot capture: call it, or the operator once eagerly, before capturing a step that uses it."""
         import torch
@@ -399,6 +401,23 @@ class PgcnPlan:
             self._gated_walks = (GatedWalk(lp.rowptr, lp.colidx, chunk, self.device),
                                  GatedWalk(lp.t_rowptr, lp.t_colidx, chunk, self.device))
         return self._gated_walks
+
+    def global_ids(self):
+        """The global ids of the owned rows, then of the halo rows ([halo by peer] order): a CUDA int32 [m + h] tensor,
+        the ids the transformer attention's dropout mask is drawn from (include/pgcn_transformer.h), so that every
+        partition draws the same mask. Built on first use by a host-to-device copy, which a CUDA graph cannot capture:
+        call it, or the operator once eagerly, before capturing a step that uses it."""
+        import torch
+        if self._global_ids is None:
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError("PgcnPlan.global_ids is built by a host-to-device copy, which a CUDA-graph capture "
+                                   "cannot hold: call plan.global_ids() once before the capture")
+            lp = self.lp
+            if lp.n > np.iinfo(np.int32).max:
+                raise ValueError("n=%d: global_ids holds global ids as int32" % lp.n)
+            ids = np.concatenate([lp.owned, lp.halo]).astype(np.int32)
+            self._global_ids = torch.from_numpy(ids).to(self.device)
+        return self._global_ids
 
     def algorithmic_bytes(self, f):
         b = cabi.PgcnBytes()
