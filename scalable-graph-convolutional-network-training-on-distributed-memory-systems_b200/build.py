@@ -2,8 +2,9 @@
 
   lib/libpgcn_b200.so     csrc/pgcn_b200.cu (+ spmm_kernels.cuh, spmm_ring.cuh, sddmm.cuh, attention.cuh, spmm_max.cuh, gatv2.cuh)   nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo
   lib/libpgcn_dropout.so  csrc/edge_dropout.cu (+ philox.cuh)                                                                        the same flags
-  lib/libpgcn_gated.so    csrc/gated.cu                                                                                              the same flags
+  lib/libpgcn_gated.so    csrc/gated.cu (+ gated_math.cuh)                                                                           the same flags
   lib/libpgcn_transformer.so csrc/transformer.cu (+ philox.cuh, pgcn_gated.h for the walk struct)                                     the same flags
+  lib/libpgcn_gatedgcn.so csrc/gatedgcn.cu (+ gated_math.cuh, pgcn_gated.h for the walk struct)                                       the same flags
   (the CPU oracle under oracle/ is built by oracle/build_oracle.py — test infrastructure only)
 
 nvcc cross-compiles without a GPU; `python -m <pkg>.build` or `__graft_entry__.build()` runs this.
@@ -36,13 +37,20 @@ DROPOUT_DEPS = DROPOUT_SOURCES + [os.path.join(CSRC, "philox.cuh"), os.path.join
 # so has the gated-aggregation library
 GATED_LIB = os.path.join(LIBDIR, "libpgcn_gated.so")
 GATED_SOURCES = [os.path.join(CSRC, "gated.cu")]
-GATED_DEPS = GATED_SOURCES + [os.path.join(ROOT, "include", "pgcn_gated.h"), os.path.abspath(__file__)]
+GATED_DEPS = GATED_SOURCES + [os.path.join(CSRC, "gated_math.cuh"), os.path.join(ROOT, "include", "pgcn_gated.h"),
+                              os.path.abspath(__file__)]
 # and the transformer-attention library, which takes the gated library's walk struct and the dropout's Philox
 TRANSFORMER_LIB = os.path.join(LIBDIR, "libpgcn_transformer.so")
 TRANSFORMER_SOURCES = [os.path.join(CSRC, "transformer.cu")]
 TRANSFORMER_DEPS = TRANSFORMER_SOURCES + [os.path.join(CSRC, "philox.cuh"),
                                           os.path.join(ROOT, "include", "pgcn_transformer.h"),
                                           os.path.join(ROOT, "include", "pgcn_gated.h"), os.path.abspath(__file__)]
+# and the GatedGCN library, which takes the gated library's walk struct and its gate (gated_math.cuh)
+GATEDGCN_LIB = os.path.join(LIBDIR, "libpgcn_gatedgcn.so")
+GATEDGCN_SOURCES = [os.path.join(CSRC, "gatedgcn.cu")]
+GATEDGCN_DEPS = GATEDGCN_SOURCES + [os.path.join(CSRC, "gated_math.cuh"),
+                                    os.path.join(ROOT, "include", "pgcn_gatedgcn.h"),
+                                    os.path.join(ROOT, "include", "pgcn_gated.h"), os.path.abspath(__file__)]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -79,6 +87,10 @@ def gated_is_stale():
 
 def transformer_is_stale():
     return _stale(TRANSFORMER_LIB, TRANSFORMER_DEPS)
+
+
+def gatedgcn_is_stale():
+    return _stale(GATEDGCN_LIB, GATEDGCN_DEPS)
 
 
 def _compile(lib, sources, defs, verbose):
@@ -125,9 +137,17 @@ def build_transformer(force=False, verbose=False):
     return _compile(TRANSFORMER_LIB, TRANSFORMER_SOURCES, [], verbose)
 
 
+def build_gatedgcn(force=False, verbose=False):
+    """Compile libpgcn_gatedgcn.so for sm_90a if missing or older than its sources. Returns its path."""
+    if not force and not gatedgcn_is_stale():
+        return GATEDGCN_LIB
+    return _compile(GATEDGCN_LIB, GATEDGCN_SOURCES, [], verbose)
+
+
 if __name__ == "__main__":
     force, verbose = "--force" in sys.argv, "-v" in sys.argv
     print(build(force=force, verbose=verbose))
     print(build_dropout(force=force, verbose=verbose))
     print(build_gated(force=force, verbose=verbose))
     print(build_transformer(force=force, verbose=verbose))
+    print(build_gatedgcn(force=force, verbose=verbose))

@@ -1,8 +1,9 @@
 """ctypes binding of include/pgcn_b200.h — the C-ABI drop-in boundary (SURVEY.md §8b) — and of include/pgcn_b200_halo.h,
-include/pgcn_dropout.h, include/pgcn_gated.h and include/pgcn_transformer.h.
+include/pgcn_dropout.h, include/pgcn_gated.h, include/pgcn_transformer.h and include/pgcn_gatedgcn.h.
 
 Nothing here computes: it loads lib/libpgcn_b200.so (load), lib/libpgcn_dropout.so (load_dropout) and
-lib/libpgcn_gated.so (load_gated) and lib/libpgcn_transformer.so (load_transformer), declares every exported symbol and turns negative status codes into RuntimeError. If the library is missing there is no fallback: the
+lib/libpgcn_gated.so (load_gated), lib/libpgcn_transformer.so (load_transformer) and lib/libpgcn_gatedgcn.so
+(load_gatedgcn), declares every exported symbol and turns negative status codes into RuntimeError. If the library is missing there is no fallback: the
 product path fails loudly (the CPU oracle under oracle/ is test infrastructure only).
 """
 import ctypes as C
@@ -41,6 +42,10 @@ GATED_SYMBOLS = ["pgcn_gated_version", "pgcn_gated_last_error", "pgcn_gated_chun
 TRANSFORMER_SYMBOLS = ["pgcn_transformer_version", "pgcn_transformer_last_error", "pgcn_transformer_forward",
                        "pgcn_transformer_backward_rows", "pgcn_transformer_backward_cols"]
 
+# every symbol declared in include/pgcn_gatedgcn.h
+GATEDGCN_SYMBOLS = ["pgcn_gatedgcn_version", "pgcn_gatedgcn_last_error", "pgcn_gatedgcn_load",
+                    "pgcn_gatedgcn_forward", "pgcn_gatedgcn_backward_rows", "pgcn_gatedgcn_backward_cols"]
+
 
 class PgcnBytes(C.Structure):
     _fields_ = [(n, C.c_int64) for n in (
@@ -60,6 +65,7 @@ _lib = None
 _dropout = None
 _gated = None
 _transformer = None
+_gatedgcn = None
 
 
 def lib_path():
@@ -76,6 +82,10 @@ def gated_lib_path():
 
 def transformer_lib_path():
     return _build.TRANSFORMER_LIB
+
+
+def gatedgcn_lib_path():
+    return _build.GATEDGCN_LIB
 
 
 def _built(path, stale, build, build_if_missing):
@@ -286,4 +296,38 @@ def check_transformer(rc):
     if rc < 0:
         msg = load_transformer().pgcn_transformer_last_error()
         raise RuntimeError("pgcn_transformer error %d: %s" % (rc, (msg or b"").decode("utf-8", "replace")))
+    return rc
+
+
+def load_gatedgcn(build_if_missing=True):
+    """Load libpgcn_gatedgcn.so (building it first when stale and nvcc is available)."""
+    global _gatedgcn
+    if _gatedgcn is not None:
+        return _gatedgcn
+    lib = C.CDLL(_built(_build.GATEDGCN_LIB, _build.gatedgcn_is_stale, _build.build_gatedgcn, build_if_missing))
+    vp, i32, f32, walk = C.c_void_p, C.c_int32, C.c_float, C.POINTER(PgcnGatedWalk)
+    lib.pgcn_gatedgcn_version.restype = C.c_char_p
+    lib.pgcn_gatedgcn_version.argtypes = []
+    lib.pgcn_gatedgcn_last_error.restype = C.c_char_p
+    lib.pgcn_gatedgcn_last_error.argtypes = []
+    lib.pgcn_gatedgcn_load.restype = C.c_int
+    lib.pgcn_gatedgcn_load.argtypes = []
+    # (walk, m, h, Dx_own, EB_own, EB_halo, Ce, eps, Z, den, Ehat, work, f, stream)
+    lib.pgcn_gatedgcn_forward.restype = C.c_int
+    lib.pgcn_gatedgcn_forward.argtypes = [walk, i32, i32, vp, vp, vp, vp, f32, vp, vp, vp, vp, i32, vp]
+    # (walk, m, h, EB_own, EB_halo, Ehat, gEhat, Z, den, gZ, eps, U, dCe, dDx, work, f, stream)
+    lib.pgcn_gatedgcn_backward_rows.restype = C.c_int
+    lib.pgcn_gatedgcn_backward_rows.argtypes = [walk, i32, i32, vp, vp, vp, vp, vp, vp, vp, f32, vp, vp, vp, vp, i32, vp]
+    # (walk, perm, m, h, Ehat, dCe, U, dEB, work, f, stream)
+    lib.pgcn_gatedgcn_backward_cols.restype = C.c_int
+    lib.pgcn_gatedgcn_backward_cols.argtypes = [walk, vp, i32, i32, vp, vp, vp, vp, vp, i32, vp]
+    _gatedgcn = lib
+    return lib
+
+
+def check_gatedgcn(rc):
+    """Raise RuntimeError carrying pgcn_gatedgcn_last_error when a libpgcn_gatedgcn call returned a negative status."""
+    if rc < 0:
+        msg = load_gatedgcn().pgcn_gatedgcn_last_error()
+        raise RuntimeError("pgcn_gatedgcn error %d: %s" % (rc, (msg or b"").decode("utf-8", "replace")))
     return rc

@@ -854,6 +854,154 @@ class PTransformerAttention(torch.autograd.Function):
         return None, _to_layout(A, dQ), _to_layout(A, dK), _to_layout(A, dV), None, None, None
 
 
+# ---- GatedGCN (libpgcn_gatedgcn.so) ----------------------------------------------------------------------------------
+
+GATEDGCN_EPS = 1e-6
+
+
+def _gatedgcn(dev, name, *args):
+    """libpgcn_gatedgcn.<name>(*args, stream) on `dev`'s current stream, its status checked."""
+    with torch.cuda.device(dev):
+        cabi.check_gatedgcn(getattr(cabi.load_gatedgcn(), name)(*args, _stream_ptr()))
+
+
+def _check_eps(eps):
+    import math
+    eps = float(eps)
+    if not (eps >= 0.0) or math.isinf(eps):
+        raise ValueError("eps=%r: GatedGCN's eps must be finite and >= 0" % (eps,))
+    return eps
+
+
+def _check_edges(plan, x, f, what):
+    """x, a per-entry tensor: fp32 CUDA [nnz_local, f] in the plan's forward-entry order. Returns it contiguous."""
+    _check_f32(x, what)
+    nnz = plan.lp.nnz()
+    if x.dim() != 2 or tuple(x.shape) != (nnz, f):
+        raise ValueError("%s must be [%d, %d] (the plan's local entries, edge_pairs() order), got %s" % (
+            what, nnz, f, tuple(x.shape)))
+    return x.contiguous()
+
+
+def _gatedgcn_operands(plan, Dx_own, Ex_own, Bx_own, eps, what):
+    """The walks and the transposed entries, then eps and Dx_own, Ex_own, Bx_own checked ([m, f] each, 2f <= f_max, a
+    bound plan), then the kernels loaded (pgcn_gatedgcn_load). The tables come first, so that a capture that needs them
+    before they exist is refused before any work is enqueued."""
+    walks = plan.gated_walks()
+    perm = plan.transposed_entries()
+    eps = _check_eps(eps)
+    f = Dx_own.shape[-1]
+    if 2 * f > plan.f_max:
+        raise ValueError("f=%d: %s exchanges [Ex | Bx] rows of 2f = %d floats, the plan's f_max is %d: build the plan "
+                         "with f_max >= 2f" % (f, what, 2 * f, plan.f_max))
+    Dx_own = _check_feat(plan, Dx_own, plan.m, "Dx")
+    Ex_own = _check_feat(plan, Ex_own, plan.m, "Ex")
+    Bx_own = _check_feat(plan, Bx_own, plan.m, "Bx")
+    if Ex_own.shape[1] != f or Bx_own.shape[1] != f:
+        raise ValueError("Dx, Ex and Bx must have the same width, got %d, %d and %d" % (f, Ex_own.shape[1],
+                                                                                       Bx_own.shape[1]))
+    _require_bound(plan, "%s exchanges [Ex | Bx] through pgcn_halo_rows" % what)
+    with torch.cuda.device(plan.device):
+        # every kernel loaded before the exchange: ranks of one process must not load one behind a waiting exchange
+        cabi.check_gatedgcn(cabi.load_gatedgcn().pgcn_gatedgcn_load())
+    return walks, perm, Dx_own, Ex_own, Bx_own, eps
+
+
+def aggregate_gatedgcn(plan, Dx_own, Ex_own, Bx_own, Ce, eps=GATEDGCN_EPS):
+    """(Z_own, Ehat, den, EB_own, EB_halo): GatedGCN's edge-gated aggregation over the plan's stored pattern
+    (pgcn_gatedgcn_forward). For every local entry e = (i, j): Ehat_e = (Dx[i] + Ex[j]) + Ce_e, s_e = sigmoid(Ehat_e),
+    Z_own[i] = sum_e s_e Bx[j] / (sum_e s_e + eps), element-wise. Dx_own, Ex_own, Bx_own, Z_own and den (the rows' sums
+    of gates) are [m, f]; Ce and Ehat are [nnz_local, f] in edge_pairs() order. EB_own is [Ex | Bx] ([m, 2f]) and EB_halo
+    [h, 2f] its halo rows from one exchange (pgcn_halo_rows), which aggregate_gatedgcn_backward takes. Needs a bound
+    plan with f_max >= 2f."""
+    (fwd, _), _, Dx_own, Ex_own, Bx_own, eps = _gatedgcn_operands(plan, Dx_own, Ex_own, Bx_own, eps,
+                                                                  "aggregate_gatedgcn")
+    lp, f, dev = plan.lp, Dx_own.shape[1], Dx_own.device
+    Ce = _check_edges(plan, Ce, f, "Ce")
+    EB = torch.cat([Ex_own, Bx_own], 1)
+    EB_halo = torch.empty((lp.h, 2 * f), dtype=torch.float32, device=dev)
+    _call(plan, dev, "pgcn_halo_rows", EB.data_ptr(), EB_halo.data_ptr(), 2 * f, exchange=False)
+    Z = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+    den = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+    Ehat = torch.empty((lp.nnz(), f), dtype=torch.float32, device=dev)
+    work = torch.empty((fwd.nslots, 2 * f), dtype=torch.float32, device=dev)
+    _gatedgcn(dev, "pgcn_gatedgcn_forward", C.byref(fwd.c), lp.m, lp.h, Dx_own.data_ptr(), EB.data_ptr(),
+              EB_halo.data_ptr(), Ce.data_ptr(), eps, Z.data_ptr(), den.data_ptr(), Ehat.data_ptr(), work.data_ptr(), f)
+    return Z, Ehat, den, EB, EB_halo
+
+
+def aggregate_gatedgcn_backward(plan, Ehat, EB_own, EB_halo, Z_own, den, gZ_own, gEhat=None, eps=GATEDGCN_EPS):
+    """(dDx, dEx, dBx, dCe): the gradients of aggregate_gatedgcn's outputs for the output gradients gZ_own [m, f] and
+    gEhat [nnz_local, f] (None: zero), from its Ehat, EB_own, EB_halo, Z_own and den and the same eps. The row walk
+    (pgcn_gatedgcn_backward_rows) forms U = gZ / (den + eps) once per row and gives dCe ([nnz_local, f], the gradient of
+    Ehat and of Ce) and dDx; the column walk over the transposed entries (pgcn_gatedgcn_backward_cols) gives dEx and dBx,
+    whose halo rows go back to their owners and are added there (pgcn_halo_rows_add)."""
+    f = Z_own.shape[-1]
+    (fwd, tr), perm, Z_own, den, gZ_own, eps = _gatedgcn_operands(plan, Z_own, den, gZ_own, eps,
+                                                                  "aggregate_gatedgcn_backward")
+    lp, dev = plan.lp, Z_own.device
+    Ehat = _check_edges(plan, Ehat, f, "Ehat")
+    if gEhat is not None:
+        gEhat = _check_edges(plan, gEhat, f, "gEhat")
+    EB_own, EB_halo = EB_own.contiguous(), EB_halo.contiguous()
+    if tuple(EB_own.shape) != (lp.m, 2 * f) or tuple(EB_halo.shape) != (lp.h, 2 * f):
+        raise ValueError("EB_own / EB_halo must be [%d, %d] / [%d, %d], got %s / %s" % (
+            lp.m, 2 * f, lp.h, 2 * f, tuple(EB_own.shape), tuple(EB_halo.shape)))
+    U = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+    dDx = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+    dCe = torch.empty((lp.nnz(), f), dtype=torch.float32, device=dev)
+    work = torch.empty((fwd.nslots, f), dtype=torch.float32, device=dev)
+    _gatedgcn(dev, "pgcn_gatedgcn_backward_rows", C.byref(fwd.c), lp.m, lp.h, EB_own.data_ptr(), EB_halo.data_ptr(),
+              Ehat.data_ptr(), _ptr(gEhat), Z_own.data_ptr(), den.data_ptr(), gZ_own.data_ptr(), eps, U.data_ptr(),
+              dCe.data_ptr(), dDx.data_ptr(), work.data_ptr(), f)
+    dEB = torch.empty((lp.m + lp.h, 2 * f), dtype=torch.float32, device=dev)
+    work = torch.empty((tr.nslots, 2 * f), dtype=torch.float32, device=dev)
+    _gatedgcn(dev, "pgcn_gatedgcn_backward_cols", C.byref(tr.c), perm.data_ptr(), lp.m, lp.h, Ehat.data_ptr(),
+              dCe.data_ptr(), U.data_ptr(), dEB.data_ptr(), work.data_ptr(), f)
+    _call(plan, dev, "pgcn_halo_rows_add", dEB[lp.m:].data_ptr(), dEB.data_ptr(), 2 * f, exchange=True)
+    return dDx, dEB[:lp.m, :f], dEB[:lp.m, f:], dCe
+
+
+class PGatedGCN(torch.autograd.Function):
+    """GatedGCN's edge-gated aggregation over the plan's stored pattern (Bresson & Laurent; the layer of Dwivedi et
+    al.'s benchmarking-gnns and GraphGPS's default local layer), with an edge-feature stream:
+
+        Z, Ehat = PGatedGCN.apply(A, Dx, Ex, Bx, Ce, eps=1e-6)
+        Ehat_e = (Dx[i] + Ex[j]) + Ce_e                      for every stored entry e = (i, j)
+        Z[i]   = sum_e sigmoid(Ehat_e) Bx[j] / (sum_e sigmoid(Ehat_e) + eps)          (element-wise, f features)
+
+    Dx, Ex and Bx are [rows, f] fp32 CUDA tensors and Z is [rows, f] (rows = m in the "local" layout, n in the "global"
+    one, as PSpMM). Ce and Ehat are [nnz_local, f] in both layouts: one row per local entry in the order of
+    PgcnPlan.edge_pairs(). They never cross ranks, since every entry belongs to the rank that owns its row. The values of
+    A are not read; every stored entry contributes, duplicates included. A row without entries gives 0 (NaN when
+    eps == 0). One exchange per layer carries [Ex | Bx] (2f floats per row), so the plan's f_max must be at least 2f; the
+    backward returns the halo rows' partial dEx and dBx to their owners in one reverse exchange. Saved for the backward:
+    Ehat (the output), Z, the rows' gate sums and the [Ex | Bx] own and halo rows; the gates are recomputed. An unused
+    Ehat costs no gradient tensor: its gradient reaches the kernel as NULL. Gradients go to Dx, Ex, Bx and Ce.
+    Deterministic. The exchanges are the unsplit ones (no per-source overlap). The plan must be bound
+    (PgcnPlan.bind_values); the first call builds its index tables (PgcnPlan.gated_walks,
+    PgcnPlan.transposed_entries)."""
+
+    @staticmethod
+    def forward(ctx, A, Dx, Ex, Bx, Ce, eps=GATEDGCN_EPS):
+        ctx.set_materialize_grads(False)
+        A.gated_walks()
+        A.transposed_entries()
+        Z, Ehat, den, EB, EB_halo = aggregate_gatedgcn(A, _own(A, Dx, "Dx"), _own(A, Ex, "Ex"), _own(A, Bx, "Bx"),
+                                                       Ce, eps)
+        ctx.plan, ctx.eps = A, _check_eps(eps)
+        ctx.save_for_backward(Ehat, Z, den, EB, EB_halo)
+        return _to_layout(A, Z), Ehat
+
+    @staticmethod
+    def backward(ctx, gZ, gEhat):
+        A = ctx.plan
+        Ehat, Z, den, EB, EB_halo = ctx.saved_tensors
+        gZ = torch.zeros_like(Z) if gZ is None else _own(A, gZ, "grad Z")
+        dDx, dEx, dBx, dCe = aggregate_gatedgcn_backward(A, Ehat, EB, EB_halo, Z, den, gZ, gEhat, ctx.eps)
+        return None, _to_layout(A, dDx), _to_layout(A, dEx), _to_layout(A, dBx), dCe, None
+
+
 # ---- the pieces, individually callable (NCCL transport), mirroring communicate_fgm ----------------
 
 def spmm_local(plan, H_own, H_halo=None, transpose=False):

@@ -89,12 +89,14 @@ def _cuda_device(rank, backend, name):
 
 
 def train(rank, size, nlayers, nfeatures, path_A, path_partvec, backend, name, layer, f_max, grad_H,
-          transport="auto", out=sys.stdout, seed=None, epochs=50):
+          transport="auto", out=sys.stdout, seed=None, epochs=50, model=None):
     """The training loop of PGAT.py and PSAGE.py (`name`): a bound plan of width f_max, inputs H[i, :] = i (requiring
     grad when grad_H) and labels i % f, nlayers layers `layer(plan)` (f -> f) built under `seed` and averaged over
     ranks, Adam lr 1e-3, `epochs` epochs of the loss sum_owned nll / n with gradients averaged over ranks. Rank 0 prints
     `Epoch {:05d} | Loss {:.4f}` (the all-reduced loss) per epoch and `Elapsed time {:.4f}`. Returns the losses, the
-    elapsed time, the transport and plan.stats."""
+    elapsed time, the transport and plan.stats. model: a factory model(plan) of the whole network (H -> logits), built
+    under `seed` in place of the stack of `layer`s, for a network that is not a plain sequence of layers (PGATEDGCN.py:
+    an edge-feature stream beside the node features)."""
     device = _cuda_device(rank, backend, name)
     lp_host = planmod.read_local_plan(path_A, path_partvec, rank, size)
     n = lp_host.n
@@ -109,7 +111,8 @@ def train(rank, size, nlayers, nfeatures, path_A, path_partvec, backend, name, l
 
     if seed is not None:
         torch.manual_seed(seed)
-    model = nn.Sequential(*[layer(plan) for _ in range(nlayers)]).to(device)
+    factory = model
+    model = (factory(plan) if factory is not None else nn.Sequential(*[layer(plan) for _ in range(nlayers)])).to(device)
     if size > 1:
         initialize_parameters(model, size)
     optimizer = torch.optim.Adam(model.parameters(), lr=1e-3)

@@ -240,6 +240,7 @@ class PgcnPlan:
         self._edge_pairs = None
         self._gated_walks = None
         self._global_ids = None
+        self._transposed_entries = None
         # edge values (bind_values / set_values): which values the records hold, as far as this process knows
         self._bound = False
         self._resident = "creation"      # "creation", a key of the tensor set last, or None: unknown
@@ -418,6 +419,25 @@ class PgcnPlan:
             ids = np.concatenate([lp.owned, lp.halo]).astype(np.int32)
             self._global_ids = torch.from_numpy(ids).to(self.device)
         return self._global_ids
+
+    def transposed_entries(self):
+        """The forward entry of every transposed entry: a CUDA int32 [nnz] tensor `perm` with lp.t_colidx ==
+        rows[perm] (rows the forward entries' rows), from a stable sort of the forward entries by column, so duplicated
+        entries keep their forward order. GatedGCN's column walk (op.PGatedGCN, include/pgcn_gatedgcn.h) reads the
+        per-entry tensors through it. 4 B per entry. Built on first use by a host-to-device copy, which a CUDA graph
+        cannot capture: call it, or the operator once eagerly, before capturing a step that uses it."""
+        import torch
+        if self._transposed_entries is None:
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError("PgcnPlan.transposed_entries is built by a host-to-device copy, which a CUDA-graph "
+                                   "capture cannot hold: call plan.transposed_entries() once before the capture")
+            lp = self.lp
+            perm = np.argsort(lp.colidx, kind="stable")
+            rows = np.repeat(np.arange(lp.m, dtype=np.int32), np.diff(lp.rowptr.astype(np.int64)))
+            if not np.array_equal(rows[perm], lp.t_colidx):
+                raise ValueError("the plan's transposed CSR is not the stable column sort of its forward CSR")
+            self._transposed_entries = torch.from_numpy(perm.astype(np.int32)).to(self.device)
+        return self._transposed_entries
 
     def algorithmic_bytes(self, f):
         b = cabi.PgcnBytes()
