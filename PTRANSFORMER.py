@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Graph transformer layers (TransformerConv), launched like PGCN.py, PGAT.py, PSAGE.py and PGATED.py:
     python PTRANSFORMER.py -a A.mtx -p A.mtx.<k>.<hp|gp|rp> -b nccl -s <k> -l <layers> -f <features> [--heads K]
-                           [--attn-dropout P] [--seed N]
+                           [--attn-dropout P] [--edge-values] [--seed N]
 One process per GPU; rank/size from SLURM_PROCID/SLURM_NPROCS or RANK/WORLD_SIZE (torchrun)."""
 import sys
 

@@ -3,7 +3,8 @@
   lib/libpgcn_b200.so     csrc/pgcn_b200.cu (+ spmm_kernels.cuh, spmm_ring.cuh, sddmm.cuh, attention.cuh, spmm_max.cuh, gatv2.cuh)   nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo
   lib/libpgcn_dropout.so  csrc/edge_dropout.cu (+ philox.cuh)                                                                        the same flags
   lib/libpgcn_gated.so    csrc/gated.cu (+ gated_math.cuh)                                                                           the same flags
-  lib/libpgcn_transformer.so csrc/transformer.cu (+ philox.cuh, pgcn_gated.h for the walk struct)                                     the same flags
+  lib/libpgcn_transformer.so csrc/transformer.cu (+ transformer_math.cuh, philox.cuh, pgcn_gated.h for the walk struct)               the same flags
+  lib/libpgcn_transformer_edge.so csrc/transformer_edge.cu (+ transformer_math.cuh, philox.cuh, pgcn_gated.h)                         the same flags
   lib/libpgcn_gatedgcn.so csrc/gatedgcn.cu (+ gated_math.cuh, pgcn_gated.h for the walk struct)                                       the same flags
   (the CPU oracle under oracle/ is built by oracle/build_oracle.py — test infrastructure only)
 
@@ -42,7 +43,7 @@ GATED_DEPS = GATED_SOURCES + [os.path.join(CSRC, "gated_math.cuh"), os.path.join
 # and the transformer-attention library, which takes the gated library's walk struct and the dropout's Philox
 TRANSFORMER_LIB = os.path.join(LIBDIR, "libpgcn_transformer.so")
 TRANSFORMER_SOURCES = [os.path.join(CSRC, "transformer.cu")]
-TRANSFORMER_DEPS = TRANSFORMER_SOURCES + [os.path.join(CSRC, "philox.cuh"),
+TRANSFORMER_DEPS = TRANSFORMER_SOURCES + [os.path.join(CSRC, "transformer_math.cuh"), os.path.join(CSRC, "philox.cuh"),
                                           os.path.join(ROOT, "include", "pgcn_transformer.h"),
                                           os.path.join(ROOT, "include", "pgcn_gated.h"), os.path.abspath(__file__)]
 # and the GatedGCN library, which takes the gated library's walk struct and its gate (gated_math.cuh)
@@ -51,6 +52,14 @@ GATEDGCN_SOURCES = [os.path.join(CSRC, "gatedgcn.cu")]
 GATEDGCN_DEPS = GATEDGCN_SOURCES + [os.path.join(CSRC, "gated_math.cuh"),
                                     os.path.join(ROOT, "include", "pgcn_gatedgcn.h"),
                                     os.path.join(ROOT, "include", "pgcn_gated.h"), os.path.abspath(__file__)]
+# and the transformer attention with edge features, which shares the transformer's lane math (transformer_math.cuh)
+TRANSFORMER_EDGE_LIB = os.path.join(LIBDIR, "libpgcn_transformer_edge.so")
+TRANSFORMER_EDGE_SOURCES = [os.path.join(CSRC, "transformer_edge.cu")]
+TRANSFORMER_EDGE_DEPS = TRANSFORMER_EDGE_SOURCES + [os.path.join(CSRC, "transformer_math.cuh"),
+                                                    os.path.join(CSRC, "philox.cuh"),
+                                                    os.path.join(ROOT, "include", "pgcn_transformer_edge.h"),
+                                                    os.path.join(ROOT, "include", "pgcn_gated.h"),
+                                                    os.path.abspath(__file__)]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -91,6 +100,10 @@ def transformer_is_stale():
 
 def gatedgcn_is_stale():
     return _stale(GATEDGCN_LIB, GATEDGCN_DEPS)
+
+
+def transformer_edge_is_stale():
+    return _stale(TRANSFORMER_EDGE_LIB, TRANSFORMER_EDGE_DEPS)
 
 
 def _compile(lib, sources, defs, verbose):
@@ -144,6 +157,13 @@ def build_gatedgcn(force=False, verbose=False):
     return _compile(GATEDGCN_LIB, GATEDGCN_SOURCES, [], verbose)
 
 
+def build_transformer_edge(force=False, verbose=False):
+    """Compile libpgcn_transformer_edge.so for sm_90a if missing or older than its sources. Returns its path."""
+    if not force and not transformer_edge_is_stale():
+        return TRANSFORMER_EDGE_LIB
+    return _compile(TRANSFORMER_EDGE_LIB, TRANSFORMER_EDGE_SOURCES, [], verbose)
+
+
 if __name__ == "__main__":
     force, verbose = "--force" in sys.argv, "-v" in sys.argv
     print(build(force=force, verbose=verbose))
@@ -151,3 +171,4 @@ if __name__ == "__main__":
     print(build_gated(force=force, verbose=verbose))
     print(build_transformer(force=force, verbose=verbose))
     print(build_gatedgcn(force=force, verbose=verbose))
+    print(build_transformer_edge(force=force, verbose=verbose))

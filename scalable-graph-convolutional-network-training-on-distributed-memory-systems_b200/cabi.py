@@ -1,9 +1,10 @@
 """ctypes binding of include/pgcn_b200.h — the C-ABI drop-in boundary (SURVEY.md §8b) — and of include/pgcn_b200_halo.h,
-include/pgcn_dropout.h, include/pgcn_gated.h, include/pgcn_transformer.h and include/pgcn_gatedgcn.h.
+include/pgcn_dropout.h, include/pgcn_gated.h, include/pgcn_transformer.h, include/pgcn_gatedgcn.h and
+include/pgcn_transformer_edge.h.
 
 Nothing here computes: it loads lib/libpgcn_b200.so (load), lib/libpgcn_dropout.so (load_dropout) and
-lib/libpgcn_gated.so (load_gated), lib/libpgcn_transformer.so (load_transformer) and lib/libpgcn_gatedgcn.so
-(load_gatedgcn), declares every exported symbol and turns negative status codes into RuntimeError. If the library is missing there is no fallback: the
+lib/libpgcn_gated.so (load_gated), lib/libpgcn_transformer.so (load_transformer), lib/libpgcn_gatedgcn.so
+(load_gatedgcn) and lib/libpgcn_transformer_edge.so (load_transformer_edge), declares every exported symbol and turns negative status codes into RuntimeError. If the library is missing there is no fallback: the
 product path fails loudly (the CPU oracle under oracle/ is test infrastructure only).
 """
 import ctypes as C
@@ -46,6 +47,11 @@ TRANSFORMER_SYMBOLS = ["pgcn_transformer_version", "pgcn_transformer_last_error"
 GATEDGCN_SYMBOLS = ["pgcn_gatedgcn_version", "pgcn_gatedgcn_last_error", "pgcn_gatedgcn_load",
                     "pgcn_gatedgcn_forward", "pgcn_gatedgcn_backward_rows", "pgcn_gatedgcn_backward_cols"]
 
+# every symbol declared in include/pgcn_transformer_edge.h
+TRANSFORMER_EDGE_SYMBOLS = ["pgcn_transformer_edge_version", "pgcn_transformer_edge_last_error",
+                            "pgcn_transformer_edge_load", "pgcn_transformer_edge_forward",
+                            "pgcn_transformer_edge_backward_rows", "pgcn_transformer_edge_backward_cols"]
+
 
 class PgcnBytes(C.Structure):
     _fields_ = [(n, C.c_int64) for n in (
@@ -66,6 +72,7 @@ _dropout = None
 _gated = None
 _transformer = None
 _gatedgcn = None
+_transformer_edge = None
 
 
 def lib_path():
@@ -86,6 +93,10 @@ def transformer_lib_path():
 
 def gatedgcn_lib_path():
     return _build.GATEDGCN_LIB
+
+
+def transformer_edge_lib_path():
+    return _build.TRANSFORMER_EDGE_LIB
 
 
 def _built(path, stale, build, build_if_missing):
@@ -330,4 +341,41 @@ def check_gatedgcn(rc):
     if rc < 0:
         msg = load_gatedgcn().pgcn_gatedgcn_last_error()
         raise RuntimeError("pgcn_gatedgcn error %d: %s" % (rc, (msg or b"").decode("utf-8", "replace")))
+    return rc
+
+
+def load_transformer_edge(build_if_missing=True):
+    """Load libpgcn_transformer_edge.so (building it first when stale and nvcc is available)."""
+    global _transformer_edge
+    if _transformer_edge is not None:
+        return _transformer_edge
+    lib = C.CDLL(_built(_build.TRANSFORMER_EDGE_LIB, _build.transformer_edge_is_stale, _build.build_transformer_edge,
+                        build_if_missing))
+    vp, i32, u32, f32, walk = C.c_void_p, C.c_int32, C.c_uint32, C.c_float, C.POINTER(PgcnGatedWalk)
+    lib.pgcn_transformer_edge_version.restype = C.c_char_p
+    lib.pgcn_transformer_edge_version.argtypes = []
+    lib.pgcn_transformer_edge_last_error.restype = C.c_char_p
+    lib.pgcn_transformer_edge_last_error.argtypes = []
+    lib.pgcn_transformer_edge_load.restype = C.c_int
+    lib.pgcn_transformer_edge_load.argtypes = []
+    # (walk, m, h, heads, Q_own, KV_own, KV_halo, E, scale, gid, drop, threshold, keep_scale, ...)
+    head = [walk, i32, i32, i32, vp, vp, vp, vp, f32, vp, vp, u32, f32]
+    lib.pgcn_transformer_edge_forward.restype = C.c_int
+    lib.pgcn_transformer_edge_forward.argtypes = head + [vp, vp, vp, i32, vp]
+    # (..., gZ, Z, L, dQ, D, PS, dE, work, f, stream)
+    lib.pgcn_transformer_edge_backward_rows.restype = C.c_int
+    lib.pgcn_transformer_edge_backward_rows.argtypes = head + [vp, vp, vp, vp, vp, vp, vp, vp, i32, vp]
+    # (walk, perm, m, h, heads, Q_own, gZ, PS, scale, dKV, work, f, stream)
+    lib.pgcn_transformer_edge_backward_cols.restype = C.c_int
+    lib.pgcn_transformer_edge_backward_cols.argtypes = [walk, vp, i32, i32, i32, vp, vp, vp, f32, vp, vp, i32, vp]
+    _transformer_edge = lib
+    return lib
+
+
+def check_transformer_edge(rc):
+    """Raise RuntimeError carrying pgcn_transformer_edge_last_error when a libpgcn_transformer_edge call returned a
+    negative status."""
+    if rc < 0:
+        msg = load_transformer_edge().pgcn_transformer_edge_last_error()
+        raise RuntimeError("pgcn_transformer_edge error %d: %s" % (rc, (msg or b"").decode("utf-8", "replace")))
     return rc

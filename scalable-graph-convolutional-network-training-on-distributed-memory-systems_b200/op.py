@@ -1002,6 +1002,129 @@ class PGatedGCN(torch.autograd.Function):
         return None, _to_layout(A, dDx), _to_layout(A, dEx), _to_layout(A, dBx), dCe, None
 
 
+# ---- graph transformer attention with edge features (libpgcn_transformer_edge.so) ----------------------------------
+
+def _transformer_edge(dev, name, *args):
+    """libpgcn_transformer_edge.<name>(*args, stream) on `dev`'s current stream, its status checked."""
+    with torch.cuda.device(dev):
+        cabi.check_transformer_edge(getattr(cabi.load_transformer_edge(), name)(*args, _stream_ptr()))
+
+
+def _transformer_edge_operands(plan, Q_own, K_own, V_own, E, heads, drop, what):
+    """_transformer_operands, then the transposed entries, E checked ([nnz_local, f]) and the kernels loaded
+    (pgcn_transformer_edge_load). Every table comes before any work is enqueued, so that a capture that needs one
+    before it exists is refused first."""
+    walks, gid, Q_own, K_own, V_own = _transformer_operands(plan, Q_own, K_own, V_own, heads, drop, what)
+    perm = plan.transposed_entries()
+    E = _check_edges(plan, E, Q_own.shape[1], "E")
+    with torch.cuda.device(plan.device):
+        # every kernel loaded before the exchange: ranks of one process must not load one behind a waiting exchange
+        cabi.check_transformer_edge(cabi.load_transformer_edge().pgcn_transformer_edge_load())
+    return walks, perm, gid, Q_own, K_own, V_own, E
+
+
+def aggregate_transformer_edge(plan, Q_own, K_own, V_own, E, heads, scale=None, drop=None):
+    """(Z_own, L, KV_own, KV_halo, snap): aggregate_transformer with an edge term E ([nnz_local, f] in edge_pairs()
+    order) added to the keys and values of every local entry e = (i, j) (pgcn_transformer_edge_forward):
+    s_eh = scale <Q[i, h], K[j, h] + E_e[h]>, alpha = softmax of s over each row's stored entries per head,
+    Z_own[i, h] = sum_e alpha_eh M_eh (V[j, h] + E_e[h]). Outputs, scale and drop as aggregate_transformer;
+    aggregate_transformer_edge_backward takes them. E never crosses ranks. Needs a bound plan with f_max >= 2f."""
+    drop = _active(drop)
+    (fwd, _), _, gid, Q_own, K_own, V_own, E = _transformer_edge_operands(plan, Q_own, K_own, V_own, E, heads, drop,
+                                                                          "aggregate_transformer_edge")
+    lp, f, dev = plan.lp, Q_own.shape[1], Q_own.device
+    scale = transformer_scale(f, heads) if scale is None else float(scale)
+    snap = drop.draw() if drop else None
+    KV = torch.cat([K_own, V_own], 1)
+    KV_halo = torch.empty((lp.h, 2 * f), dtype=torch.float32, device=dev)
+    _call(plan, dev, "pgcn_halo_rows", KV.data_ptr(), KV_halo.data_ptr(), 2 * f, exchange=False)
+    Z = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+    L = torch.empty((lp.m, heads), dtype=torch.float32, device=dev)
+    work = torch.empty((fwd.nslots, f + 2 * heads), dtype=torch.float32, device=dev)
+    _transformer_edge(dev, "pgcn_transformer_edge_forward", C.byref(fwd.c), lp.m, lp.h, heads, Q_own.data_ptr(),
+                      KV.data_ptr(), KV_halo.data_ptr(), E.data_ptr(), scale, gid.data_ptr(), *_drop_args(drop, snap),
+                      Z.data_ptr(), L.data_ptr(), work.data_ptr(), f)
+    return Z, L, KV, KV_halo, snap
+
+
+def aggregate_transformer_edge_backward(plan, Q_own, KV_own, KV_halo, E, Z_own, L, gZ_own, heads, scale=None,
+                                        drop=None, snap=None, need_dE=True):
+    """(dQ, dK, dV, dE): the gradients of aggregate_transformer_edge's Z_own for the output gradient gZ_own [m, f], from
+    its KV_own, KV_halo, Z_own and L, the same E and, with dropout, the same `drop` and its forward's `snap`. The row
+    walk (pgcn_transformer_edge_backward_rows) gives dQ, dE ([nnz_local, f]; None when need_dE is false, and then it is
+    not computed) and each entry's [P | ds] ([nnz_local, 2 heads]); the column walk over the transposed entries
+    (pgcn_transformer_edge_backward_cols) reads those and gives dK and dV, whose halo rows go back to their owners and
+    are added there (pgcn_halo_rows_add)."""
+    drop = _active(drop)
+    f = Q_own.shape[-1]
+    if drop is not None and snap is None:
+        raise ValueError("aggregate_transformer_edge_backward with dropout needs the forward's snapshot")
+    (fwd, tr), perm, gid, Q_own, gZ_own, Z_own, E = _transformer_edge_operands(
+        plan, Q_own, gZ_own, Z_own, E, heads, drop, "aggregate_transformer_edge_backward")
+    lp, dev = plan.lp, Q_own.device
+    KV_own, KV_halo, L = KV_own.contiguous(), KV_halo.contiguous(), L.contiguous()
+    if tuple(KV_own.shape) != (lp.m, 2 * f) or tuple(KV_halo.shape) != (lp.h, 2 * f):
+        raise ValueError("KV_own / KV_halo must be [%d, %d] / [%d, %d], got %s / %s" % (
+            lp.m, 2 * f, lp.h, 2 * f, tuple(KV_own.shape), tuple(KV_halo.shape)))
+    if tuple(L.shape) != (lp.m, heads):
+        raise ValueError("L must be [%d, %d], got %s" % (lp.m, heads, tuple(L.shape)))
+    scale = transformer_scale(f, heads) if scale is None else float(scale)
+    dQ = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+    D = torch.empty((lp.m, heads), dtype=torch.float32, device=dev)
+    PS = torch.empty((lp.nnz(), 2 * heads), dtype=torch.float32, device=dev)
+    dE = torch.empty((lp.nnz(), f), dtype=torch.float32, device=dev) if need_dE else None
+    work = torch.empty((fwd.nslots, f), dtype=torch.float32, device=dev)
+    _transformer_edge(dev, "pgcn_transformer_edge_backward_rows", C.byref(fwd.c), lp.m, lp.h, heads,
+                      Q_own.data_ptr(), KV_own.data_ptr(), KV_halo.data_ptr(), E.data_ptr(), scale, gid.data_ptr(),
+                      *_drop_args(drop, snap), gZ_own.data_ptr(), Z_own.data_ptr(), L.data_ptr(), dQ.data_ptr(),
+                      D.data_ptr(), PS.data_ptr(), _ptr(dE), work.data_ptr(), f)
+    dKV = torch.empty((lp.m + lp.h, 2 * f), dtype=torch.float32, device=dev)
+    work = torch.empty((tr.nslots, 2 * f), dtype=torch.float32, device=dev)
+    _transformer_edge(dev, "pgcn_transformer_edge_backward_cols", C.byref(tr.c), perm.data_ptr(), lp.m, lp.h, heads,
+                      Q_own.data_ptr(), gZ_own.data_ptr(), PS.data_ptr(), scale, dKV.data_ptr(), work.data_ptr(), f)
+    _call(plan, dev, "pgcn_halo_rows_add", dKV[lp.m:].data_ptr(), dKV.data_ptr(), 2 * f, exchange=True)
+    return dQ, dKV[:lp.m, :f], dKV[:lp.m, f:], dE
+
+
+class PTransformerEdgeAttention(torch.autograd.Function):
+    """PTransformerAttention with edge features, the attention of PyG's TransformerConv(edge_dim=..., concat=True,
+    beta=False) with E = lin_edge(edge_attr) formed by the caller:
+
+        PTransformerEdgeAttention.apply(A, Q, K, V, E, heads, scale=None, dropout=None)
+        s_eh = scale <Q[i, h], K[j, h] + E_e[h]>,  alpha_.h = softmax of s_.h over row i's stored entries,
+        out[i, h] = sum over the stored entries e = (i, j) of  alpha_eh (V[j, h] + E_e[h])
+
+    Q, K, V and out as PTransformerAttention's ([rows, f] in the plan's layout). E is [nnz_local, f] in both layouts:
+    one row per local entry in the order of PgcnPlan.edge_pairs(). It never crosses ranks, since every entry belongs to
+    the rank that owns its row. Gradients go to Q, K, V and E; dE is computed only when E requires it. The backward
+    stores each entry's [P | ds] (2 heads floats) between its two walks, so that the column walk reads no E. dropout,
+    heads, scale, the exchanges and the plan's tables as PTransformerAttention's; the first call also builds
+    PgcnPlan.transposed_entries. Deterministic."""
+
+    @staticmethod
+    def forward(ctx, A, Q, K, V, E, heads, scale=None, dropout=None):
+        drop = _active(dropout)
+        A.gated_walks()
+        A.global_ids()
+        A.transposed_entries()
+        Q_own = _own(A, Q, "Q")
+        Z, L, KV, KV_halo, snap = aggregate_transformer_edge(A, Q_own, _own(A, K, "K"), _own(A, V, "V"), E, heads,
+                                                             scale, drop)
+        ctx.plan, ctx.heads, ctx.drop = A, heads, drop
+        ctx.scale = transformer_scale(Q_own.shape[1], heads) if scale is None else float(scale)
+        ctx.save_for_backward(Q_own, KV, KV_halo, E.contiguous(), Z, L, snap)
+        return _to_layout(A, Z)
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        A = ctx.plan
+        Q_own, KV, KV_halo, E, Z, L, snap = ctx.saved_tensors
+        dQ, dK, dV, dE = aggregate_transformer_edge_backward(A, Q_own, KV, KV_halo, E, Z, L,
+                                                             _own(A, grad_output, "grad_output"), ctx.heads,
+                                                             ctx.scale, ctx.drop, snap, ctx.needs_input_grad[4])
+        return None, _to_layout(A, dQ), _to_layout(A, dK), _to_layout(A, dV), dE, None, None, None
+
+
 # ---- the pieces, individually callable (NCCL transport), mirroring communicate_fgm ----------------
 
 def spmm_local(plan, H_own, H_halo=None, transpose=False):
