@@ -6,6 +6,7 @@
   lib/libpgcn_transformer.so csrc/transformer.cu (+ transformer_math.cuh, philox.cuh, pgcn_gated.h for the walk struct)               the same flags
   lib/libpgcn_transformer_edge.so csrc/transformer_edge.cu (+ transformer_math.cuh, philox.cuh, pgcn_gated.h)                         the same flags
   lib/libpgcn_gatedgcn.so csrc/gatedgcn.cu (+ gated_math.cuh, pgcn_gated.h for the walk struct)                                       the same flags
+  lib/libpgcn_gine.so     csrc/gine.cu (+ gated_math.cuh, pgcn_gated.h for the walk struct)                                           the same flags
   (the CPU oracle under oracle/ is built by oracle/build_oracle.py — test infrastructure only)
 
 nvcc cross-compiles without a GPU; `python -m <pkg>.build` or `__graft_entry__.build()` runs this.
@@ -60,6 +61,11 @@ TRANSFORMER_EDGE_DEPS = TRANSFORMER_EDGE_SOURCES + [os.path.join(CSRC, "transfor
                                                     os.path.join(ROOT, "include", "pgcn_transformer_edge.h"),
                                                     os.path.join(ROOT, "include", "pgcn_gated.h"),
                                                     os.path.abspath(__file__)]
+# and GINE, which takes the gated library's walk struct and its lane loads (gated_math.cuh)
+GINE_LIB = os.path.join(LIBDIR, "libpgcn_gine.so")
+GINE_SOURCES = [os.path.join(CSRC, "gine.cu")]
+GINE_DEPS = GINE_SOURCES + [os.path.join(CSRC, "gated_math.cuh"), os.path.join(ROOT, "include", "pgcn_gine.h"),
+                            os.path.join(ROOT, "include", "pgcn_gated.h"), os.path.abspath(__file__)]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -104,6 +110,10 @@ def gatedgcn_is_stale():
 
 def transformer_edge_is_stale():
     return _stale(TRANSFORMER_EDGE_LIB, TRANSFORMER_EDGE_DEPS)
+
+
+def gine_is_stale():
+    return _stale(GINE_LIB, GINE_DEPS)
 
 
 def _compile(lib, sources, defs, verbose):
@@ -164,6 +174,13 @@ def build_transformer_edge(force=False, verbose=False):
     return _compile(TRANSFORMER_EDGE_LIB, TRANSFORMER_EDGE_SOURCES, [], verbose)
 
 
+def build_gine(force=False, verbose=False):
+    """Compile libpgcn_gine.so for sm_90a if missing or older than its sources. Returns its path."""
+    if not force and not gine_is_stale():
+        return GINE_LIB
+    return _compile(GINE_LIB, GINE_SOURCES, [], verbose)
+
+
 if __name__ == "__main__":
     force, verbose = "--force" in sys.argv, "-v" in sys.argv
     print(build(force=force, verbose=verbose))
@@ -172,3 +189,4 @@ if __name__ == "__main__":
     print(build_transformer(force=force, verbose=verbose))
     print(build_gatedgcn(force=force, verbose=verbose))
     print(build_transformer_edge(force=force, verbose=verbose))
+    print(build_gine(force=force, verbose=verbose))

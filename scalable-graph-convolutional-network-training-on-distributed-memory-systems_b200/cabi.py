@@ -1,10 +1,10 @@
 """ctypes binding of include/pgcn_b200.h — the C-ABI drop-in boundary (SURVEY.md §8b) — and of include/pgcn_b200_halo.h,
-include/pgcn_dropout.h, include/pgcn_gated.h, include/pgcn_transformer.h, include/pgcn_gatedgcn.h and
-include/pgcn_transformer_edge.h.
+include/pgcn_dropout.h, include/pgcn_gated.h, include/pgcn_transformer.h, include/pgcn_gatedgcn.h,
+include/pgcn_transformer_edge.h and include/pgcn_gine.h.
 
 Nothing here computes: it loads lib/libpgcn_b200.so (load), lib/libpgcn_dropout.so (load_dropout) and
 lib/libpgcn_gated.so (load_gated), lib/libpgcn_transformer.so (load_transformer), lib/libpgcn_gatedgcn.so
-(load_gatedgcn) and lib/libpgcn_transformer_edge.so (load_transformer_edge), declares every exported symbol and turns negative status codes into RuntimeError. If the library is missing there is no fallback: the
+(load_gatedgcn), lib/libpgcn_transformer_edge.so (load_transformer_edge) and lib/libpgcn_gine.so (load_gine), declares every exported symbol and turns negative status codes into RuntimeError. If the library is missing there is no fallback: the
 product path fails loudly (the CPU oracle under oracle/ is test infrastructure only).
 """
 import ctypes as C
@@ -52,6 +52,10 @@ TRANSFORMER_EDGE_SYMBOLS = ["pgcn_transformer_edge_version", "pgcn_transformer_e
                             "pgcn_transformer_edge_load", "pgcn_transformer_edge_forward",
                             "pgcn_transformer_edge_backward_rows", "pgcn_transformer_edge_backward_cols"]
 
+# every symbol declared in include/pgcn_gine.h
+GINE_SYMBOLS = ["pgcn_gine_version", "pgcn_gine_last_error", "pgcn_gine_load", "pgcn_gine_forward",
+                "pgcn_gine_backward"]
+
 
 class PgcnBytes(C.Structure):
     _fields_ = [(n, C.c_int64) for n in (
@@ -73,6 +77,7 @@ _gated = None
 _transformer = None
 _gatedgcn = None
 _transformer_edge = None
+_gine = None
 
 
 def lib_path():
@@ -97,6 +102,10 @@ def gatedgcn_lib_path():
 
 def transformer_edge_lib_path():
     return _build.TRANSFORMER_EDGE_LIB
+
+
+def gine_lib_path():
+    return _build.GINE_LIB
 
 
 def _built(path, stale, build, build_if_missing):
@@ -378,4 +387,35 @@ def check_transformer_edge(rc):
     if rc < 0:
         msg = load_transformer_edge().pgcn_transformer_edge_last_error()
         raise RuntimeError("pgcn_transformer_edge error %d: %s" % (rc, (msg or b"").decode("utf-8", "replace")))
+    return rc
+
+
+def load_gine(build_if_missing=True):
+    """Load libpgcn_gine.so (building it first when stale and nvcc is available)."""
+    global _gine
+    if _gine is not None:
+        return _gine
+    lib = C.CDLL(_built(_build.GINE_LIB, _build.gine_is_stale, _build.build_gine, build_if_missing))
+    vp, i32, walk = C.c_void_p, C.c_int32, C.POINTER(PgcnGatedWalk)
+    lib.pgcn_gine_version.restype = C.c_char_p
+    lib.pgcn_gine_version.argtypes = []
+    lib.pgcn_gine_last_error.restype = C.c_char_p
+    lib.pgcn_gine_last_error.argtypes = []
+    lib.pgcn_gine_load.restype = C.c_int
+    lib.pgcn_gine_load.argtypes = []
+    # (walk, m, h, X_own, X_halo, E, Z, work, f, stream)
+    lib.pgcn_gine_forward.restype = C.c_int
+    lib.pgcn_gine_forward.argtypes = [walk, i32, i32, vp, vp, vp, vp, vp, i32, vp]
+    # (walk, perm, m, h, X_own, X_halo, E, gZ, dE, dX, work, f, stream)
+    lib.pgcn_gine_backward.restype = C.c_int
+    lib.pgcn_gine_backward.argtypes = [walk, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, i32, vp]
+    _gine = lib
+    return lib
+
+
+def check_gine(rc):
+    """Raise RuntimeError carrying pgcn_gine_last_error when a libpgcn_gine call returned a negative status."""
+    if rc < 0:
+        msg = load_gine().pgcn_gine_last_error()
+        raise RuntimeError("pgcn_gine error %d: %s" % (rc, (msg or b"").decode("utf-8", "replace")))
     return rc

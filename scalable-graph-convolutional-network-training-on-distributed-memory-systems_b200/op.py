@@ -1125,6 +1125,104 @@ class PTransformerEdgeAttention(torch.autograd.Function):
         return None, _to_layout(A, dQ), _to_layout(A, dK), _to_layout(A, dV), dE, None, None, None
 
 
+# ---- GINE (libpgcn_gine.so) ------------------------------------------------------------------------------------------
+
+def _gine(dev, name, *args):
+    """libpgcn_gine.<name>(*args, stream) on `dev`'s current stream, its status checked."""
+    with torch.cuda.device(dev):
+        cabi.check_gine(getattr(cabi.load_gine(), name)(*args, _stream_ptr()))
+
+
+def _gine_operands(plan, X_own, E, what):
+    """The walks and the transposed entries, then X_own ([m, f], f <= f_max) and E ([nnz_local, f]) checked and the plan
+    bound, then the kernels loaded (pgcn_gine_load). The tables come first, so that a capture that needs them before
+    they exist is refused before any work is enqueued."""
+    walks = plan.gated_walks()
+    perm = plan.transposed_entries()
+    X_own = _check_feat(plan, X_own, plan.m, "X")
+    E = _check_edges(plan, E, X_own.shape[1], "E")
+    _require_bound(plan, "%s exchanges X through pgcn_halo_rows" % what)
+    with torch.cuda.device(plan.device):
+        # every kernel loaded before the exchange: ranks of one process must not load one behind a waiting exchange
+        cabi.check_gine(cabi.load_gine().pgcn_gine_load())
+    return walks, perm, X_own, E
+
+
+def aggregate_gine(plan, X_own, E):
+    """(Z_own, X_halo): GINE's aggregation over the plan's stored pattern (pgcn_gine_forward). For every local entry
+    e = (i, j): Z_own[i] = sum_e relu(X[j] + E_e), element-wise, over [own | halo] columns. X_own and Z_own are [m, f],
+    E is [nnz_local, f] in edge_pairs() order; X_halo [h, f] is X's halo rows from one exchange (pgcn_halo_rows), which
+    aggregate_gine_backward takes. Needs a bound plan with f_max >= f."""
+    (fwd, _), _, X_own, E = _gine_operands(plan, X_own, E, "aggregate_gine")
+    lp, f, dev = plan.lp, X_own.shape[1], X_own.device
+    X_halo = torch.empty((lp.h, f), dtype=torch.float32, device=dev)
+    _call(plan, dev, "pgcn_halo_rows", X_own.data_ptr(), X_halo.data_ptr(), f, exchange=False)
+    Z = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+    work = torch.empty((fwd.nslots, f), dtype=torch.float32, device=dev)
+    _gine(dev, "pgcn_gine_forward", C.byref(fwd.c), lp.m, lp.h, X_own.data_ptr(), X_halo.data_ptr(), E.data_ptr(),
+          Z.data_ptr(), work.data_ptr(), f)
+    return Z, X_halo
+
+
+def aggregate_gine_backward(plan, X_own, X_halo, E, gZ_own, need_dE=True):
+    """(dX_own, dE): the gradients of aggregate_gine's Z_own for the output gradient gZ_own [m, f], from the same X_own
+    and E and its X_halo. One column walk over the transposed entries (pgcn_gine_backward) recomputes each entry's ReLU
+    mask and gives dE ([nnz_local, f]; None when need_dE is false, and then it is not computed) and dX, whose halo rows
+    go back to their owners and are added there (pgcn_halo_rows_add)."""
+    (_, tr), perm, X_own, E = _gine_operands(plan, X_own, E, "aggregate_gine_backward")
+    lp, f, dev = plan.lp, X_own.shape[1], X_own.device
+    gZ_own = _check_feat(plan, gZ_own, plan.m, "gZ")
+    if gZ_own.shape[1] != f:
+        raise ValueError("X and gZ must have the same width, got %d and %d" % (f, gZ_own.shape[1]))
+    X_halo = X_halo.contiguous()
+    if tuple(X_halo.shape) != (lp.h, f):
+        raise ValueError("X_halo must be [%d, %d], got %s" % (lp.h, f, tuple(X_halo.shape)))
+    dE = torch.empty((lp.nnz(), f), dtype=torch.float32, device=dev) if need_dE else None
+    dX = torch.empty((lp.m + lp.h, f), dtype=torch.float32, device=dev)
+    work = torch.empty((tr.nslots, f), dtype=torch.float32, device=dev)
+    _gine(dev, "pgcn_gine_backward", C.byref(tr.c), perm.data_ptr(), lp.m, lp.h, X_own.data_ptr(), X_halo.data_ptr(),
+          E.data_ptr(), gZ_own.data_ptr(), _ptr(dE), dX.data_ptr(), work.data_ptr(), f)
+    _call(plan, dev, "pgcn_halo_rows_add", dX[lp.m:].data_ptr(), dX.data_ptr(), f, exchange=True)
+    return dX[:lp.m], dE
+
+
+class PGINE(torch.autograd.Function):
+    """GINE's aggregation over the plan's stored pattern (Hu et al.; the message of PyG's GINEConv, without the self
+    term (1 + eps) x_i and the MLP, which the layer adds):
+
+        Z = PGINE.apply(A, X, E)
+        Z[i] = sum over the stored entries e = (i, j) of  relu(X[j] + E_e)                (element-wise, f features)
+
+    X and Z are [rows, f] fp32 CUDA tensors (rows = m in the "local" layout, n in the "global" one, as PSpMM). E is
+    [nnz_local, f] in both layouts: one row per local entry in the order of PgcnPlan.edge_pairs(). It never crosses
+    ranks, since every entry belongs to the rank that owns its row. The values of A are not read; every stored entry
+    contributes, duplicates included. relu is torch's: NaN propagates, -0 stays -0, and the gradient passes where
+    X[j] + E_e > 0 or is NaN. One exchange per layer carries X (f floats per row), so the plan's f_max must be at least
+    f; the backward returns the halo rows' partial dX to their owners in one reverse exchange. Saved for the backward:
+    X's own and halo rows and E; the ReLU mask is recomputed. Gradients go to X and E; dE is computed only when E
+    requires it. Deterministic. The exchanges are the unsplit ones (no per-source overlap). The plan must be bound
+    (PgcnPlan.bind_values); the first call builds its index tables (PgcnPlan.gated_walks,
+    PgcnPlan.transposed_entries)."""
+
+    @staticmethod
+    def forward(ctx, A, X, E):
+        A.gated_walks()
+        A.transposed_entries()
+        X_own = _own(A, X, "X")
+        Z, X_halo = aggregate_gine(A, X_own, E)
+        ctx.plan = A
+        ctx.save_for_backward(X_own, X_halo, E)
+        return _to_layout(A, Z)
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        A = ctx.plan
+        X_own, X_halo, E = ctx.saved_tensors
+        dX, dE = aggregate_gine_backward(A, X_own, X_halo, E, _own(A, grad_output, "grad_output"),
+                                         ctx.needs_input_grad[2])
+        return None, _to_layout(A, dX), dE
+
+
 # ---- the pieces, individually callable (NCCL transport), mirroring communicate_fgm ----------------
 
 def spmm_local(plan, H_own, H_halo=None, transpose=False):
