@@ -7,6 +7,7 @@
   lib/libpgcn_transformer_edge.so csrc/transformer_edge.cu (+ transformer_math.cuh, philox.cuh, pgcn_gated.h)                         the same flags
   lib/libpgcn_gatedgcn.so csrc/gatedgcn.cu (+ gated_math.cuh, pgcn_gated.h for the walk struct)                                       the same flags
   lib/libpgcn_gine.so     csrc/gine.cu (+ gated_math.cuh, pgcn_gated.h for the walk struct)                                           the same flags
+  lib/libpgcn_rgcn.so     csrc/rgcn.cu (+ gated_math.cuh, pgcn_gated.h for the walk struct)                                           the same flags
   (the CPU oracle under oracle/ is built by oracle/build_oracle.py — test infrastructure only)
 
 nvcc cross-compiles without a GPU; `python -m <pkg>.build` or `__graft_entry__.build()` runs this.
@@ -66,6 +67,11 @@ GINE_LIB = os.path.join(LIBDIR, "libpgcn_gine.so")
 GINE_SOURCES = [os.path.join(CSRC, "gine.cu")]
 GINE_DEPS = GINE_SOURCES + [os.path.join(CSRC, "gated_math.cuh"), os.path.join(ROOT, "include", "pgcn_gine.h"),
                             os.path.join(ROOT, "include", "pgcn_gated.h"), os.path.abspath(__file__)]
+# and R-GCN's relational aggregation, which takes the same walk struct and lane loads
+RGCN_LIB = os.path.join(LIBDIR, "libpgcn_rgcn.so")
+RGCN_SOURCES = [os.path.join(CSRC, "rgcn.cu")]
+RGCN_DEPS = RGCN_SOURCES + [os.path.join(CSRC, "gated_math.cuh"), os.path.join(ROOT, "include", "pgcn_rgcn.h"),
+                            os.path.join(ROOT, "include", "pgcn_gated.h"), os.path.abspath(__file__)]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -114,6 +120,10 @@ def transformer_edge_is_stale():
 
 def gine_is_stale():
     return _stale(GINE_LIB, GINE_DEPS)
+
+
+def rgcn_is_stale():
+    return _stale(RGCN_LIB, RGCN_DEPS)
 
 
 def _compile(lib, sources, defs, verbose):
@@ -181,6 +191,13 @@ def build_gine(force=False, verbose=False):
     return _compile(GINE_LIB, GINE_SOURCES, [], verbose)
 
 
+def build_rgcn(force=False, verbose=False):
+    """Compile libpgcn_rgcn.so for sm_90a if missing or older than its sources. Returns its path."""
+    if not force and not rgcn_is_stale():
+        return RGCN_LIB
+    return _compile(RGCN_LIB, RGCN_SOURCES, [], verbose)
+
+
 if __name__ == "__main__":
     force, verbose = "--force" in sys.argv, "-v" in sys.argv
     print(build(force=force, verbose=verbose))
@@ -190,3 +207,4 @@ if __name__ == "__main__":
     print(build_gatedgcn(force=force, verbose=verbose))
     print(build_transformer_edge(force=force, verbose=verbose))
     print(build_gine(force=force, verbose=verbose))
+    print(build_rgcn(force=force, verbose=verbose))

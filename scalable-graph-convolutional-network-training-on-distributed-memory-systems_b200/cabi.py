@@ -1,10 +1,10 @@
 """ctypes binding of include/pgcn_b200.h — the C-ABI drop-in boundary (SURVEY.md §8b) — and of include/pgcn_b200_halo.h,
 include/pgcn_dropout.h, include/pgcn_gated.h, include/pgcn_transformer.h, include/pgcn_gatedgcn.h,
-include/pgcn_transformer_edge.h and include/pgcn_gine.h.
+include/pgcn_transformer_edge.h, include/pgcn_gine.h and include/pgcn_rgcn.h.
 
 Nothing here computes: it loads lib/libpgcn_b200.so (load), lib/libpgcn_dropout.so (load_dropout) and
 lib/libpgcn_gated.so (load_gated), lib/libpgcn_transformer.so (load_transformer), lib/libpgcn_gatedgcn.so
-(load_gatedgcn), lib/libpgcn_transformer_edge.so (load_transformer_edge) and lib/libpgcn_gine.so (load_gine), declares every exported symbol and turns negative status codes into RuntimeError. If the library is missing there is no fallback: the
+(load_gatedgcn), lib/libpgcn_transformer_edge.so (load_transformer_edge), lib/libpgcn_gine.so (load_gine) and lib/libpgcn_rgcn.so (load_rgcn), declares every exported symbol and turns negative status codes into RuntimeError. If the library is missing there is no fallback: the
 product path fails loudly (the CPU oracle under oracle/ is test infrastructure only).
 """
 import ctypes as C
@@ -56,6 +56,10 @@ TRANSFORMER_EDGE_SYMBOLS = ["pgcn_transformer_edge_version", "pgcn_transformer_e
 GINE_SYMBOLS = ["pgcn_gine_version", "pgcn_gine_last_error", "pgcn_gine_load", "pgcn_gine_forward",
                 "pgcn_gine_backward"]
 
+# every symbol declared in include/pgcn_rgcn.h
+RGCN_SYMBOLS = ["pgcn_rgcn_version", "pgcn_rgcn_last_error", "pgcn_rgcn_load", "pgcn_rgcn_forward",
+                "pgcn_rgcn_backward"]
+
 
 class PgcnBytes(C.Structure):
     _fields_ = [(n, C.c_int64) for n in (
@@ -78,6 +82,7 @@ _transformer = None
 _gatedgcn = None
 _transformer_edge = None
 _gine = None
+_rgcn = None
 
 
 def lib_path():
@@ -106,6 +111,10 @@ def transformer_edge_lib_path():
 
 def gine_lib_path():
     return _build.GINE_LIB
+
+
+def rgcn_lib_path():
+    return _build.RGCN_LIB
 
 
 def _built(path, stale, build, build_if_missing):
@@ -418,4 +427,35 @@ def check_gine(rc):
     if rc < 0:
         msg = load_gine().pgcn_gine_last_error()
         raise RuntimeError("pgcn_gine error %d: %s" % (rc, (msg or b"").decode("utf-8", "replace")))
+    return rc
+
+
+def load_rgcn(build_if_missing=True):
+    """Load libpgcn_rgcn.so (building it first when stale and nvcc is available)."""
+    global _rgcn
+    if _rgcn is not None:
+        return _rgcn
+    lib = C.CDLL(_built(_build.RGCN_LIB, _build.rgcn_is_stale, _build.build_rgcn, build_if_missing))
+    vp, i32, walk = C.c_void_p, C.c_int32, C.POINTER(PgcnGatedWalk)
+    lib.pgcn_rgcn_version.restype = C.c_char_p
+    lib.pgcn_rgcn_version.argtypes = []
+    lib.pgcn_rgcn_last_error.restype = C.c_char_p
+    lib.pgcn_rgcn_last_error.argtypes = []
+    lib.pgcn_rgcn_load.restype = C.c_int
+    lib.pgcn_rgcn_load.argtypes = []
+    # (walk, perm, m, h, R, X_own, X_halo, w, Z, work, f, stream)
+    lib.pgcn_rgcn_forward.restype = C.c_int
+    lib.pgcn_rgcn_forward.argtypes = [walk, vp, i32, i32, i32, vp, vp, vp, vp, vp, i32, vp]
+    # (walk, perm, m, h, R, gZ, w, dX, work, f, stream)
+    lib.pgcn_rgcn_backward.restype = C.c_int
+    lib.pgcn_rgcn_backward.argtypes = [walk, vp, i32, i32, i32, vp, vp, vp, vp, i32, vp]
+    _rgcn = lib
+    return lib
+
+
+def check_rgcn(rc):
+    """Raise RuntimeError carrying pgcn_rgcn_last_error when a libpgcn_rgcn call returned a negative status."""
+    if rc < 0:
+        msg = load_rgcn().pgcn_rgcn_last_error()
+        raise RuntimeError("pgcn_rgcn error %d: %s" % (rc, (msg or b"").decode("utf-8", "replace")))
     return rc

@@ -1223,6 +1223,117 @@ class PGINE(torch.autograd.Function):
         return None, _to_layout(A, dX), dE
 
 
+# ---- R-GCN relational aggregation (libpgcn_rgcn.so) ------------------------------------------------------------------
+
+RGCN_AGGRS = ("add", "mean")
+
+
+def _rgcn(dev, name, *args):
+    """libpgcn_rgcn.<name>(*args, stream) on `dev`'s current stream, its status checked."""
+    with torch.cuda.device(dev):
+        cabi.check_rgcn(getattr(cabi.load_rgcn(), name)(*args, _stream_ptr()))
+
+
+def rgcn_weights(plan, walks, w, aggr):
+    """The entries' fp32 weights [nnz_local] the relational kernels take, in edge_pairs() order, or None for all ones:
+    w for aggr="add", 1 / c for aggr="mean" (walks.mean, c the entries of the entry's (row, relation) pair), and the
+    fp32 product w * (1 / c) for both. w has no gradient: one that requires it is refused."""
+    from .plan import check_values
+    if aggr not in RGCN_AGGRS:
+        raise ValueError("aggr=%r: R-GCN aggregates with one of %s" % (aggr, ", ".join(map(repr, RGCN_AGGRS))))
+    if w is not None:
+        if torch.is_tensor(w) and w.requires_grad:
+            raise ValueError("w requires grad, but the relational aggregation has no gradient for its edge weights: "
+                             "pass w.detach()")
+        w = check_values(plan, w)
+    if aggr == "add":
+        return w
+    return walks.mean if w is None else w * walks.mean
+
+
+def _rgcn_prepare(plan, what):
+    """The plan bound, then the kernels loaded (pgcn_rgcn_load)."""
+    _require_bound(plan, "%s exchanges through pgcn_halo_rows" % what)
+    with torch.cuda.device(plan.device):
+        # every kernel loaded before the exchange: ranks of one process must not load one behind a waiting exchange
+        cabi.check_rgcn(cabi.load_rgcn().pgcn_rgcn_load())
+
+
+def aggregate_rgcn(plan, walks, X_own, w):
+    """(Z_own, X_halo): the per-relation aggregation over the plan's stored pattern (pgcn_rgcn_forward). With `walks`
+    = plan.relation_walks(rel, R) and for every local entry e = (i, j): Z_own[i, rel_e] += w_e X[j], over [own | halo]
+    columns, each relation's sum in forward CSR order. X_own is [m, f], Z_own [m, R, f]; w fp32 [nnz_local] in
+    edge_pairs() order or None (all ones), e.g. rgcn_weights(...). X_halo [h, f] is X's halo rows from one exchange
+    (pgcn_halo_rows), whatever R is. Needs a bound plan with f_max >= f."""
+    X_own = _check_feat(plan, X_own, plan.m, "X")
+    _rgcn_prepare(plan, "aggregate_rgcn")
+    lp, f, dev, R = plan.lp, X_own.shape[1], X_own.device, walks.R
+    X_halo = torch.empty((lp.h, f), dtype=torch.float32, device=dev)
+    _call(plan, dev, "pgcn_halo_rows", X_own.data_ptr(), X_halo.data_ptr(), f, exchange=False)
+    Z = torch.empty((lp.m, R, f), dtype=torch.float32, device=dev)
+    work = torch.empty((walks.fwd.nslots, f), dtype=torch.float32, device=dev)
+    _rgcn(dev, "pgcn_rgcn_forward", C.byref(walks.fwd.c), walks.perm_f.data_ptr(), lp.m, lp.h, R, X_own.data_ptr(),
+          X_halo.data_ptr(), _ptr(w), Z.data_ptr(), work.data_ptr(), f)
+    return Z, X_halo
+
+
+def aggregate_rgcn_backward(plan, walks, gZ_own, w):
+    """dX_own [m, f]: the gradient of aggregate_rgcn's Z_own for gZ_own [m, R, f] with the same walks and w. One column
+    walk over the transposed entries (pgcn_rgcn_backward) gives dX[j] = sum_{e in column j} w_e gZ[i_e, rel_e] for the
+    own and halo columns; the halo rows go back to their owners and are added there (pgcn_halo_rows_add)."""
+    lp, R = plan.lp, walks.R
+    _check_f32(gZ_own, "gZ")
+    if gZ_own.dim() != 3 or tuple(gZ_own.shape[:2]) != (lp.m, R):
+        raise ValueError("gZ must be [%d, %d, f], got %s" % (lp.m, R, tuple(gZ_own.shape)))
+    f, dev = gZ_own.shape[2], gZ_own.device
+    if f > plan.f_max:
+        raise ValueError("f=%d exceeds the plan's f_max=%d" % (f, plan.f_max))
+    gZ_own = gZ_own.contiguous()
+    perm = plan.transposed_entries()
+    _rgcn_prepare(plan, "aggregate_rgcn_backward")
+    dX = torch.empty((lp.m + lp.h, f), dtype=torch.float32, device=dev)
+    work = torch.empty((walks.tr.nslots, f), dtype=torch.float32, device=dev)
+    _rgcn(dev, "pgcn_rgcn_backward", C.byref(walks.tr.c), perm.data_ptr(), lp.m, lp.h, R, gZ_own.data_ptr(), _ptr(w),
+          dX.data_ptr(), work.data_ptr(), f)
+    _call(plan, dev, "pgcn_halo_rows_add", dX[lp.m:].data_ptr(), dX.data_ptr(), f, exchange=True)
+    return dX[:lp.m]
+
+
+class PRGCN(torch.autograd.Function):
+    """R-GCN's relational aggregation over the plan's stored pattern (Schlichtkrull et al.; the message of PyG's
+    RGCNConv and DGL's RelGraphConv, before the per-relation weights, which the layer applies):
+
+        Z = PRGCN.apply(A, X, rel, R, w=None, aggr="mean")
+        Z[i, r] = sum over the stored entries e = (i, j) with rel_e = r of  w_e X[j]          (element-wise, f features)
+
+    X is [rows, f] and Z [rows, R, f], fp32 CUDA tensors (rows = m in the "local" layout, n in the "global" one, as
+    PSpMM). rel is an integer tensor [nnz_local] of relations in [0, R), w None (every weight 1) or fp32 [nnz_local],
+    both in the order of PgcnPlan.edge_pairs() in both layouts. aggr="add" takes w_e as given; aggr="mean" (PyG's
+    default) multiplies it by 1 / c, c the number of entries of the entry's (row, relation) pair. The values of A are
+    not read; every stored entry contributes, duplicates included; a (row, relation) pair without entries gives zeros.
+    One exchange per layer carries X (f floats per row, whatever R is), so the plan's f_max must be at least f; the
+    backward returns the halo rows' partial dX to their owners in one reverse exchange. Nothing is saved for the
+    backward but the weights. The gradient goes to X only: a w that requires grad is refused. Deterministic. The
+    exchanges are the unsplit ones (no per-source overlap). The plan must be bound (PgcnPlan.bind_values); the first
+    call with a rel tensor builds its tables (PgcnPlan.relation_walks)."""
+
+    @staticmethod
+    def forward(ctx, A, X, rel, R, w=None, aggr="mean"):
+        walks = A.relation_walks(rel, R)
+        weights = rgcn_weights(A, walks, w, aggr)
+        Z, _ = aggregate_rgcn(A, walks, _own(A, X, "X"), weights)
+        ctx.plan, ctx.walks = A, walks
+        ctx.save_for_backward(weights)
+        return _to_layout(A, Z)
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        A, walks = ctx.plan, ctx.walks
+        (weights,) = ctx.saved_tensors
+        dX = aggregate_rgcn_backward(A, walks, _owned(A, grad_output), weights)
+        return None, _to_layout(A, dX), None, None, None, None
+
+
 # ---- the pieces, individually callable (NCCL transport), mirroring communicate_fgm ----------------
 
 def spmm_local(plan, H_own, H_halo=None, transpose=False):

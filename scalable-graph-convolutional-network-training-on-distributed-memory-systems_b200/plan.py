@@ -13,6 +13,7 @@ n x n COO with global indices (:53-64). Here the same information is produced wi
   * `PgcnPlan`: owns the device-side plan (C-ABI handle) and the host stats the reference keeps in
     device counters (GPU/PGCN.py:78-83).
 """
+import collections
 import ctypes as C
 
 import numpy as np
@@ -241,6 +242,7 @@ class PgcnPlan:
         self._gated_walks = None
         self._global_ids = None
         self._transposed_entries = None
+        self._relation_walks = {}        # (_values_key(rel), R) -> (rel, walks): relation_walks' tables per rel and R
         # edge values (bind_values / set_values): which values the records hold, as far as this process knows
         self._bound = False
         self._resident = "creation"      # "creation", a key of the tensor set last, or None: unknown
@@ -439,6 +441,68 @@ class PgcnPlan:
             self._transposed_entries = torch.from_numpy(perm.astype(np.int32)).to(self.device)
         return self._transposed_entries
 
+    def relation_walks(self, rel, R):
+        """RelationWalks (fwd, tr, perm_f, mean, R): the walks of the relational aggregation (op.PRGCN,
+        include/pgcn_rgcn.h) for the relation types `rel` (an integer tensor [nnz_local] in edge_pairs() order, values
+        in [0, R)), numbering the output rows v = i R + r for row i and relation r:
+
+          perm_f  CUDA int32 [nnz]: the forward entries sorted stably by (row, relation), so a virtual row keeps its
+                  entries in forward CSR order; perm_f[e] is the forward entry of sorted entry e
+          fwd     GatedWalk over the m R virtual rows with idx = colidx[perm_f]
+          tr      GatedWalk over the transposed CSR (m + h columns) with idx = t_colidx R + rel[perm_t], perm_t =
+                  transposed_entries()
+          mean    CUDA fp32 [nnz] in forward entry order: 1 / c, the fp32 quotient, c the number of entries of the
+                  entry's (row, relation) pair (aggr="mean")
+
+        Built on the host on first use and kept per rel tensor (its identity and version, as the edge values are) and
+        R; the tables take about 16 B per entry and 16 B per virtual row. Building them copies to the device, which a
+        CUDA graph cannot capture: call it, or the operator once eagerly, before capturing a step that uses it."""
+        import operator
+        import torch
+        if isinstance(R, bool):
+            raise TypeError("R must be an integer, got %r" % (R,))
+        R = operator.index(R)
+        if not torch.is_tensor(rel):
+            raise TypeError("rel must be an integer tensor, got %s" % type(rel).__name__)
+        key = (_values_key(rel), R)
+        hit = self._relation_walks.get(key)
+        if hit is not None and hit[0] is rel:
+            return hit[1]
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("PgcnPlan.relation_walks is built by host-to-device copies, which a CUDA-graph capture "
+                               "cannot hold: call plan.relation_walks(rel, R) once before the capture")
+        lp = self.lp
+        if rel.dtype.is_floating_point or rel.dtype.is_complex or rel.dtype == torch.bool:
+            raise TypeError("rel must be an integer tensor, got %s" % rel.dtype)
+        nnz = lp.nnz()
+        if rel.dim() != 1 or rel.shape[0] != nnz:
+            raise ValueError("rel must be [%d] (the plan's local entries, edge_pairs() order), got %s" % (
+                nnz, tuple(rel.shape)))
+        if R < 1:
+            raise ValueError("R=%d: need at least one relation" % R)
+        if lp.m * R > np.iinfo(np.int32).max:
+            raise ValueError("m R = %d * %d virtual rows exceed 2^31 - 1" % (lp.m, R))
+        r = rel.detach().cpu().numpy().astype(np.int64)
+        if nnz and (r.min() < 0 or r.max() >= R):
+            bad = int(r.min() if r.min() < 0 else r.max())
+            raise ValueError("rel holds relation %d, outside [0, R) = [0, %d)" % (bad, R))
+        chunk = cabi.load_gated().pgcn_gated_chunk()
+        rows = np.repeat(np.arange(lp.m, dtype=np.int64), np.diff(lp.rowptr.astype(np.int64)))
+        vrow = rows * R + r
+        perm_f = np.argsort(vrow, kind="stable")
+        count = np.bincount(vrow, minlength=lp.m * R)
+        vptr = np.concatenate([[0], np.cumsum(count)])
+        perm_t = self.transposed_entries().cpu().numpy().astype(np.int64)
+        mean = np.float32(1.0) / count[vrow].astype(np.float32)
+        walks = RelationWalks(GatedWalk(vptr, lp.colidx[perm_f], chunk, self.device),
+                              GatedWalk(lp.t_rowptr, lp.t_colidx.astype(np.int64) * R + r[perm_t], chunk, self.device),
+                              torch.from_numpy(perm_f.astype(np.int32)).to(self.device),
+                              torch.from_numpy(mean).to(self.device), R)
+        # a rel tensor changed in place leaves its old tables behind: drop them
+        self._relation_walks = {k: v for k, v in self._relation_walks.items() if v[0] is not rel}
+        self._relation_walks[key] = (rel, walks)
+        return walks
+
     def algorithmic_bytes(self, f):
         b = cabi.PgcnBytes()
         cabi.check(self._lib.pgcn_algorithmic_bytes(self.handle, int(f), C.byref(b)), self._h)
@@ -556,6 +620,10 @@ class GatedWalk:
         self.splits = torch.from_numpy(splits).to(device)
         self.c = cabi.PgcnGatedWalk(self.idx.data_ptr(), self.items.data_ptr(), self.splits.data_ptr(), self.rows,
                                     len(items), len(splits), self.nslots)
+
+
+# The tables of the relational aggregation (PgcnPlan.relation_walks): two GatedWalks, perm_f, the mean weights and R.
+RelationWalks = collections.namedtuple("RelationWalks", "fwd tr perm_f mean R")
 
 
 def _values_key(vals):
