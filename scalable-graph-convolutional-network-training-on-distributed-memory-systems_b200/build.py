@@ -8,6 +8,7 @@
   lib/libpgcn_gatedgcn.so csrc/gatedgcn.cu (+ gated_math.cuh, pgcn_gated.h for the walk struct)                                       the same flags
   lib/libpgcn_gine.so     csrc/gine.cu (+ gated_math.cuh, pgcn_gated.h for the walk struct)                                           the same flags
   lib/libpgcn_rgcn.so     csrc/rgcn.cu (+ gated_math.cuh, pgcn_gated.h for the walk struct)                                           the same flags
+  lib/libpgcn_gatv2_edge.so csrc/gatv2_edge.cu (+ transformer_math.cuh, philox.cuh, pgcn_gated.h)                                     the same flags
   (the CPU oracle under oracle/ is built by oracle/build_oracle.py — test infrastructure only)
 
 nvcc cross-compiles without a GPU; `python -m <pkg>.build` or `__graft_entry__.build()` runs this.
@@ -72,6 +73,12 @@ RGCN_LIB = os.path.join(LIBDIR, "libpgcn_rgcn.so")
 RGCN_SOURCES = [os.path.join(CSRC, "rgcn.cu")]
 RGCN_DEPS = RGCN_SOURCES + [os.path.join(CSRC, "gated_math.cuh"), os.path.join(ROOT, "include", "pgcn_rgcn.h"),
                             os.path.join(ROOT, "include", "pgcn_gated.h"), os.path.abspath(__file__)]
+# and GATv2 with edge features, which takes the transformer's lane math (transformer_math.cuh) and the same walk struct
+GATV2_EDGE_LIB = os.path.join(LIBDIR, "libpgcn_gatv2_edge.so")
+GATV2_EDGE_SOURCES = [os.path.join(CSRC, "gatv2_edge.cu")]
+GATV2_EDGE_DEPS = GATV2_EDGE_SOURCES + [os.path.join(CSRC, "transformer_math.cuh"), os.path.join(CSRC, "philox.cuh"),
+                                        os.path.join(ROOT, "include", "pgcn_gatv2_edge.h"),
+                                        os.path.join(ROOT, "include", "pgcn_gated.h"), os.path.abspath(__file__)]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -124,6 +131,10 @@ def gine_is_stale():
 
 def rgcn_is_stale():
     return _stale(RGCN_LIB, RGCN_DEPS)
+
+
+def gatv2_edge_is_stale():
+    return _stale(GATV2_EDGE_LIB, GATV2_EDGE_DEPS)
 
 
 def _compile(lib, sources, defs, verbose):
@@ -198,6 +209,13 @@ def build_rgcn(force=False, verbose=False):
     return _compile(RGCN_LIB, RGCN_SOURCES, [], verbose)
 
 
+def build_gatv2_edge(force=False, verbose=False):
+    """Compile libpgcn_gatv2_edge.so for sm_90a if missing or older than its sources. Returns its path."""
+    if not force and not gatv2_edge_is_stale():
+        return GATV2_EDGE_LIB
+    return _compile(GATV2_EDGE_LIB, GATV2_EDGE_SOURCES, [], verbose)
+
+
 if __name__ == "__main__":
     force, verbose = "--force" in sys.argv, "-v" in sys.argv
     print(build(force=force, verbose=verbose))
@@ -208,3 +226,4 @@ if __name__ == "__main__":
     print(build_transformer_edge(force=force, verbose=verbose))
     print(build_gine(force=force, verbose=verbose))
     print(build_rgcn(force=force, verbose=verbose))
+    print(build_gatv2_edge(force=force, verbose=verbose))

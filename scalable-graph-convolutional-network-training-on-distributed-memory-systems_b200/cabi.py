@@ -60,6 +60,11 @@ GINE_SYMBOLS = ["pgcn_gine_version", "pgcn_gine_last_error", "pgcn_gine_load", "
 RGCN_SYMBOLS = ["pgcn_rgcn_version", "pgcn_rgcn_last_error", "pgcn_rgcn_load", "pgcn_rgcn_forward",
                 "pgcn_rgcn_backward"]
 
+# every symbol declared in include/pgcn_gatv2_edge.h
+GATV2_EDGE_SYMBOLS = ["pgcn_gatv2_edge_version", "pgcn_gatv2_edge_last_error", "pgcn_gatv2_edge_work_rows",
+                      "pgcn_gatv2_edge_load", "pgcn_gatv2_edge_forward", "pgcn_gatv2_edge_backward_rows",
+                      "pgcn_gatv2_edge_backward_cols"]
+
 
 class PgcnBytes(C.Structure):
     _fields_ = [(n, C.c_int64) for n in (
@@ -83,6 +88,7 @@ _gatedgcn = None
 _transformer_edge = None
 _gine = None
 _rgcn = None
+_gatv2_edge = None
 
 
 def lib_path():
@@ -115,6 +121,10 @@ def gine_lib_path():
 
 def rgcn_lib_path():
     return _build.RGCN_LIB
+
+
+def gatv2_edge_lib_path():
+    return _build.GATV2_EDGE_LIB
 
 
 def _built(path, stale, build, build_if_missing):
@@ -458,4 +468,43 @@ def check_rgcn(rc):
     if rc < 0:
         msg = load_rgcn().pgcn_rgcn_last_error()
         raise RuntimeError("pgcn_rgcn error %d: %s" % (rc, (msg or b"").decode("utf-8", "replace")))
+    return rc
+
+
+def load_gatv2_edge(build_if_missing=True):
+    """Load libpgcn_gatv2_edge.so (building it first when stale and nvcc is available)."""
+    global _gatv2_edge
+    if _gatv2_edge is not None:
+        return _gatv2_edge
+    lib = C.CDLL(_built(_build.GATV2_EDGE_LIB, _build.gatv2_edge_is_stale, _build.build_gatv2_edge, build_if_missing))
+    vp, i32, u32, f32, walk = C.c_void_p, C.c_int32, C.c_uint32, C.c_float, C.POINTER(PgcnGatedWalk)
+    lib.pgcn_gatv2_edge_version.restype = C.c_char_p
+    lib.pgcn_gatv2_edge_version.argtypes = []
+    lib.pgcn_gatv2_edge_last_error.restype = C.c_char_p
+    lib.pgcn_gatv2_edge_last_error.argtypes = []
+    lib.pgcn_gatv2_edge_work_rows.restype = C.c_int64
+    lib.pgcn_gatv2_edge_work_rows.argtypes = [walk]
+    lib.pgcn_gatv2_edge_load.restype = C.c_int
+    lib.pgcn_gatv2_edge_load.argtypes = []
+    # (walk, m, h, heads, XL_own, XL_halo, XR, att, E, negative_slope, gid, drop, threshold, keep_scale, ...)
+    head = [walk, i32, i32, i32, vp, vp, vp, vp, vp, f32, vp, vp, u32, f32]
+    # (..., Z, L, work, f, stream)
+    lib.pgcn_gatv2_edge_forward.restype = C.c_int
+    lib.pgcn_gatv2_edge_forward.argtypes = head + [vp, vp, vp, i32, vp]
+    # (..., gZ, Z, L, dXR, D, PS, G, datt, work, f, stream)
+    lib.pgcn_gatv2_edge_backward_rows.restype = C.c_int
+    lib.pgcn_gatv2_edge_backward_rows.argtypes = head + [vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp]
+    # (walk, perm, m, h, heads, gZ, PS, G, dXL, work, f, stream)
+    lib.pgcn_gatv2_edge_backward_cols.restype = C.c_int
+    lib.pgcn_gatv2_edge_backward_cols.argtypes = [walk, vp, i32, i32, i32, vp, vp, vp, vp, vp, i32, vp]
+    _gatv2_edge = lib
+    return lib
+
+
+def check_gatv2_edge(rc):
+    """Raise RuntimeError carrying pgcn_gatv2_edge_last_error when a libpgcn_gatv2_edge call returned a negative
+    status."""
+    if rc < 0:
+        msg = load_gatv2_edge().pgcn_gatv2_edge_last_error()
+        raise RuntimeError("pgcn_gatv2_edge error %d: %s" % (rc, (msg or b"").decode("utf-8", "replace")))
     return rc

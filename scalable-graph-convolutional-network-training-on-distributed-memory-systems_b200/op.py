@@ -1334,6 +1334,174 @@ class PRGCN(torch.autograd.Function):
         return None, _to_layout(A, dX), None, None, None, None
 
 
+# ---- GATv2 attention with edge features (libpgcn_gatv2_edge.so) -----------------------------------------------------
+
+GATV2_EDGE_MAX_F = 256
+
+
+def _gatv2_edge(dev, name, *args):
+    """libpgcn_gatv2_edge.<name>(*args, stream) on `dev`'s current stream, its status checked."""
+    with torch.cuda.device(dev):
+        cabi.check_gatv2_edge(getattr(cabi.load_gatv2_edge(), name)(*args, _stream_ptr()))
+
+
+def _gatv2_att(att, f):
+    """att checked as PGATv2Attention checks it ([K, f / K], K in HEADS, fp32 CUDA): (its heads, att detached and
+    contiguous)."""
+    if att.dim() != 2:
+        raise ValueError("att must be [heads, f / heads], got %s" % (tuple(att.shape),))
+    K = att.shape[0]
+    if K not in HEADS:
+        raise ValueError("heads=%d: the GATv2 kernels take 1, 2, 4 or 8 heads" % K)
+    if f % K:
+        raise ValueError("f=%d is not a multiple of heads=%d" % (f, K))
+    if tuple(att.shape) != (K, f // K):
+        raise ValueError("att must be [%d, %d], got %s" % (K, f // K, tuple(att.shape)))
+    if not att.is_cuda or att.dtype != torch.float32:
+        raise TypeError("att must be a float32 CUDA tensor")
+    return K, att.detach().contiguous()
+
+
+def _gatv2_edge_operands(plan, XL_own, XR_own, att, E, drop, what):
+    """The walks, the transposed entries and the global ids, then XL_own and XR_own ([m, f] each, f <= 256 and
+    f <= f_max), att ([K, f / K]) and E ([nnz_local, f]) checked and the plan bound, then the kernels loaded
+    (pgcn_gatv2_edge_load). The tables come first, so that a capture that needs them before they exist is refused
+    before any work is enqueued."""
+    walks = plan.gated_walks()
+    perm = plan.transposed_entries()
+    gid = plan.global_ids()
+    if drop is not None and drop.state.device != plan.device:
+        raise ValueError("the EdgeDropout state lives on %s, the plan on %s" % (drop.state.device, plan.device))
+    XL_own = _check_feat(plan, XL_own, plan.m, "XL")
+    XR_own = _check_feat(plan, XR_own, plan.m, "XR")
+    f = XL_own.shape[1]
+    if XR_own.shape[1] != f:
+        raise ValueError("XL and XR must have the same width, got %d and %d" % (f, XR_own.shape[1]))
+    if f > GATV2_EDGE_MAX_F:
+        raise ValueError("f=%d: the GATv2 edge kernels hold a row in registers, f <= %d" % (f, GATV2_EDGE_MAX_F))
+    K, att = _gatv2_att(att, f)
+    E = _check_edges(plan, E, f, "E")
+    _require_bound(plan, "%s exchanges XL through pgcn_halo_rows" % what)
+    with torch.cuda.device(plan.device):
+        # every kernel loaded before the exchange: ranks of one process must not load one behind a waiting exchange
+        cabi.check_gatv2_edge(cabi.load_gatv2_edge().pgcn_gatv2_edge_load())
+    return walks, perm, gid, XL_own, XR_own, K, att, E
+
+
+def aggregate_gatv2_edge(plan, XL_own, XR_own, att, E, negative_slope=0.2, drop=None):
+    """(Z_own, L, XL_halo, snap): GATv2 attention with an edge term in the score over the plan's stored pattern
+    (pgcn_gatv2_edge_forward). For every local entry e = (i, j), K = att.shape[0] heads of width d = f / K:
+    t_e = (XR[i] + XL[j]) + E_e, s_eh = sum_c att[h, c] LeakyReLU(t_e[h d + c]), p = softmax of s over each row's stored
+    entries per head, Z_own[i, h] = sum_e M_eh p_eh XL[j, h]. XL_own, XR_own and Z_own are [m, f], E [nnz_local, f] in
+    edge_pairs() order, L [m, K] the rows' log-sum-exp. XL_halo [h, f] is XL's halo rows from one exchange
+    (pgcn_halo_rows). drop (an EdgeDropout) with p > 0 draws a new counter (its snapshot `snap`, else None) and applies
+    the mask M; aggregate_gatv2_edge_backward takes the same snapshot. E never crosses ranks. Needs a bound plan with
+    f_max >= f."""
+    drop = _active(drop)
+    (fwd, _), _, gid, XL_own, XR_own, K, att, E = _gatv2_edge_operands(plan, XL_own, XR_own, att, E, drop,
+                                                                       "aggregate_gatv2_edge")
+    lp, f, dev = plan.lp, XL_own.shape[1], XL_own.device
+    snap = drop.draw() if drop else None
+    XL_halo = torch.empty((lp.h, f), dtype=torch.float32, device=dev)
+    _call(plan, dev, "pgcn_halo_rows", XL_own.data_ptr(), XL_halo.data_ptr(), f, exchange=False)
+    Z = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+    L = torch.empty((lp.m, K), dtype=torch.float32, device=dev)
+    work = torch.empty((fwd.nslots, f + 2 * K), dtype=torch.float32, device=dev)
+    _gatv2_edge(dev, "pgcn_gatv2_edge_forward", C.byref(fwd.c), lp.m, lp.h, K, XL_own.data_ptr(), XL_halo.data_ptr(),
+                XR_own.data_ptr(), att.data_ptr(), E.data_ptr(), float(negative_slope), gid.data_ptr(),
+                *_drop_args(drop, snap), Z.data_ptr(), L.data_ptr(), work.data_ptr(), f)
+    return Z, L, XL_halo, snap
+
+
+def aggregate_gatv2_edge_backward(plan, XL_own, XL_halo, XR_own, att, E, Z_own, L, gZ_own, negative_slope=0.2,
+                                  drop=None, snap=None, need_dE=True):
+    """(dXL, dXR, datt, dE): the gradients of aggregate_gatv2_edge's Z_own for the output gradient gZ_own [m, f], from
+    the same XL_own, XR_own, att, E and negative_slope, its XL_halo, Z_own and L and, with dropout, the same `drop` and
+    its forward's `snap`. The row walk (pgcn_gatv2_edge_backward_rows) gives dXR, datt ([K, f / K]), each entry's
+    g ([nnz_local, f], which is dE; None is returned when need_dE is false, and the buffer is scratch) and [P | ds]
+    ([nnz_local, 2K]); the column walk over the transposed entries (pgcn_gatv2_edge_backward_cols) reads those and gives
+    dXL, whose halo rows go back to their owners and are added there (pgcn_halo_rows_add)."""
+    drop = _active(drop)
+    if drop is not None and snap is None:
+        raise ValueError("aggregate_gatv2_edge_backward with dropout needs the forward's snapshot")
+    (fwd, tr), perm, gid, XL_own, XR_own, K, att, E = _gatv2_edge_operands(
+        plan, XL_own, XR_own, att, E, drop, "aggregate_gatv2_edge_backward")
+    lp, f, dev = plan.lp, XL_own.shape[1], XL_own.device
+    gZ_own = _check_feat(plan, gZ_own, plan.m, "gZ")
+    Z_own = _check_feat(plan, Z_own, plan.m, "Z")
+    if gZ_own.shape[1] != f or Z_own.shape[1] != f:
+        raise ValueError("XL, Z and gZ must have the same width, got %d, %d and %d" % (f, Z_own.shape[1],
+                                                                                      gZ_own.shape[1]))
+    XL_halo, L = XL_halo.contiguous(), L.contiguous()
+    if tuple(XL_halo.shape) != (lp.h, f):
+        raise ValueError("XL_halo must be [%d, %d], got %s" % (lp.h, f, tuple(XL_halo.shape)))
+    if tuple(L.shape) != (lp.m, K):
+        raise ValueError("L must be [%d, %d], got %s" % (lp.m, K, tuple(L.shape)))
+    dXR = torch.empty((lp.m, f), dtype=torch.float32, device=dev)
+    D = torch.empty((lp.m, K), dtype=torch.float32, device=dev)
+    PS = torch.empty((lp.nnz(), 2 * K), dtype=torch.float32, device=dev)
+    G = torch.empty((lp.nnz(), f), dtype=torch.float32, device=dev)
+    datt = torch.empty((K, f // K), dtype=torch.float32, device=dev)
+    work = torch.empty((cabi.load_gatv2_edge().pgcn_gatv2_edge_work_rows(C.byref(fwd.c)), f), dtype=torch.float32,
+                       device=dev)
+    _gatv2_edge(dev, "pgcn_gatv2_edge_backward_rows", C.byref(fwd.c), lp.m, lp.h, K, XL_own.data_ptr(),
+                XL_halo.data_ptr(), XR_own.data_ptr(), att.data_ptr(), E.data_ptr(), float(negative_slope),
+                gid.data_ptr(), *_drop_args(drop, snap), gZ_own.data_ptr(), Z_own.data_ptr(), L.data_ptr(),
+                dXR.data_ptr(), D.data_ptr(), PS.data_ptr(), G.data_ptr(), datt.data_ptr(), work.data_ptr(), f)
+    dXL = torch.empty((lp.m + lp.h, f), dtype=torch.float32, device=dev)
+    work = torch.empty((tr.nslots, f), dtype=torch.float32, device=dev)
+    _gatv2_edge(dev, "pgcn_gatv2_edge_backward_cols", C.byref(tr.c), perm.data_ptr(), lp.m, lp.h, K,
+                gZ_own.data_ptr(), PS.data_ptr(), G.data_ptr(), dXL.data_ptr(), work.data_ptr(), f)
+    _call(plan, dev, "pgcn_halo_rows_add", dXL[lp.m:].data_ptr(), dXL.data_ptr(), f, exchange=True)
+    return dXL[:lp.m], dXR, datt, G if need_dE else None
+
+
+class PGATv2EdgeAttention(torch.autograd.Function):
+    """PGATv2Attention with edge features in the score and attention dropout, the attention of PyG's
+    GATv2Conv(edge_dim=..., dropout=p, concat=True, bias=False, add_self_loops=False) with XL = lin_l(x),
+    XR = lin_r(x) and E = lin_edge(edge_attr) formed by the caller:
+
+        PGATv2EdgeAttention.apply(A, XL, XR, att, E, negative_slope=0.2, dropout=None)
+        t_e = (XR[i] + XL[j]) + E_e,  s_eh = sum_c att[h, c] * LeakyReLU(t_e[h d + c]),
+        p_.h = softmax of s_.h over row i's stored entries,  out[i, h] = sum over the stored entries e = (i, j) of
+        M_eh p_eh XL[j, h]
+
+    XL, XR, att and out as PGATv2Attention's (K = att.shape[0] heads of width d = f / K, [rows, f] in the plan's layout;
+    f <= 256). E is [nnz_local, f] in both layouts: one row per local entry in the order of PgcnPlan.edge_pairs(). It
+    enters the score only and never crosses ranks, since every entry belongs to the rank that owns its row. Passing one
+    tensor as XL and XR is share_weights=True. The values of A are not read; every stored entry contributes, duplicates
+    included; a row without entries gives 0. One exchange per layer carries XL (f floats per row, so f_max >= f); the
+    backward returns the halo rows' partial dXL to their owners in one reverse exchange. Only the rows' log-sum-exp
+    ([rows, K]) is kept besides the operands: the backward recomputes the probabilities. Gradients go to XL, XR, att and
+    E; dE is returned only when E requires it. Deterministic. The plan must be bound (PgcnPlan.bind_values); the first
+    call builds its index tables (PgcnPlan.gated_walks, PgcnPlan.transposed_entries, PgcnPlan.global_ids).
+
+    dropout (an op.EdgeDropout with p > 0): attention dropout on every head, the mask of op.edge_dropout drawn inline
+    from the global (row, column) of each entry, as PTransformerAttention's. None or p == 0: no mask is drawn."""
+
+    @staticmethod
+    def forward(ctx, A, XL, XR, att, E, negative_slope=0.2, dropout=None):
+        drop = _active(dropout)
+        A.gated_walks()
+        A.transposed_entries()
+        A.global_ids()
+        XL_own = _own(A, XL, "XL")
+        XR_own = _own(A, XR, "XR")
+        Z, L, XL_halo, snap = aggregate_gatv2_edge(A, XL_own, XR_own, att, E, negative_slope, drop)
+        ctx.plan, ctx.slope, ctx.drop = A, float(negative_slope), drop
+        ctx.save_for_backward(XL_own, XL_halo, XR_own, att.detach(), E.detach().contiguous(), Z, L, snap)
+        return _to_layout(A, Z)
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        A = ctx.plan
+        XL_own, XL_halo, XR_own, att, E, Z, L, snap = ctx.saved_tensors
+        dXL, dXR, datt, dE = aggregate_gatv2_edge_backward(A, XL_own, XL_halo, XR_own, att, E, Z, L,
+                                                           _own(A, grad_output, "grad_output"), ctx.slope, ctx.drop,
+                                                           snap, ctx.needs_input_grad[4])
+        return None, _to_layout(A, dXL), _to_layout(A, dXR), datt, dE, None, None
+
+
 # ---- the pieces, individually callable (NCCL transport), mirroring communicate_fgm ----------------
 
 def spmm_local(plan, H_own, H_halo=None, transpose=False):

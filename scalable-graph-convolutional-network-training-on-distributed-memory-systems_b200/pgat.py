@@ -24,18 +24,26 @@ er[:, h] = Z_h a[d:, h] for head h's slice Z_h of Z (op.PGATMultiHeadAttention).
 of every layer while training (op.EdgeDropout, the GAT paper's recipe uses 0.6). The mask is a function of the global
 edge, so any partition trains the same model. Layer l draws with key seed * 2^16 + l (seed 0 when --seed is absent) and
 call counter epoch + 1; nothing is drawn from torch's generator, so the parameters are those of a run without the flag.
-Not taken with --v2.
+Taken with --v2 only together with --edge-values (below).
 
 --v2: GATv2 layers instead (dynamic attention, op.PGATv2Attention), with --heads K as above. Per layer lin_l and lin_r
 (Linear(f, f, bias=False)) and att (K x d), drawn in that order, each xavier_normal with the relu gain; the layer is
 PyG GATv2Conv(share_weights=False, concat=True, bias=False, add_self_loops=False) over the stored pattern.
+
+--v2 --edge-values: GATv2Conv with edge_dim = 1, the edge input being each stored entry's fp32 value of A (the plan's
+lp.vals, in the order of PgcnPlan.edge_pairs()) as [nnz, 1]. Each layer then also has lin_edge = Linear(1, f,
+bias=False) with torch's default initialisation, drawn after lin_l, lin_r and att, and
+    E = lin_edge(vals),  out = PGATv2EdgeAttention(A, lin_l(H), lin_r(H), att, E)    score of (XR[i] + XL[j]) + E_e
+The edge input stays on the rank that owns its row. Without the flag the layers and their parameter draws are as above.
+--attn-dropout P is taken with --v2 only together with --edge-values (the edge kernels draw the mask; the GATv2 kernels
+without edges do not), with the keys and counters above. --edge-values without --v2 is refused.
 """
 import sys
 
 import torch
 import torch.nn as nn
 
-from .op import HEADS, EdgeDropout, PGATAttention, PGATMultiHeadAttention, PGATv2Attention
+from .op import HEADS, EdgeDropout, PGATAttention, PGATMultiHeadAttention, PGATv2Attention, PGATv2EdgeAttention
 from .pgcn import launch, parse_args, train
 
 
@@ -77,16 +85,27 @@ class PGAT(nn.Module):
 
 
 class PGATv2(nn.Module):
-    """GATv2 layer f -> f with K heads: out = PGATv2Attention(A, lin_l(H), lin_r(H), att)."""
+    """GATv2 layer f -> f with K heads: out = PGATv2Attention(A, lin_l(H), lin_r(H), att). edge_values: the values of A,
+    through lin_edge = Linear(1, out_features, bias=False) (drawn after the other parameters), are the edge features of
+    every entry, and out = PGATv2EdgeAttention(A, lin_l(H), lin_r(H), att, lin_edge(vals)). attn_dropout (an
+    op.EdgeDropout or None) drops attention coefficients while the module is training; it needs edge_values."""
 
-    def __init__(self, A, in_features, out_features, negative_slope=0.2, heads=1):
+    def __init__(self, A, in_features, out_features, negative_slope=0.2, heads=1, edge_values=False,
+                 attn_dropout=None):
         super().__init__()
+        if attn_dropout is not None and not edge_values:
+            raise ValueError("GATv2 attention dropout is drawn by the edge-feature kernels: it needs edge_values=True")
         self.A = A
         self.negative_slope = negative_slope
+        self.attn_dropout = attn_dropout
         self.lin_l = nn.Linear(in_features, out_features, bias=False)
         self.lin_r = nn.Linear(in_features, out_features, bias=False)
         self.att = nn.Parameter(torch.empty(size=(heads, out_features // heads)))
         self.reset_parameters()
+        self.lin_edge = nn.Linear(1, out_features, bias=False) if edge_values else None
+        if edge_values:
+            self.register_buffer("edge_input", torch.from_numpy(A.lp.vals.astype("float32")).reshape(-1, 1),
+                                 persistent=False)
 
     def reset_parameters(self):
         gain = nn.init.calculate_gain("relu")
@@ -95,7 +114,11 @@ class PGATv2(nn.Module):
         nn.init.xavier_normal_(self.att, gain=gain)
 
     def forward(self, H):
-        return PGATv2Attention.apply(self.A, self.lin_l(H), self.lin_r(H), self.att, self.negative_slope)
+        if self.lin_edge is None:
+            return PGATv2Attention.apply(self.A, self.lin_l(H), self.lin_r(H), self.att, self.negative_slope)
+        drop = self.attn_dropout if self.training else None
+        return PGATv2EdgeAttention.apply(self.A, self.lin_l(H), self.lin_r(H), self.att,
+                                         self.lin_edge(self.edge_input), self.negative_slope, drop)
 
 
 def dropout_key(seed, layer):
@@ -104,23 +127,23 @@ def dropout_key(seed, layer):
 
 
 def run(rank, size, nlayers, nfeatures, path_A, path_partvec, backend, transport="auto", out=sys.stdout, seed=None,
-        negative_slope=1.0, epochs=50, heads=1, v2=False, attn_dropout=0.0):
+        negative_slope=1.0, epochs=50, heads=1, v2=False, attn_dropout=0.0, edge_values=False):
     # the multi-head backward gets d_er from an aggregation of width 4 K (PGATMultiHeadAttention)
     f_max = nfeatures if heads == 1 or v2 else max(nfeatures, 4 * heads)
-    if v2:
-        make = lambda plan: PGATv2(plan, nfeatures, nfeatures, negative_slope, heads)
-    else:
-        index = iter(range(nlayers))      # train builds the layers in order
+    index = iter(range(nlayers))          # train builds the layers in order
 
-        def make(plan):
-            drop = EdgeDropout(attn_dropout, dropout_key(seed, next(index)), plan.device) if attn_dropout > 0 else None
-            return PGAT(plan, nfeatures, nfeatures, negative_slope, heads, drop)
+    def make(plan):
+        drop = EdgeDropout(attn_dropout, dropout_key(seed, next(index)), plan.device) if attn_dropout > 0 else None
+        if v2:
+            return PGATv2(plan, nfeatures, nfeatures, negative_slope, heads, edge_values, drop)
+        return PGAT(plan, nfeatures, nfeatures, negative_slope, heads, drop)
     return train(rank, size, nlayers, nfeatures, path_A, path_partvec, backend, "PGAT", make, f_max, True,
                  transport=transport, out=out, seed=seed, epochs=epochs)
 
 
 USAGE = ("usage: PGAT.py -a <A.mtx> -p <partvec> -b nccl -s <nparts> -l <nlayers> -f <nfeatures> "
-         "[--seed N] [--negative-slope S] [--heads 1|2|4|8, dividing nfeatures] [--attn-dropout P, 0 <= P < 1] [--v2]")
+         "[--seed N] [--negative-slope S] [--heads 1|2|4|8, dividing nfeatures] [--attn-dropout P, 0 <= P < 1] [--v2] "
+         "[--edge-values, with --v2; --attn-dropout with --v2 needs it]")
 
 
 def _heads(arg):
@@ -134,12 +157,13 @@ def _valid(size, nlayers, nfeatures, kw):
     heads = kw.get("heads", 1)
     p = kw.get("attn_dropout", 0.0)
     return (heads in HEADS and nfeatures % heads == 0 and 0.0 <= p < 1.0
-            and not ("attn_dropout" in kw and kw.get("v2")))
+            and not ("attn_dropout" in kw and kw.get("v2") and not kw.get("edge_values"))
+            and not (kw.get("edge_values") and not kw.get("v2")))
 
 
 def main(argv):
     options = {"--negative-slope": ("negative_slope", float), "--heads": ("heads", _heads), "--v2": ("v2", None),
-               "--attn-dropout": ("attn_dropout", float)}
+               "--attn-dropout": ("attn_dropout", float), "--edge-values": ("edge_values", None)}
     launch(run, *parse_args(argv, USAGE, options, _valid))
 
 
